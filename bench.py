@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- images/sec of the hot path on B200, BASELINE.json's metric.
+"""bench.py -- images/sec of the hot path on H100, BASELINE.json's metric.
 
     python bench.py [--config hg_fpd] --gpus 1 --steps 20 --warmup 5
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
@@ -58,7 +58,7 @@ CONFIGS = {
         family="hourglass", student=(128, 4), teacher=None, batch=128, H=256, W=256, J=16, lr=0.0,
         flop_per_image=15.629e9, kind="infer",
         roof=dict(cin=64, cout=64, k=3, h=64, w=64)),
-    # --- beyond BASELINE.json (SURVEY 8 f4): the third registered model family, as experiments/mpii/resnet/res50_256x256_*
+    # --- beyond BASELINE.json the third registered model family, as experiments/mpii/resnet/res50_256x256_*
     "res50_mse": dict(
         workload="pose_resnet-50 (3 x 256-filter 4x4 deconv head) train, MSE only (function.train), 256x256, batch 32/GPU",
         family="resnet", student=50, teacher=None, batch=32, H=256, W=256, J=16, lr=1e-3,
@@ -75,7 +75,6 @@ CONFIGS = {
         family="hourglass", student=(256, 8), teacher=None, batch=32, H=256, W=256, J=16, lr=0.0,
         flop_per_image=56.189e9, kind="infer", flip=False, roof=dict(cin=128, cout=128, k=3, h=64, w=64)),
 }
-CONV_H_3X3_DRAM_BYTES = 89.88e6   # dram__bytes_read + write, conv_tc_h 3x3 128->128 @64x64 B=32: profiles/r2_prof_conv_h_3x3.md
 
 
 def cfg(f, s, j=16):
@@ -112,7 +111,7 @@ def hrnet_cfg(w, j=17):
 
 
 def synthetic_batch(B, seed, H=256, W=256, J=16):
-    """SURVEY.md 8d: N(0,1) images, reference-style Gaussian targets (sigma 2, 13x13, peak 1), 0/1 weights."""
+    """N(0,1) images, reference-style Gaussian targets (sigma 2, 13x13, peak 1), 0/1 weights."""
     import numpy as np
     import torch
     rng = np.random.RandomState(seed)
@@ -134,7 +133,7 @@ def synthetic_batch(B, seed, H=256, W=256, J=16):
 
 
 def synthetic_boxes(n, seed, W=256):
-    """SURVEY.md 8d NMS input: x1,y1 ~ U(0,W), w,h ~ U(8,128), score ~ U(0,1); returned sorted by score descending."""
+    """NMS input: x1,y1 ~ U(0,W), w,h ~ U(8,128), score ~ U(0,1); returned sorted by score descending."""
     import numpy as np
     rng = np.random.RandomState(seed)
     x1, y1 = rng.uniform(0, W, n), rng.uniform(0, W, n)
@@ -147,11 +146,11 @@ def workload_config(name, world, batch):
     # identical in both arms (GPU and `--impl reference`), so that a driver comparing the two lines sees one configuration
     return {"workload": c["workload"], "name": name, "global_batch": batch * world, "per_gpu_batch": batch,
             "parallelism": "dp%d" % world,
-            "l2": "per-step working set (activations: several GB) exceeds the 126 MB L2; no flush needed"}
+            "l2": "per-step working set (activations: several GB) exceeds the 50 MB L2; no flush needed"}
 
 
 class ClockSampler:
-    """Samples nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """Samples nvidia-smi clocks / throttle reasons DURING the timed region (clocks and throttle reasons behind the number)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -209,17 +208,16 @@ def measured_peaks():
         with open(path) as fh:
             d = json.load(fh)
         return d, "measured (MEASURED_PEAKS.json)"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback (B200_PROFILING.md)"
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "H100 SXM data sheet (dense, 700 W)"
 
 
 # --------------------------------------------------------------------------------------------------
 # CPU legs: the reference's own modules (oracle/_ref) on the host cores -- cpu_baseline and --impl reference.
 # The ONLY place bench.py touches oracle/.
 # --------------------------------------------------------------------------------------------------
-# Fastest (batch per step, threads) of the reference's CPU path on the B200 box's host (128 schedulable CPUs, Xeon 8562Y+),
-# from the committed sweep profiles/r2_cpu_thread_sweep.txt (tools/cpu_thread_sweep.py): more threads or larger batches
-# are SLOWER per image there (hg_fpd: 6.7 img/s at B=4 / 16 threads, 3.0 at B=8, 1.6 at B=32; 1.1 with 64 threads), so the
-# CPU legs run the sample size and thread count the reference is fastest with. FPD_CPU_THREADS / --batch override.
+# Batch per step and thread count for the reference's CPU path (tools/cpu_thread_sweep.py picks them per host): on a
+# many-core host more threads or larger batches were slower per image, so the CPU legs run a small sample with a
+# moderate thread count. FPD_CPU_THREADS / --batch override.
 CPU_BEST = {"hg_fpd": (4, 16), "hg_mse_s1": (2, 8), "hrnet_fpd": (8, 16), "hg_infer": (8, 16), "res50_mse": (8, 16)}
 
 
@@ -330,12 +328,18 @@ class CpuReference:
         """function.py:212-240 + inference.get_max_preds + numpy nms, on the CPU."""
         import numpy as np
         import torch
-        inf, tr, ns = self.dec
+        if self.kind == "port":     # oracle restatements of the same forward / decode / NMS
+            from oracle import decode_oracle as D
+            from oracle import hourglass_oracle as O
+            inf, tr, ns = D, D, {"nms": D.nms}
+            student = lambda t: O.hourglass_net(self.s_sd, t, self.c["student"][1], training=False)   # noqa: E731
+        else:
+            (inf, tr, ns), student = self.dec, self.student
         with torch.no_grad():
-            out = self.student(self.x)
+            out = student(self.x)
             out = out[-1] if isinstance(out, list) else out
             xf = torch.from_numpy(np.flip(self.x.numpy(), 3).copy())
-            of = self.student(xf)
+            of = student(xf)
             of = of[-1] if isinstance(of, list) else of
             of = torch.from_numpy(tr.flip_back(of.numpy(), MPII_FLIP_PAIRS).copy())
             of[:, :, :, 1:] = of.clone()[:, :, :, 0:-1]
@@ -370,7 +374,7 @@ def run_reference(args, rank):
     ips, n, threads, kind = time_cpu(name, B, args.steps, args.warmup, max_seconds=float(os.environ.get("FPD_CPU_MAX_S", "900")))
     sample = ("%s: the reference's own lib/models + lib/core/loss modules (oracle/_ref), loop body of lib/core/function.py, "
               "teacher under no_grad, %d images per step (the sample size and thread count the CPU path is fastest with, "
-              "profiles/r2_cpu_thread_sweep.txt), %d timed steps after %d warm-up, fp32, %d threads" % (
+              "tools/cpu_thread_sweep.py), %d timed steps after %d warm-up, fp32, %d threads" % (
                   kind, B, n, args.warmup, threads))
     line = {"impl": "reference", "metric": "images/sec", "value": ips, "unit": "images/s", "n_gpus": args.gpus,
             "steps": n, "warmup": args.warmup, "ms_per_step": 1000.0 * B / ips, "higher_is_better": True,
@@ -389,9 +393,9 @@ def run_reference(args, rank):
 # GPU arm
 # --------------------------------------------------------------------------------------------------
 def time_dominant_kernel(B, roof):
-    """Live CUDA-event timing of the dominant kernel (conv_tc_h_kernel<f16>: tcgen05 kind::f16 implicit-GEMM conv, halo
-    tile fetched + BN/ReLU-transformed + split once per channel block, taps as shifted copies into TMEM) on the config's
-    heaviest shape, 3xFP16. Eight launches per timed region over four rotating input/output sets (larger than the 126 MB
+    """Live CUDA-event timing of the dominant kernel (conv_wgmma_kernel<f16>: fp16 wgmma implicit-GEMM conv with the
+    BN/ReLU transform and operand split fused into the operand staging) on the config's
+    heaviest shape, 3xFP16. Eight launches per timed region over four rotating input/output sets (larger than the 50 MB
     L2 at the bench batch sizes, plus an explicit L2 flush before each group), replayed from a CUDA graph so that host
     launch cost is not in the region -- the same way the kernel runs inside the step."""
     import torch
@@ -500,6 +504,9 @@ def run_b200(args, rank, local_rank, world):
         d2h = 12
         launches = lambda: int(step.launches_per_step or 0)                  # noqa: E731
         final = lambda: float(loss_host[2])                                   # noqa: E731
+        # what a training loop gets from the last step: its losses and the updated weights (a fixed, seeded sample of the
+        # flat parameter vector, at most 4M values)
+        outputs = lambda: {"losses": loss_host.numpy(), "weights_sample": seeded_sample(step.flat.flat)}  # noqa: E731
     else:
         from fpd_b200.infer_step import FlipTestInference
         boxes = torch.from_numpy(synthetic_boxes(1024, 1)).to(dev)
@@ -519,6 +526,8 @@ def run_b200(args, rank, local_rank, world):
         d2h = idx_host.numel() * 4 + max_host.numel() * 4 + keep_host.numel() * 4
         launches = lambda: int(getattr(inf, "launches", 0))                  # noqa: E731
         final = lambda: float(max_host.sum())                                # noqa: E731
+        outputs = lambda: {"idx": idx_host.numpy().astype("float64"), "maxval": max_host.numpy(),   # noqa: E731
+                           "nms_keep": keep_host.numpy().astype("float64")}
 
     def barrier():
         if world > 1:
@@ -554,6 +563,8 @@ def run_b200(args, rank, local_rank, world):
         run_e2e()
     ms_e2e = timed(run_e2e, args.steps) / args.steps
     e2e_value = world * B / (ms_e2e / 1000.0)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, outputs())
 
     if rank != 0:
         _finish(world, dist)
@@ -575,20 +586,20 @@ def run_b200(args, rank, local_rank, world):
     step_frac = value / world * c["flop_per_image"] / 1e12 / peaks["bf16_tflops_sustained"]
     try:
         k_ms, k_flops = time_dominant_kernel(B, c["roof"])
-        f16_peak = peaks["bf16_tflops"]  # kind::f16 runs at the bf16 rate; burst figure: the kernel is timed alone
+        f16_peak = peaks["bf16_tflops"]  # fp16 wgmma runs at the bf16 rate; burst figure: the kernel is timed alone
         ach = k_flops / (k_ms * 1e-3) / 1e12
         r = c["roof"]
         line["roofline"] = {"bound": "tensor", "achieved": ach, "peak": f16_peak, "unit": "TFLOP/s",
                             "frac": ach / f16_peak,
-                            "traffic": CONV_H_3X3_DRAM_BYTES if (name == "hg_fpd" and B == 32) else None,
-                            "kernel": "conv_tc_h_kernel<f16> %dx%d %d->%d @%dx%d B=%d (3xFP16: 3 MMA passes per algorithmic "
+                            "traffic": None,   # DRAM bytes of the kernel: not measured on H100
+                            "kernel": "conv_wgmma_kernel<f16> %dx%d %d->%d @%dx%d B=%d (3xFP16: 3 MMA passes per algorithmic "
                                       "FLOP; executed-MMA fraction of peak = 3 x frac)" % (r["k"], r["k"], r["cin"], r["cout"],
                                                                                            r["h"], r["w"], B),
-                            "kernel_ms": k_ms, "peak_source": peak_src + ", kind::f16 = bf16 rate",
+                            "kernel_ms": k_ms, "peak_source": peak_src + ", fp16 wgmma = bf16 rate",
                             # best shape above; the whole step's algorithmic conv FLOP/s over the sustained peak:
                             "step_frac_of_f16_peak": step_frac,
                             # launch-weighted average of the dominant kernel over ALL its launches in a step (conv FLOPs of the
-                            # step / summed kernel time), from the committed launch list -- see profiles/README.md
+                            # step / summed kernel time) from a profiled step; null where not measured
                             "frac_launch_weighted": LAUNCH_WEIGHTED.get(name)}
     except Exception as exc:  # never lose the headline line to a side measurement
         line["roofline"] = {"error": repr(exc), "step_frac_of_f16_peak": step_frac}
@@ -604,6 +615,27 @@ def run_b200(args, rank, local_rank, world):
             line["cpu_baseline"] = {"error": repr(exc)}
     print(json.dumps(line), flush=True)
     _finish(world, dist)
+
+
+def seeded_sample(t, n=1 << 22):
+    """float32 copy of t, flattened, or of n of its elements at fixed seeded positions (sorted) when it is longer."""
+    import torch
+    flat = t.detach().reshape(-1).float()
+    if flat.numel() > n:
+        g = torch.Generator().manual_seed(12345)
+        idx = torch.randperm(flat.numel(), generator=g)[:n].sort().values.to(flat.device)
+        flat = flat[idx]
+    return flat.cpu().numpy()
+
+
+def dump_outputs(dirname, arrays):
+    """--dump-outputs: one DIR/<name>.npy per array (float32 / float64), so two builds can be compared output for output."""
+    import numpy as np
+    os.makedirs(dirname, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.ascontiguousarray(a)
+        assert a.dtype in (np.float32, np.float64), (name, a.dtype)
+        np.save(os.path.join(dirname, name + ".npy"), a)
 
 
 def _finish(world, dist):
@@ -623,11 +655,9 @@ def _finish(world, dist):
         os._exit(0)
 
 
-# launch-weighted roofline fraction of conv_tc_h_kernel over one whole step (all its launches): conv FLOPs it executes
-# in the step / its summed duration / peak. Filled from profiles/<tag>_launches.csv.gz by tools/summarize_profiles.py.
-# r2: 2.30 TFLOP of forward + data-gradient convolutions in 24.64 ms summed over its 765 launches (ncu launch list,
-# profiles/r2_launches_summary.md: cold caches, serialised; the warm CUPTI sum of profiles/r2_step_cupti.txt gives 0.064)
-LAUNCH_WEIGHTED = {"hg_fpd": 0.057}
+# launch-weighted roofline fraction of the dominant conv kernel over one whole step (all its launches), per config, from
+# a profiled step (tools/summarize_profiles.py); not measured on H100 yet, so reported as null
+LAUNCH_WEIGHTED = {}
 
 
 def main():
@@ -640,7 +670,13 @@ def main():
     ap.add_argument("--batch", type=int, default=0, help="images per GPU (default: the config's)")
     ap.add_argument("--no-graph", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default="",
+                    help="after the timed steps, write what the last step computed as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes the GPU path's outputs; it does not apply to --impl reference")
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))

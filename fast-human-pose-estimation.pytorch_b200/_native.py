@@ -29,7 +29,6 @@ _SIGNATURES = {
     "fpd_conv2d_tc_h_supported": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int]),
     "fpd_conv2d_tc_h": (c_int, [P, P, P, P, c_int, P, P, c_int, P, P, P, P, c_float, P, c_int, c_int, c_int, c_int, c_int,
                                 c_int, P]),
-    "fpd_conv2d_tc_h_set_profile_buffer": (c_int, [P]),
     "fpd_conv2d_tc_h_stats_blocks": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int]),
     "fpd_conv2d_tc_h_stats": (c_int, [P, P, P, P, c_int, P, P, c_int, P, P, P, c_float, c_int, c_int, c_int, c_int, c_int,
                                       c_int, P, P, P]),
@@ -105,7 +104,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise NativeLibraryMissing(
                 "libfpd_b200.so not found at %s -- run `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(there is no CPU / PyTorch fallback for the B200 kernels)" % LIB_PATH)
+                "(there is no CPU / PyTorch fallback for the H100 kernels)" % LIB_PATH)
         h = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in _SIGNATURES.items():
             fn = getattr(h, name)  # AttributeError here = header/library mismatch: fail loudly

@@ -1,7 +1,7 @@
-"""Build libfpd_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libfpd_b200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
 Usage: python build.py [--force]. Used by __graft_entry__.build(). Objects are cached under
-csrc/_build/ keyed on source mtime; the .so is git-ignored but travels with gpurun snapshots.
+csrc/_build/ keyed on source mtime; the .so and the objects are build products (git-ignored).
 """
 import os
 import subprocess
@@ -12,10 +12,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libfpd_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
          "--expt-relaxed-constexpr", "-Xptxas", "-v"]
-SOURCES = ["api.cu", "conv_tc3.cu", "conv_tc5.cu", "wgrad_tc2.cu", "wgrad_tc3.cu", "conv_simt.cu", "elementwise.cu", "loss.cu", "decode.cu", "nms.cu",
-           "adam.cu"]
+SOURCES = ["api.cu", "conv_wgmma.cu", "conv_simt.cu", "elementwise.cu", "loss.cu", "decode.cu", "nms.cu", "adam.cu"]
 
 
 def _newer(a, b):
@@ -25,7 +24,7 @@ def _newer(a, b):
 def build(force=False, verbose=False):
     bdir = os.path.join(CSRC, "_build")
     os.makedirs(bdir, exist_ok=True)
-    headers = [os.path.join(CSRC, h) for h in ("common.cuh", "kernels.h")] + [
+    headers = [os.path.join(CSRC, h) for h in ("common.cuh", "kernels.h", "wgmma.cuh")] + [
         os.path.join(HERE, "..", "include", "fpd_b200.h")]
     hdr_m = max(os.path.getmtime(h) for h in headers)
     jobs = []

@@ -31,7 +31,7 @@ int adam_flat(float* param, const float* grad, float* exp_avg, float* exp_avg_sq
   const double bc1 = 1.0 - pow((double)beta1, (double)step);
   const double bc2 = 1.0 - pow((double)beta2, (double)step);
   int64_t blocks = (n + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
   if (blocks < 1) blocks = 1;
   adam_kernel<<<(int)blocks, 256, 0, stream>>>(param, grad, exp_avg, exp_avg_sq, n, lr, beta1, beta2, eps,
                                                weight_decay, (float)bc1, (float)(1.0 / sqrt(bc2)), grad_scale);

@@ -1,6 +1,5 @@
 // api.cu -- the extern "C" surface declared in include/fpd_b200.h: thin argument-checking wrappers over
-// the launchers in kernels.h, the thread-local error string, the TMA descriptor encoder and the
-// `_nms`-compatible host entry point.
+// the launchers in kernels.h, the thread-local error string and the `_nms`-compatible host entry point.
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -22,57 +21,6 @@ void set_last_error(const char* fmt, ...) {
   va_start(ap, fmt);
   vsnprintf(g_err, sizeof(g_err), fmt, ap);
   va_end(ap);
-}
-
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn get_encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  static std::once_flag once;
-  std::call_once(once, [] {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-  });
-  return fn;
-}
-
-int encode_tmap(CUtensorMap* out, const void* gptr, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                const uint32_t* box, CUtensorMapSwizzle swz) {
-  return encode_tmap_dt(out, gptr, 0, rank, dims, strides_bytes, box, swz);
-}
-
-int encode_tmap_dt(CUtensorMap* out, const void* gptr, int dtype, int rank, const uint64_t* dims,
-                   const uint64_t* strides_bytes, const uint32_t* box, CUtensorMapSwizzle swz) {
-  EncodeTiledFn fn = get_encode_fn();
-  if (!fn) {
-    set_last_error("cuTensorMapEncodeTiled not available from the driver");
-    return FPD_ERR_CUDA;
-  }
-  cuuint64_t d[5];
-  cuuint64_t s[4];
-  cuuint32_t b[5], es[5];
-  for (int i = 0; i < rank; ++i) {
-    d[i] = dims[i];
-    b[i] = box[i];
-    es[i] = 1;
-  }
-  for (int i = 0; i + 1 < rank; ++i) s[i] = strides_bytes[i];
-  CUresult r = fn(out, dtype == 1 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (cuuint32_t)rank, const_cast<void*>(gptr), d, s, b, es,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_last_error("cuTensorMapEncodeTiled failed (CUresult %d): rank=%d dims=[%llu,%llu,%llu,%llu] box=[%u,%u,%u,%u]",
-                   (int)r, rank, (unsigned long long)d[0], (unsigned long long)(rank > 1 ? d[1] : 0),
-                   (unsigned long long)(rank > 2 ? d[2] : 0), (unsigned long long)(rank > 3 ? d[3] : 0), b[0],
-                   rank > 1 ? b[1] : 0, rank > 2 ? b[2] : 0, rank > 3 ? b[3] : 0);
-    return FPD_ERR_CUDA;
-  }
-  return FPD_OK;
 }
 
 }  // namespace fpd
@@ -151,11 +99,6 @@ int fpd_bn_stats_fused(const float* x, int64_t P, int C, const float* gamma, con
                         invstd, workspace, workspace_bytes, counter, S(stream));
 }
 
-int fpd_conv2d_tc_h_set_profile_buffer(long long* device_buf) {
-  conv_tc_h_set_profile_buffer(device_buf);
-  return FPD_OK;
-}
-
 int fpd_weight_prep_f16(const float* w, void* w_hi, void* w_lo, int O, int I, int k, int for_dgrad,
                         fpd_stream_t stream) {
   return weight_prep_f16(w, w_hi, w_lo, O, I, k, for_dgrad, S(stream));
@@ -173,10 +116,7 @@ int fpd_conv2d_wgrad_tc_supported(int Cin, int Cout, int ksize) {
   return wgrad_tc_supported(Cin, Cout, ksize) ? 1 : 0;
 }
 size_t fpd_conv2d_wgrad_tc_workspace_bytes(int B, int H, int W, int Cin, int Cout, int ksize) {
-  const size_t a = wgrad_tc_workspace_bytes(B, H, W, Cin, Cout, ksize, device_sm_count());
-  const size_t b = wgrad_tc3_supported(H, W, Cin, Cout, ksize)
-                       ? wgrad_tc3_workspace_bytes(B, H, W, Cin, Cout, device_sm_count()) : 0;
-  return a > b ? a : b;
+  return wgrad_tc_workspace_bytes(B, H, W, Cin, Cout, ksize, device_sm_count());
 }
 
 int fpd_conv2d_wgrad_tc_fused(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,

@@ -1,9 +1,7 @@
-// common.cuh -- sm_100a PTX wrappers (mbarrier / TMA / tcgen05 / TMEM) and small device helpers shared
-// by every kernel in libfpd_b200. Nothing here is portable: compile with
-//   -gencode arch=compute_100a,code=sm_100a
+// common.cuh -- error plumbing and small device helpers shared by every kernel in libfpd_b200 (built for sm_90a:
+//   -gencode arch=compute_90a,code=sm_90a)
 #pragma once
 #include <cuda_runtime.h>
-#include <cuda.h>
 #include <stdint.h>
 #include <cstdio>
 
@@ -44,6 +42,11 @@ void count_launch();
     FPD_CUDA_CHECK(cudaPeekAtLastError());  \
   } while (0)
 
+// Grid sizes of the bandwidth-bound kernels are multiples of the H100 SXM's 132 SMs (a few waves keep enough bytes in
+// flight for HBM; fixed caps keep the reductions' partial buffers, and so their summation order, independent of the
+// device they run on).
+constexpr int kNumSMs = 132;
+
 // ------------------------------------------------------------------------------------------------
 // numeric helpers
 // ------------------------------------------------------------------------------------------------
@@ -60,7 +63,7 @@ __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
 }
 
 // Same split with the rounding done in integer arithmetic (2 ALU ops instead of the multi-instruction emulation ptxas
-// emits for cvt.rna.tf32 on sm_100a): adding half an ulp of the 13 dropped bits and truncating is round-to-nearest,
+// emits for cvt.rna.tf32): adding half an ulp of the 13 dropped bits and truncating is round-to-nearest,
 // ties away from zero, i.e. exactly cvt.rna for finite inputs. Used inside the tensor-core pipelines where the
 // transform competes with the MMA issue for scheduler slots.
 __device__ __forceinline__ void split_tf32_fast(float x, float& hi, float& lo) {
@@ -84,205 +87,9 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred P1;\n\t"
-      "elect.sync _|P1, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, P1;\n\t"
-      "}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
-
-// ------------------------------------------------------------------------------------------------
-// mbarrier
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_fence_init() {
-  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
-               : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t"
-      "}\n"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-// Bounded wait: a protocol bug becomes a trap (-> CUDA error on the host) instead of a hung GPU.
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t spins = 0;
-  while (!mbar_try_wait(bar, parity)) {
-    if (++spins > (1u << 26)) {
-      printf("fpd: mbarrier wait timeout block=(%d,%d) thread=%d parity=%u\n", blockIdx.x, blockIdx.y,
-             threadIdx.x, parity);
-      __trap();
-    }
-  }
-}
-
-// generic-proxy smem writes -> visible to the async proxy (TMA / UMMA reads)
+// generic-proxy smem writes -> visible to the async proxy (wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
-
-// ------------------------------------------------------------------------------------------------
-// TMA (cp.async.bulk.tensor)
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
-  asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                            int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                            int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2),
-      "r"(c3)
-      : "memory");
-}
-
-// ------------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
-// ------------------------------------------------------------------------------------------------
-template <int kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst) {  // one full warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_alloc_dyn(uint32_t* smem_dst, uint32_t cols) {  // one full warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(cols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_dyn(uint32_t taddr, uint32_t cols) {  // same warp as alloc
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before_sync() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after_sync() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], tf32 inputs, fp32 accumulate. One thread issues.
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Same, A operand taken from tensor memory (lane m = row m, one tf32 per column), B from shared memory.
-__device__ __forceinline__ void umma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
-      "%15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// UMMA shared-memory matrix descriptor (see DESIGN.md "UMMA descriptors").
-//  bits [0,14)  start address >> 4      bits [16,30) leading byte offset >> 4
-//  bits [32,46) stride byte offset >> 4 bits [46,48) version (1 on sm_100)
-//  bits [49,52) base offset             bits [61,64) layout (2 = SWIZZLE_128B)
-__device__ __forceinline__ uint64_t umma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                              uint32_t layout_type) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)(layout_type & 7) << 61;
-  return d;
-}
-// K-major operand tile, 128-byte rows, SWIZZLE_128B (TMA: CU_TENSOR_MAP_SWIZZLE_128B)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  return umma_desc(smem_addr, lbo_bytes, sbo_bytes, 2);
-}
-// MN-major tf32 operand tile: the only legal swizzle is "128B with 32-byte atoms" (layout type 1, Swizzle<2,5,2>:
-// 32-byte chunk index ^= row & 3, 4-row / 512-byte pattern; TMA: CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B).
-__device__ __forceinline__ uint64_t umma_desc_sw128_32b(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  return umma_desc(smem_addr, lbo_bytes, sbo_bytes, 1);
-}
-// Instruction descriptor for kind::tf32 with fp32 accumulation.
-//  [4,6) c_format=1(F32)  [7,10) a_format=2(TF32)  [10,13) b_format=2  [15] a_major  [16] b_major
-//  [17,23) N>>3  [24,29) M>>4
-__host__ __device__ constexpr uint32_t umma_idesc_tf32(uint32_t M, uint32_t N, uint32_t a_mn_major,
-                                                       uint32_t b_mn_major) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | (a_mn_major << 15) | (b_mn_major << 16) | ((N >> 3) << 17) |
-         ((M >> 4) << 24);
-}
-
-// ------------------------------------------------------------------------------------------------
-// host side: driver entry point for cuTensorMapEncodeTiled (resolved through the runtime so the
-// library has no link-time dependency on libcuda).
-// ------------------------------------------------------------------------------------------------
-int encode_tmap(CUtensorMap* out, const void* gptr, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                const uint32_t* box, CUtensorMapSwizzle swz);
-// dtype: 0 = fp32 elements, 1 = fp16 elements (dims / box in elements, strides in bytes)
-int encode_tmap_dt(CUtensorMap* out, const void* gptr, int dtype, int rank, const uint64_t* dims,
-                   const uint64_t* strides_bytes, const uint32_t* box, CUtensorMapSwizzle swz);
 
 }  // namespace fpd

@@ -238,7 +238,7 @@ __global__ void conv_wgrad_final_kernel(const float* __restrict__ partial, float
 
 inline int grid_for(int64_t n, int threads) {
   int64_t b = (n + threads - 1) / threads;
-  const int64_t cap = 148 * 16;
+  const int64_t cap = kNumSMs * 16;
   return (int)(b < cap ? (b < 1 ? 1 : b) : cap);
 }
 
@@ -251,7 +251,7 @@ inline WgradGeom wgrad_geom(int64_t P, int Cin, int Cout, int k) {
   const int CoutP8 = (Cout + 7) & ~7;
   const size_t per_chunk = (size_t)k * k * Cin * CoutP8 * sizeof(float);
   // aim for ~2 waves of CTAs but keep the partial buffer under ~64 MB
-  int64_t nch = 148 * 4;
+  int64_t nch = kNumSMs * 4;
   const int64_t cap = (int64_t)((64u << 20) / per_chunk);
   if (nch > cap) nch = cap < 1 ? 1 : cap;
   int64_t chunk = (P + nch - 1) / nch;
@@ -280,7 +280,7 @@ int conv_simt_fwd(const float* x, const float* w_oihw, const float* bias, const 
     attr = true;
   }
   int grid = grid_for(n, 256);
-  if (use_smem && grid > 148 * 4) grid = 148 * 4;  // amortise the weight staging over a grid-stride loop
+  if (use_smem && grid > kNumSMs * 4) grid = kNumSMs * 4;  // amortise the weight staging over a grid-stride loop
   conv_fwd_kernel<<<grid, 256, smem, stream>>>(x, w_oihw, bias, residual, y, B, H, W, Cin, Cout, k, stride, pad, Ho,
                                                Wo, use_smem);
   FPD_LAUNCH_CHECK();
@@ -302,7 +302,7 @@ int conv_simt_dgrad(const float* dy, const float* w_oihw, float* dx, int B, int 
     attr = true;
   }
   int grid = grid_for(n, 256);
-  if (use_smem && grid > 148 * 4) grid = 148 * 4;
+  if (use_smem && grid > kNumSMs * 4) grid = kNumSMs * 4;
   conv_dgrad_kernel<<<grid, 256, smem, stream>>>(dy, w_oihw, dx, B, H, W, Cin, Cout, k, stride, pad, Ho, Wo,
                                                  use_smem);
   FPD_LAUNCH_CHECK();

@@ -3,7 +3,7 @@
 // BN+ReLU apply fused with the tf32 hi/lo operand split, BN backward, 2x2 max-pool fwd/bwd
 // (hourglass.py:82,124), nearest-2x upsample + add (hourglass.py:60,90-91), layout converts, weight
 // re-layout. All kernels are vectorised (float4 along the channel axis = the contiguous NHWC axis) and
-// sized for >= 2 waves of 148 SMs; reductions are deterministic (fixed-order partial buffers, no atomics).
+// sized for >= 2 waves of the H100's 132 SMs (kNumSMs); reductions are deterministic (fixed-order partial buffers, no atomics).
 #include <cuda_fp16.h>
 
 #include "common.cuh"
@@ -14,7 +14,7 @@ namespace fpd {
 namespace {
 
 constexpr int kRedThreads = 256;
-constexpr int kMaxRedBlocks = 592;   // 4 x 148 SMs: enough bytes in flight for HBM, and a short second stage
+constexpr int kMaxRedBlocks = 4 * kNumSMs;   // enough bytes in flight for HBM, and a short second stage
 
 struct RedGeom {
   int L;       // float4 lanes across channels (C/4)
@@ -25,7 +25,7 @@ struct RedGeom {
 
 inline RedGeom red_geom(int64_t P, int C, int max_blocks = kMaxRedBlocks);
 // the single-launch (last block finishes) forms keep the second stage short: one wave of blocks
-constexpr int kMaxFusedRedBlocks = 148;
+constexpr int kMaxFusedRedBlocks = kNumSMs;
 inline RedGeom red_geom(int64_t P, int C, int max_blocks) {
   RedGeom g;
   g.L = C / 4;
@@ -312,7 +312,7 @@ bn_sums_finalize_kernel(const double* __restrict__ part, int nblocks, const floa
 // -------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void write_amax_scale(float m, float* amax_scale) {
   // power-of-two scale that puts max|v| into [2^14, 2^15): fp16 hi/lo operands of v * S then keep every element to within
-  // 2^-39 of the largest one (csrc/conv_tc5.cu in_scale). Zero / non-finite maxima -> no scaling.
+  // 2^-39 of the largest one (csrc/conv_wgmma.cu in_scale). Zero / non-finite maxima -> no scaling.
   float S = 1.f;
   if (m > 0.f && m < 3.0e38f) {
     int e;
@@ -920,7 +920,7 @@ __global__ void weight_prep_kernel(const float* __restrict__ w, float* __restric
   }
 }
 
-// fp16 hi/lo operand form of the weights for the 3xFP16 convolution (conv_tc5.cu): w * 2^scale_log2 = hi + lo with
+// fp16 hi/lo operand form of the weights for the 3xFP16 convolution (conv_wgmma.cu): w * 2^scale_log2 = hi + lo with
 // hi = fp16(w'), lo = fp16(w' - hi); the power-of-two pre-scale keeps lo out of the fp16 subnormal range for ordinary
 // weight magnitudes (|w| ~ 1e-2) and is undone exactly in the convolution epilogue. Saturates at +-65504.
 __global__ void weight_prep_f16_kernel(const float* __restrict__ w, __half* __restrict__ hi, __half* __restrict__ lo,
@@ -1060,7 +1060,7 @@ __global__ void im2col_kernel(const float* __restrict__ x, float4* __restrict__ 
 
 inline int grid_for(int64_t n, int threads) {
   int64_t b = (n + threads - 1) / threads;
-  const int64_t cap = 148 * 16;
+  const int64_t cap = kNumSMs * 16;
   return (int)(b < cap ? (b < 1 ? 1 : b) : cap);
 }
 
@@ -1264,7 +1264,7 @@ template <int NV, class F>
 static int run_channel_reduce_fused(F f, int64_t P, int C, float scale, float* out, float* amax_scale, void* workspace,
                                     size_t ws_bytes, unsigned int* counter, cudaStream_t stream) {
   // Two launches (partial + final). A single-launch "last block finishes" form exists behind counter != null in the
-  // kernel, but measured ~2x slower on B200 (one wave of blocks starves the main pass of memory parallelism, many blocks
+  // kernel, but measured ~2x slower on an earlier GPU (one wave of blocks starves the main pass of memory parallelism, many blocks
   // make the one-CTA tail long), so the counter is accepted for ABI stability and ignored.
   (void)counter;
   FPD_REQUIRE(C % 4 == 0 && C >= 4 && C <= 4096, "channel reduce: C=%d must be a multiple of 4 in [4,4096]", C);
@@ -1532,8 +1532,8 @@ int device_sm_count() {
   static int n = 0;
   if (n == 0) {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return kNumSMs;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = kNumSMs;
   }
   return n;
 }

@@ -7,7 +7,7 @@
 
 namespace fpd {
 
-// ---- conv_tc3.cu : fused operand transform with the A operand in tensor memory (TS-mode MMA) ----
+// ---- conv_wgmma.cu : warpgroup-MMA implicit-GEMM convolution (3xTF32, Cin <= 512) ----
 bool conv_tc_ts_supported(int Cin, int Cout, int ksize);   // Cout up to 1024 in slices of <= 128 columns
 int conv_tc_ts_slice(int Cout);
 int conv_tc_ts_launch(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
@@ -15,12 +15,10 @@ int conv_tc_ts_launch(const float* x, const float* pre_mean, const float* pre_sc
                       const float* relu_mask, float* y, float out_scale, int B, int H, int W, int Cin, int Cout,
                       int ksize, int num_sms, cudaStream_t stream);
 
-// ---- conv_tc5.cu : halo-tile reuse (3x3: one fetch + one transform per channel block, nine shifted smem->TMEM copies)
-//      and optional 3xFP16 operands (f16 = 1: w_hi / w_lo are __half [tap][Cout][Cin] from weight_prep_f16, pre-scaled
+// ---- conv_wgmma.cu : the same kernel with Cin up to 2048, optional epilogue statistics and optional 3xFP16 operands (f16 = 1: w_hi / w_lo are __half [tap][Cout][Cin] from weight_prep_f16, pre-scaled
 //      by 2^kF16WeightScaleLog2; f16 = 0: fp32 containers from weight_prep, 3xTF32) ----
 constexpr int kF16WeightScaleLog2 = 8;
 bool conv_tc_h_supported(int Cin, int Cout, int ksize, int H, int W, int f16);
-void conv_tc_h_set_profile_buffer(long long* buf);   // per-CTA stall counters [grid][16] (tools/diag_conv_h.py); null = off
 int conv_tc_h_launch(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
                      int pre_relu, const void* w_hi, const void* w_lo, int f16, const float* bias,
                      const float* residual, const float* relu_mask, float* y, float out_scale, const float* in_scale,
@@ -30,8 +28,8 @@ int conv_tc_h_launch(const float* x, const float* pre_mean, const float* pre_sca
 // stat_part[blocks][Cout][2] (0: this shape cannot carry the statistics, e.g. Cout > 256)
 int conv_tc_h_stats_grid(int B, int H, int W, int Cin, int Cout, int ksize, int f16, int num_sms);
 
-// ---- wgrad_tc2.cu : tcgen05 weight-gradient GEMM (K = pixels) reading RAW x and dY; BN-apply + ReLU + tf32 split fused
-//      into the pipeline ----
+// ---- conv_wgmma.cu : warpgroup-MMA weight-gradient GEMM (K = pixels) reading RAW x and dY; BN-apply + ReLU + tf32 split
+//      fused into the operand staging ----
 bool wgrad_tc_supported(int Cin, int Cout, int ksize);
 size_t wgrad_tc_workspace_bytes(int B, int H, int W, int Cin, int Cout, int ksize, int num_sms);
 int wgrad_tc_fused_launch(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
@@ -39,13 +37,8 @@ int wgrad_tc_fused_launch(const float* x, const float* pre_mean, const float* pr
                           int Cin, int Cout, int ksize, void* workspace, size_t workspace_bytes, int num_sms,
                           cudaStream_t stream);
 
-// ---- wgrad_tc3.cu : 3x3 weight gradient, one halo tile per pixel block + all taps per CTA (taps = shifted start rows of
-//      the same MN-major shared-memory tile). wgrad_tc_fused_launch dispatches here when the shape is supported. ----
+// the 3x3 shape rule of wgrad_tc_supported (fpd_conv2d_wgrad_tc3_supported)
 bool wgrad_tc3_supported(int H, int W, int Cin, int Cout, int ksize);
-size_t wgrad_tc3_workspace_bytes(int B, int H, int W, int Cin, int Cout, int num_sms);
-int wgrad_tc3_launch(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
-                     int pre_relu, const float* dy, int passes, float* dw_oihw, float scale, int B, int H, int W,
-                     int Cin, int Cout, void* workspace, size_t workspace_bytes, int num_sms, cudaStream_t stream);
 
 // ---- conv_simt.cu : generic fp32 CUDA-core convolution (any k / stride / pad, NHWC activations,
 //      OIHW weights). Used for the shapes the tensor-core kernels do not take (7x7 stem, 16-channel
@@ -127,7 +120,7 @@ int affine_act_bwd(const float* da, const float* x, const float* mean, const flo
 // OIHW fp32 -> [tap][O][I] (fwd) or [flipped tap][I][O] (dgrad), split into tf32 hi/lo
 int weight_prep(const float* w_oihw, float* w_hi, float* w_lo, int O, int I, int k, int for_dgrad,
                 cudaStream_t stream);
-// same layouts as __half hi/lo of w * 2^kF16WeightScaleLog2 (3xFP16 operands of conv_tc5.cu)
+// same layouts as __half hi/lo of w * 2^kF16WeightScaleLog2 (3xFP16 operands of conv_wgmma.cu)
 int weight_prep_f16(const float* w_oihw, void* w_hi, void* w_lo, int O, int I, int k, int for_dgrad,
                     cudaStream_t stream);
 // forward [tap][O][I] and data-gradient [taps-1-tap][I][O] forms in one launch

@@ -1,11 +1,11 @@
-// nms.cu -- greedy box NMS for sm_100a, entirely on the device.
+// nms.cu -- greedy box NMS for sm_90a, entirely on the device.
 //
 // What it replaces: reference lib/nms/nms_kernel.cu:33-77 (pairwise-IoU bit-mask kernel) and the host
 // driver `_nms` :90-143 (cudaMalloc/cudaFree per call, full-mask D2H, serial host sweep).
 // Same arithmetic contract: boxes pre-sorted by score, IoU with the "+1 pixel" convention, a box is
 // suppressed when IoU > thresh (strict), result = indices (into the sorted list) that survive.
 //
-// B200 design:
+// Design:
 //  * pass 1 (HBM/L2-bound, embarrassingly parallel): only the upper triangle of 64x64 tiles is launched
 //    (the reference computes both triangles and throws the lower away); box tiles are staged as SoA in
 //    shared memory so the inner loop is bank-conflict free; each thread owns one row box and emits one

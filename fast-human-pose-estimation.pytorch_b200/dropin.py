@@ -1,4 +1,4 @@
-"""Wire the B200 hot path under the reference's tools WITHOUT shadowing its packages.
+"""Wire the H100 hot path under the reference's tools WITHOUT shadowing its packages.
 
 The reference resolves everything by module name after tools/_init_paths.py put `<reference>/lib` on sys.path
 (tools/fpd_train.py:27-40: `from core.function import train, fpd_train, validate`, `from core.loss import

@@ -2,7 +2,7 @@
 
 The network topology is the reference's (lib/models/hourglass.py:32-52 Bottleneck.forward, :80-95
 Hourglass._hour_glass_forward, :170-192 HourglassNet.forward); the execution is not: activations live in
-NHWC, every op is a libfpd_b200 kernel (tcgen05 implicit-GEMM convs, fused BN/ReLU/operand-split, ...),
+NHWC, every op is a libfpd_b200 kernel (wgmma implicit-GEMM convs, fused BN/ReLU/operand-split, ...),
 and the backward pass is an explicit tape of kernel launches instead of a per-op autograd graph.
 
 Python here only sequences launches and owns tensors (torch = device memory + streams); there is no
@@ -16,7 +16,7 @@ from . import ops
 
 
 # conv(relu(bn(x))): the operand transform (BN-apply + ReLU + hi/lo split) always happens inside the tensor-core kernels
-# (csrc/conv_tc5.cu, conv_tc3.cu, wgrad_tc2.cu, wgrad_tc3.cu); the round-1 two-kernel forms (pre-split operands in HBM)
+# (csrc/conv_wgmma.cu); the round-1 two-kernel forms (pre-split operands in HBM)
 # and their A/B switches were removed in round 2.
 # forward: run each hourglass level's skip branch on a side stream (see Engine.hourglass)
 FORK_UP1 = os.environ.get("FPD_FORK_UP1", "1") != "0"
@@ -68,8 +68,8 @@ class Var:
 
 
 # stride-2 3x3 convolutions (HRNet stem / transitions / fuse down paths) on the stride-1 tensor-core kernels:
-# y = subsample2(conv_s1(x)); 4x the necessary MACs, but on tcgen05 instead of the CUDA-core fallback (which was 97 % of
-# the HRNet step: profiles/r2b_timeline_hrnet.txt)
+# y = subsample2(conv_s1(x)); 4x the necessary MACs, but on the tensor cores instead of the CUDA-core fallback (hrnet_fpd on one
+# H100 SXM at 700 W: 103 ms/step, 319 ms/step with the CUDA-core path)
 STRIDE2_TC = os.environ.get("FPD_STRIDE2_TC", "1") != "0"
 
 
@@ -114,8 +114,8 @@ class ConvRef:
             return (K + 31) // 32 * 32
         return 0
 
-    # the TS kernel (csrc/conv_tc3.cu) takes Cin <= 512, Cout <= 1024 at any image size; the generation-5 kernel
-    # (csrc/conv_tc5.cu) up to 2048 channels where its tiling fits (H, W of the call decide)
+    # the tensor-core kernel (csrc/conv_wgmma.cu) takes Cin <= 512, Cout <= 1024 through ops.conv2d_tc_fused and up to
+    # 2048 channels each way through ops.conv2d_tc_h, at any image size
     def tc_fwd_at(self, H, W):
         return self.s1 and self.pad == self.k // 2 and (
             ops.conv2d_tc_supported(self.cin, self.cout, self.k)
@@ -151,8 +151,8 @@ class BNRef:
 class PreparedWeights:
     """Tensor-core operand forms of the conv weights, prepared on first use within a forward (student: every step,
     inside the captured graph; frozen teacher: once, cached with the eval context):
-    [tap][O][I] hi/lo (+ flipped/transposed for dgrad). Forward operands are __half pairs (3xFP16, csrc/conv_tc5.cu)
-    where that kernel takes the shape, fp32 containers holding tf32 values otherwise."""
+    [tap][O][I] hi/lo (+ flipped/transposed for dgrad). Forward operands are __half pairs (3xFP16, csrc/conv_wgmma.cu)
+    where ops.conv2d_tc_h takes the shape, fp32 containers holding tf32 values otherwise."""
 
     def __init__(self, passes, scale_without_bias=False):
         self.split = passes == 3
@@ -164,7 +164,8 @@ class PreparedWeights:
         self.scale_without_bias = scale_without_bias
 
     def fwd(self, c, H, W, also_dgrad=False):
-        """-> (w_hi, w_lo, use_h): use_h selects ops.conv2d_tc_h (generation-5 kernel) over the TS kernel.
+        """-> (w_hi, w_lo, use_h): use_h selects ops.conv2d_tc_h (Cin up to 2048, 3xFP16) over ops.conv2d_tc_fused
+        (3xTF32, Cin up to 512).
         also_dgrad: a backward pass will want the data-gradient form too -- when both are 3xFP16 they come out of one
         launch (one read of the weights)."""
         e = self._fwd.get(c.name)

@@ -7,7 +7,7 @@ bottleneck_post); new here are
  * the stem pool nn.MaxPool2d(3, 2, 1)                      -> Engine.maxpool3
  * strided blocks: 3x3 stride 2 = stride-1 tensor-core conv + even pick (ConvRef.as_s1), 1x1 stride-2 downsample = even
    pick + stride-1 1x1 (ConvRef.pick_first)
- * 512..2048-channel layers: csrc/conv_tc5.cu takes them whole, the weight gradients go chunk by chunk
+ * 512..2048-channel layers: csrc/conv_wgmma.cu takes them whole, the weight gradients go chunk by chunk
    (ops.conv2d_wgrad_tc_chunked)
  * ConvTranspose2d(k, stride 2) of the head = 3x3 convolution to 4 x Cout channels + depth-to-space (Engine.deconv); the
    BatchNorm + ReLU between two head layers is fused into the consuming convolution's operand pass as everywhere else.

@@ -4,7 +4,7 @@ Same public surface: `get_pose_net(cfg, is_train, **kwargs) -> nn.Module`, `forw
 list of NUM_STACKS tensors [B,J,H/4,W/4]`, and a `state_dict()` whose keys/shapes equal the reference's
 (hourglass.py:98-168), so published checkpoints load with strict=True. The module tree only *stores*
 parameters (ordinary nn.Conv2d / nn.BatchNorm2d leaves, created in the reference's order so a given seed
-yields the same initial weights); the arithmetic runs in fpd_b200.engine on libfpd_b200's sm_100a
+yields the same initial weights); the arithmetic runs in fpd_b200.engine on libfpd_b200's sm_90a
 kernels. There is no CPU / torch-op fallback: calling forward on a CPU tensor raises.
 """
 import torch
@@ -23,7 +23,7 @@ class _ParamOnly(nn.Module):
 
     def forward(self, *a, **k):
         raise RuntimeError("%s holds parameters only; run the enclosing HourglassNet (its forward drives the "
-                           "B200 engine)" % type(self).__name__)
+                           "H100 engine)" % type(self).__name__)
 
 
 class Bottleneck(_ParamOnly):
@@ -103,7 +103,7 @@ class HourglassNet(nn.Module):
     def forward(self, x):
         dev = self.conv1.weight.device
         if dev.type != "cuda":
-            raise RuntimeError("fpd_b200 HourglassNet runs on a CUDA (sm_100a) device only; the module is on %s. "
+            raise RuntimeError("fpd_b200 HourglassNet runs on a CUDA (sm_90a) device only; the module is on %s. "
                                "There is no CPU fallback: call .cuda() first." % dev)
         if not x.is_cuda:   # host batch from a DataLoader: stage it like nn.DataParallel's scatter would
             x = x.to(dev, non_blocking=True)

@@ -3,7 +3,7 @@
 Same public surface (`get_pose_net(cfg, is_train)`, `forward(x[B,3,H,W]) -> Tensor[B,J,H/4,W/4]`, `init_weights`)
 and the same `state_dict()` keys/shapes as `PoseHighResolutionNet` (pose_hrnet.py:274-423), so ImageNet-pretrained /
 published checkpoints load unchanged. Like the hourglass drop-in the tree only stores parameters (created in the
-reference's construction order); the arithmetic runs in fpd_b200.engine_hrnet on libfpd_b200's sm_100a kernels.
+reference's construction order); the arithmetic runs in fpd_b200.engine_hrnet on libfpd_b200's sm_90a kernels.
 `cfg` may be attribute-style or dict-style (the reference mixes both: pose_hrnet.py:278,291).
 """
 import logging
@@ -202,7 +202,7 @@ class PoseHighResolutionNet(nn.Module):
     def forward(self, x):
         dev = self.conv1.weight.device
         if dev.type != "cuda":
-            raise RuntimeError("fpd_b200 PoseHighResolutionNet runs on a CUDA (sm_100a) device only; the module is on "
+            raise RuntimeError("fpd_b200 PoseHighResolutionNet runs on a CUDA (sm_90a) device only; the module is on "
                                "%s. There is no CPU fallback: call .cuda() first." % dev)
         if not x.is_cuda:   # host batch from a DataLoader: stage it like nn.DataParallel's scatter would
             x = x.to(dev, non_blocking=True)

@@ -4,7 +4,7 @@ Same public surface (`get_pose_net(cfg, is_train)`, `forward(x[B,3,H,W]) -> Tens
 `resnet_spec`) and the same `state_dict()` keys/shapes as `PoseResNet` (pose_resnet.py:98-204), so torchvision ImageNet
 ResNet checkpoints (`strict=False`, pose_resnet.py:226-228) and published pose checkpoints load unchanged. Like the other
 two drop-ins the tree only stores parameters, created in the reference's construction order; the arithmetic runs in
-fpd_b200.engine_resnet on libfpd_b200's sm_100a kernels (the stride-2 transposed convolutions of the head as 3x3
+fpd_b200.engine_resnet on libfpd_b200's sm_90a kernels (the stride-2 transposed convolutions of the head as 3x3
 tensor-core convolutions + a depth-to-space shuffle, see Engine.deconv).
 """
 import logging
@@ -115,7 +115,7 @@ class PoseResNet(nn.Module):
     def forward(self, x):
         dev = self.conv1.weight.device
         if dev.type != "cuda":
-            raise RuntimeError("fpd_b200 PoseResNet runs on a CUDA (sm_100a) device only; the module is on %s. There is "
+            raise RuntimeError("fpd_b200 PoseResNet runs on a CUDA (sm_90a) device only; the module is on %s. There is "
                                "no CPU fallback: call .cuda() first." % dev)
         if not x.is_cuda:   # host batch from a DataLoader: stage it like nn.DataParallel's scatter would
             x = x.to(dev, non_blocking=True)

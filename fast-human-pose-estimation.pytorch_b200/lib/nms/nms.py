@@ -1,4 +1,4 @@
-"""Drop-in for the reference's lib/nms/nms.py, backed by libfpd_b200's sm_100a kernels (csrc/nms.cu):
+"""Drop-in for the reference's lib/nms/nms.py, backed by libfpd_b200's sm_90a kernels (csrc/nms.cu):
 
   gpu_nms / gpu_nms_wrapper   gpu_nms.pyx:19-34, nms.py:27-32  -> fpd_nms_host (C ABI, reference `_nms` signature)
   nms / py_nms_wrapper / cpu_nms_wrapper   nms.py:17-24,35-72  -> the same device path (identical keep lists)

@@ -140,8 +140,8 @@ def im2col(x, k, stride, pad, kpad, out=None):
 
 def conv2d_tc_fused(x, w_hi, w_lo, ksize, mean=None, scale=None, shift=None, relu=False, bias=None, residual=None,
                     relu_mask=None, out=None, out_scale=1.0):
-    """y = conv(relu?((x-mean)*scale+shift)) on the TS kernel (csrc/conv_tc3.cu: per-tap TMA, operand transform -> TMEM,
-    3xTF32) -- the fallback for the shapes the generation-5 kernel (conv2d_tc_h) declines."""
+    """y = conv(relu?((x-mean)*scale+shift)) on the tensor cores (csrc/conv_wgmma.cu,
+    3xTF32) -- the fallback for the shapes conv2d_tc_h declines."""
     B, H, W, Cin = x.shape
     Cout = w_hi.shape[1]
     y = out if out is not None else torch.empty((B, H, W, Cout), dtype=torch.float32, device=x.device)
@@ -151,7 +151,7 @@ def conv2d_tc_fused(x, w_hi, w_lo, ksize, mean=None, scale=None, shift=None, rel
     return y
 
 
-CONV_H = os.environ.get("FPD_CONV_H", "1") != "0"          # generation-5 kernel (halo reuse) where it supports the shape
+CONV_H = os.environ.get("FPD_CONV_H", "1") != "0"          # conv2d_tc_h (3xFP16 capable, Cin up to 2048) where it supports the shape
 CONV_F16 = os.environ.get("FPD_CONV_F16", "1") != "0"      # 3xFP16 operands for the forward convolutions
 CONV_F16_DGRAD = os.environ.get("FPD_CONV_F16_DGRAD", "1") != "0"   # ... and for the data-gradient convolutions (dY * 2^k)
 
@@ -186,9 +186,9 @@ def weight_prep_f16_both(w_oihw):
 
 
 # BatchNorm statistics of conv outputs from the conv epilogue: "0" off, "1" every tensor-core conv, "3x3" only the 3x3
-# convolutions (tensor-bound: their epilogue has slack; the 1x1 convolutions are epilogue-bound). Measured on the bench
-# configuration (profiles/r2_fusion_ab.txt): every conv 34.4 ms/step, off 33.6-33.9, 3x3 only 33.1 -- the step is bound by
-# the total time of the full-grid kernels, so the statistics pay only where the epilogue is not the conv's own limit.
+# convolutions. On the bench configuration (hg_fpd, one H100 SXM at 700 W, two runs each) the three settings are within
+# noise of each other: 3x3 83.9 / 84.0 ms/step, off 84.0 / 83.9, every conv 83.9 / 83.9. "3x3" is kept: it saves the
+# separate statistics pass over the largest tensors without adding epilogue work to the 1x1 convolutions.
 CONV_STATS = os.environ.get("FPD_CONV_STATS", "3x3").lower()
 
 
@@ -214,7 +214,7 @@ def bn_finalize_sums(part, nblocks, pivot, P, gamma, beta, eps, running_mean=Non
 
 def conv2d_tc_h(x, w_hi, w_lo, ksize, mean=None, scale=None, shift=None, relu=False, bias=None, residual=None,
                 relu_mask=None, out=None, out_scale=1.0, in_scale=None, stats_part=None, stats_pivot=None):
-    """y = conv(relu?((x-mean)*scale+shift)) on the generation-5 kernel (csrc/conv_tc5.cu). The operand precision
+    """y = conv(relu?((x-mean)*scale+shift)) on the fused tensor-core kernel (csrc/conv_wgmma.cu). The operand precision
     follows the weight dtype: float16 hi/lo -> 3xFP16 (kind::f16), float32 containers -> 3xTF32."""
     B, H, W, Cin = x.shape
     Cout = w_hi.shape[1]
@@ -387,8 +387,8 @@ def bn_bwd_reduce(da, x, mean, invstd, scale, shift, relu):
 
 
 # bias-gradient sums + dY operand scale out of the BN-backward apply pass (one launch and one read of dx less per conv);
-# measured neutral (34.35 vs 34.42 ms/step: the reduction-geometry kernel keeps fewer loads in flight than the plain
-# elementwise apply), so off by default
+# not a measurable gain on the bench configuration (hg_fpd, one H100 SXM at 700 W: 83.9 / 83.3 ms/step on, 83.9 / 84.0
+# off -- within the run-to-run spread), so off by default
 BN_APPLY_SUM = os.environ.get("FPD_BN_APPLY_SUM", "0") != "0"
 
 

@@ -3,7 +3,7 @@ buffer per step (NCCL over NVLink/NVSwitch on the GPU box; gloo in the CPU tests
 
 Replaces the reference's single-process nn.DataParallel (tools/fpd_train.py:143,173), which every iteration
 scatters the batch, re-broadcasts all parameters (13 MB student + 102 MB teacher), gathers all outputs to GPU 0 and
-reduces gradients to GPU 0 (SURVEY.md 2.3). Here weights stay resident on every rank; the teacher needs no
+reduces gradients to GPU 0. Here weights stay resident on every rank; the teacher needs no
 communication; BatchNorm statistics stay per-rank (= the reference's per-replica semantics)."""
 import torch
 import torch.distributed as dist

@@ -1,4 +1,4 @@
-"""Heat-map target generation on the device for a whole batch (SURVEY.md 8 f4): the GPU-side replacement for the per-sample
+"""Heat-map target generation on the device for a whole batch: the GPU-side replacement for the per-sample
 numpy loop of JointsDataset.generate_target (reference lib/dataset/JointsDataset.py:233-289), to be called on the joints
 that come out of the loader's augmentation (after the H2D copy) instead of shipping [B,J,h,w] float targets over PCIe."""
 import torch

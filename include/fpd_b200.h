@@ -1,4 +1,4 @@
-/* fpd_b200.h -- C ABI of libfpd_b200.so: the B200 (sm_100a) kernels behind the reference's hot path
+/* fpd_b200.h -- C ABI of libfpd_b200.so: the H100 (sm_90a) kernels behind the reference's hot path
  * (ilovepose/fast-human-pose-estimation.pytorch: stacked-hourglass / HRNet heat-map regression with the
  * Fast-Pose-Distillation loss, flip-test decode, box NMS).
  *
@@ -55,18 +55,15 @@ long long fpd_launch_count(void);
  *   y) elements with relu_mask <= 0 are written as 0 (ReLU backward fused).
  *   w_hi/w_lo : [ksize*ksize][Cout][Cin] fp32 containers holding tf32 values from fpd_weight_prep (w_lo NULL => single-pass
  *               TF32; both non-NULL => 3xTF32, fp32-grade accuracy)
- * TS kernel (csrc/conv_tc3.cu): the prepared A tiles are written to tensor memory and the MMAs run in TS mode (A from TMEM,
- * B from shared memory). Takes every shape: the fallback for what the generation-5 kernel below declines. (The round-1
- * kernels with pre-split operands in HBM -- fpd_conv2d_tc, fpd_conv2d_tc_fused, fpd_conv2d_tc_g -- were removed.) */
+ * Runs on the warpgroup-MMA implicit-GEMM kernel of csrc/conv_wgmma.cu (3xTF32 operands), Cin up to 512. */
 int fpd_conv2d_tc_ts_supported(int Cin, int Cout, int ksize); /* Cout up to 1024, processed in <=128-column slices */
 int fpd_conv2d_tc_ts(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
                      int pre_relu, const float* w_hi, const float* w_lo, const float* bias, const float* residual,
                      const float* relu_mask, float* y, float out_scale, int B, int H, int W, int Cin, int Cout,
                      int ksize, fpd_stream_t stream);
 
-/* Generation-5 fused convolution (csrc/conv_tc5.cu), same contract as fpd_conv2d_tc_ts. 3x3: the activation tile is
- * fetched with its halo and transformed once per channel block, the nine taps are shifted on-chip copies into tensor
- * memory. f16 = 1 selects 3xFP16 operands (x = hi + lo in fp16, tcgen05.mma kind::f16, fp32 accumulate): w_hi / w_lo
+/* Fused convolution (csrc/conv_wgmma.cu), same contract as fpd_conv2d_tc_ts, Cin up to 2048 and Cout up to 2048.
+ * f16 = 1 selects 3xFP16 operands (x = hi + lo in fp16, fp16 wgmma, fp32 accumulate): w_hi / w_lo
  * are then the __half arrays of fpd_weight_prep_f16; f16 = 0: fp32 containers of fpd_weight_prep (3xTF32).
  * w_lo NULL => single pass. in_scale (nullable, device float[2] {S, 1/S}, e.g. from fpd_channel_sum_fused): the operand
  * is x * S and the result is multiplied by 1/S -- exact powers of two that bring small-magnitude gradients into the fp16
@@ -81,10 +78,6 @@ int fpd_conv2d_tc_h(const float* x, const float* pre_mean, const float* pre_scal
  * weights: one launch per convolution and training step instead of two. */
 int fpd_weight_prep_f16_both(const float* w_oihw, void* f_hi, void* f_lo, void* d_hi, void* d_lo, int O, int I, int k,
                              fpd_stream_t stream);
-/* Profiling aid: when device_buf is non-NULL every following fpd_conv2d_tc_h launch writes, per CTA, 16 int64 stall
- * counters (cycles each warp role spent waiting on each pipeline barrier) to device_buf[blockIdx.x * 16 ...]; NULL
- * switches it off (the default). Not thread-safe; intended for tools/diag_conv_h.py only. */
-int fpd_conv2d_tc_h_set_profile_buffer(long long* device_buf);
 /* OIHW fp32 -> __half hi/lo of w * 2^8 in the layouts of fpd_weight_prep (w_lo may be NULL); the 2^-8 is applied by
  * fpd_conv2d_tc_h. */
 int fpd_weight_prep_f16(const float* w_oihw, void* w_hi, void* w_lo, int O, int I, int k, int for_dgrad,
@@ -109,7 +102,7 @@ int fpd_bn_finalize_sums(const double* part, int nblocks, const float* pivot, in
  * second stage and the module's finalize (affine + running statistics) run as one kernel (division-free fp64 merge), and
  * the channel sum can also return the operand scale of the 3xFP16 gradient convolutions: amax_scale (nullable float[2])
  * receives {S, 1/S} with S the power of two that puts max|dy| into [2^14, 2^15). `counter` is reserved (a single-launch
- * "last block finishes" variant measured slower on B200 and is disabled); pass a zeroed unsigned int or NULL.
+ * "last block finishes" variant measured slower and is disabled); pass a zeroed unsigned int or NULL.
  * Workspace sizes: fpd_channel_reduce_workspace_bytes / fpd_bn_stats_workspace_bytes.
  * Replace the per-channel sums of Conv2d bias backward, BatchNorm2d backward and BatchNorm2d train-mode forward
  * (lib/models/hourglass.py:18-26 modules under loss.backward(), lib/core/function.py:146). */
@@ -135,8 +128,7 @@ int fpd_conv2d_wgrad_tc_fused(const float* x, const float* pre_mean, const float
                               int W, int Cin, int Cout, int ksize, void* workspace, size_t workspace_bytes,
                               fpd_stream_t stream);
 
-/* 1 if fpd_conv2d_wgrad_tc_fused runs this 3x3 shape on the halo-tile kernel (csrc/wgrad_tc3.cu): x fetched once per
- * pixel block with its halo, taps = shifted start rows of the same shared-memory tile, all taps accumulated per CTA. */
+/* 1 if fpd_conv2d_wgrad_tc_fused takes this 3x3 shape in one launch (the same rule as fpd_conv2d_wgrad_tc_supported). */
 int fpd_conv2d_wgrad_tc3_supported(int H, int W, int Cin, int Cout, int ksize);
 
 /* Generic fp32 CUDA-core convolution (any k/stride/pad): x NHWC [B,H,W,Cin], w OIHW. */

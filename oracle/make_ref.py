@@ -18,7 +18,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 DST = os.path.join(HERE, "_ref")
 FILES = [
-    "lib/models/hourglass.py",      # Bottleneck / Hourglass / HourglassNet / get_pose_net (SURVEY 8 a1-a4)
+    "lib/models/hourglass.py",      # Bottleneck / Hourglass / HourglassNet / get_pose_net
     "lib/models/pose_hrnet.py",     # HRNet (a5-a7)
     "lib/models/pose_resnet.py",    # ResNet + deconv head (f4)
     "lib/core/loss.py",             # JointsMSELoss (a8)

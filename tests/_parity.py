@@ -50,8 +50,8 @@ def grad_report(ours, g32, g64, tag=None):
     """ours / g32 / g64: dict name -> gradient tensor. Per tensor: a = max|g - g64| for ours and for the fp32 oracle,
     normalised by max(max|g64_t|, 1e-6 * global max|g64|) -- the second term is an absolute floor for gradients that are
     EXACTLY zero in exact arithmetic (a conv bias in front of a train-mode BatchNorm: the fp64 value is ~1e-20, both fp32
-    evaluations leave ~1e-10 of cancellation noise, far below Adam's eps = 1e-8). Optionally appended to
-    gpurun_out/parity_report.jsonl for the profiles/ summary."""
+    evaluations leave ~1e-10 of cancellation noise, far below Adam's eps = 1e-8). With a tag and FPD_PARITY_REPORT set,
+    the report is appended to that file (one JSON line per call)."""
     gmax = max(float(v.abs().max()) for v in g64.values())
     rows = []
     n_o = n_3 = den = 0.0
@@ -69,18 +69,17 @@ def grad_report(ours, g32, g64, tag=None):
            "worst_ours": max(r[1] for r in rows), "worst_fp32": max(r[2] for r in rows),
            "q90_ours": _pct([r[1] for r in rows], 0.9), "q90_fp32": _pct([r[2] for r in rows], 0.9),
            "median_ratio": _pct(ratios, 0.5), "q90_ratio": _pct(ratios, 0.9), "worst_ratio": max(ratios), "rows": rows}
-    if tag is not None:
-        out = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "gpurun_out")
+    out = os.environ.get("FPD_PARITY_REPORT")
+    if tag is not None and out:
         try:
-            os.makedirs(out, exist_ok=True)
-            with open(os.path.join(out, "parity_report.jsonl"), "a") as fh:
+            with open(out, "a") as fh:
                 fh.write(json.dumps(rep) + "\n")
         except OSError:
             pass
     return rep
 
 
-# What "ill-conditioned" means here (measured on B200, profiles/r2_parity_report.md): wherever no ReLU decision differs,
+# What "ill-conditioned" means here (from per-tensor parity reports of the bench configurations): wherever no ReLU decision differs,
 # BOTH our gradients and the fp32 oracle's sit ~2e-5 from fp64 (ours slightly closer). But a network evaluation holds
 # ~1e6-1e8 pre-activations, and the handful that lie within round-off of zero get their ReLU mask decided differently by
 # any two finite-precision evaluations; ONE such flip at a low-resolution level (few pixels, each carrying a large share

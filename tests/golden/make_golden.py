@@ -1,9 +1,9 @@
 """Generate the golden vectors under tests/golden/ by running the REAL reference
 (/root/reference, read-only) on seeded synthetic inputs. Run in the build container only:
 
-    python tests/golden/make_golden.py
+    python tests/golden/make_golden.py [decode2 | resnet | layout]
 
-The reference has no tests / fixtures of its own (SURVEY.md section 4), so these vectors -- outputs of its
+The reference has no tests / fixtures of its own, so these vectors -- outputs of its
 own lib/models/hourglass.py, lib/core/loss.py, lib/core/inference.py, lib/utils/transforms.py and
 lib/nms/nms.py -- are what pins the oracle (tests/test_oracle.py) and, through it, the CUDA path.
 """
@@ -218,7 +218,45 @@ def main_resnet():
     print("resnet_small.npz", os.path.getsize(os.path.join(OUT, "resnet_small.npz")))
 
 
+def main_layout():
+    """layout.npz: what the drop-in modules are checked against without the reference present -- the reference
+    hourglass's outputs (train and eval mode) for seed 3 with a digest of its initial weights, and the pose_resnet
+    state_dict keys / shapes for every depth of resnet_spec."""
+    torch.set_num_threads(4)
+    save = {}
+    hg = load("ref_hg_live", "lib/models/hourglass.py")
+    torch.manual_seed(3)
+    net = hg.get_pose_net(cfg(64, 1), True)
+    save["hg/w_keys"] = np.array(list(net.state_dict().keys()))
+    save["hg/w_sums"] = np.array([v.double().abs().sum().item() for v in net.state_dict().values()])
+    x = torch.randn(2, 3, 64, 64)
+    save["hg/x"] = x.numpy()
+    for training in (True, False):
+        net.train(training)
+        with torch.no_grad():
+            save["hg/out_%s" % ("train" if training else "eval")] = net(x)[0].numpy()
+    R = load("ref_pose_resnet_t", "lib/models/pose_resnet.py")
+    save["resnet/spec_depths"] = np.array(sorted(R.resnet_spec))
+    save["resnet/spec_layers"] = np.array([list(R.resnet_spec[d][1]) for d in sorted(R.resnet_spec)])
+    sys.path[:0] = [os.path.join(OUT, ".."), os.path.join(OUT, "..", "..")]
+    from test_oracle import _resnet_cfg   # the configurations the test builds
+    cases = {"r18": _resnet_cfg("r18"), "r50": _resnet_cfg("r50")}
+    for depth in (34, 101, 152):          # the shipped d256x3 head on the remaining depths of resnet_spec
+        c = _resnet_cfg("r50")
+        c.MODEL.EXTRA.NUM_LAYERS = depth
+        c.MODEL.EXTRA.NUM_DECONV_FILTERS = [256, 256, 256]
+        cases["d%d" % depth] = c
+    for name, c in cases.items():
+        sd = R.get_pose_net(c, is_train=False).state_dict()
+        save["resnet/%s/keys" % name] = np.array(list(sd.keys()))
+        save["resnet/%s/shapes" % name] = np.array([list(v.shape) + [-1] * (4 - v.dim()) for v in sd.values()])
+    np.savez_compressed(os.path.join(OUT, "layout.npz"), **save)
+    print("layout.npz", os.path.getsize(os.path.join(OUT, "layout.npz")))
+
+
 def main():
+    if len(sys.argv) > 1 and sys.argv[1] == "layout":
+        return main_layout()
     if len(sys.argv) > 1 and sys.argv[1] == "decode2":
         return main_decode2()
     if len(sys.argv) > 1 and sys.argv[1] == "resnet":

@@ -48,16 +48,15 @@ def test_every_host_module_imports_on_cpu():
                  "lib.core.inference", "lib.core.evaluate", "lib.utils.transforms", "lib.nms.nms"):
         importlib.import_module("fpd_b200." + name)
     import ast
-    for script in ("bench.py", "__graft_entry__.py", "tools/profile_step.py", "tools/profile_kernel.py",
-                   "tools/profile_convs.py", "tools/diag_net.py", "tools/diag_grad.py",
-                   "tools/summarize_profiles.py", "tools/diag_conv_h.py", "tools/diag_wgrad.py", "tools/diag_wgrad3.py",
-                   "tools/diag_wgrad_shift.py", "tools/timeline_step.py"):
+    for script in ("bench.py", "__graft_entry__.py", "tools/profile_step.py", "tools/profile_convs.py",
+                   "tools/diag_net.py", "tools/diag_grad.py", "tools/diag_resnet_head.py", "tools/cpu_thread_sweep.py",
+                   "tools/timeline_step.py"):
         ast.parse(open(os.path.join(ROOT, script)).read(), script)
 
 
 def test_kernel_shape_planners_on_cpu():
-    """The support predicates of the generation-5 conv kernel and the halo weight-gradient kernel are pure host code
-    (shared-memory / TMEM plans): every shape of the BASELINE configs must be taken, the documented exceptions not."""
+    """The support predicates of the wgmma convolution and weight-gradient kernels are pure host code: every shape of
+    the BASELINE configs must be taken, the documented exceptions not."""
     import fpd_b200  # noqa: F401
     from fpd_b200 import _native as N
     lib = N.lib()
@@ -93,16 +92,17 @@ def test_kernel_shape_planners_on_cpu():
     assert ops.wgrad_channel_chunks(2048, 512, 1) == (256, 512)                # 1x1: any Cout, Cin <= 256 per launch
     assert ops.wgrad_channel_chunks(256, 1024, 1) == (256, 1024)
     assert ops.wgrad_channel_chunks(32, 17, 3) is None                         # 17-joint head: CUDA-core path
-    # halo weight-gradient kernel: 3x3, Cin in {64, 128}, W % 8 == 0, at least two pipeline stages must fit
-    for hw in (64, 32, 16, 8):
+    # 3x3 weight gradients: every shape the dispatcher sends to the tensor cores (3x3, Cin in {32, 64, 128}, Cout % 32 == 0
+    # up to 256), at any image size; other shapes do not
+    for hw in (64, 32, 16, 8, 4):
         assert lib.fpd_conv2d_wgrad_tc3_supported(hw, hw, 64, 64, 3) == 1
     assert lib.fpd_conv2d_wgrad_tc3_supported(64, 48, 64, 32, 3) == 1
-    assert lib.fpd_conv2d_wgrad_tc3_supported(4, 4, 64, 64, 3) == 0            # a K step must be 8 pixels along w
-    assert lib.fpd_conv2d_wgrad_tc3_supported(64, 64, 32, 32, 3) == 1          # Cin = 32: two taps per M = 64 instruction
-    assert lib.fpd_conv2d_wgrad_tc3_supported(64, 64, 32, 128, 3) == 0         # ... needs 5 x Cout <= 512 TMEM columns
-    assert lib.fpd_conv2d_wgrad_tc3_supported(64, 64, 16, 32, 3) == 0          # M = Cin must be 32, 64 or 128
-    assert lib.fpd_conv2d_wgrad_tc3_supported(64, 64, 64, 64, 1) == 0          # 1x1: wgrad_tc2
-    assert lib.fpd_conv2d_wgrad_tc3_supported(32, 32, 128, 128, 3) == 0        # one stage only: wgrad_tc2
+    assert lib.fpd_conv2d_wgrad_tc3_supported(64, 64, 32, 32, 3) == 1
+    assert lib.fpd_conv2d_wgrad_tc3_supported(64, 64, 32, 128, 3) == 1
+    assert lib.fpd_conv2d_wgrad_tc3_supported(32, 32, 128, 128, 3) == 1
+    assert lib.fpd_conv2d_wgrad_tc3_supported(64, 64, 16, 32, 3) == 0          # Cin must be 32, 64 or 128
+    assert lib.fpd_conv2d_wgrad_tc3_supported(64, 64, 64, 48, 3) == 0          # Cout % 32
+    assert lib.fpd_conv2d_wgrad_tc3_supported(64, 64, 64, 64, 1) == 0          # 1x1: not a 3x3 shape
     # workspace of the dispatching entry point covers whichever kernel runs
     assert lib.fpd_conv2d_wgrad_tc_workspace_bytes(32, 64, 64, 64, 64, 3) >= 9 * 64 * 64 * 4
 

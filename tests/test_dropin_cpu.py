@@ -77,7 +77,7 @@ SCRIPT = textwrap.dedent('''
                                                   NUM_JOINTS=16))
     net = models.hourglass.get_pose_net(c, is_train=True)
     assert "hg.0.hg.3.0.0.conv2.weight" in net.state_dict()
-    # checkpoint formats (SURVEY 8 f4): the reference's OWN save_checkpoint / load_checkpoint (utils/utils.py:74-86,
+    # checkpoint formats : the reference's OWN save_checkpoint / load_checkpoint (utils/utils.py:74-86,
     # 204-251: plain state_dict, DataParallel 'module.'-prefixed, and the {'state_dict': ...} training checkpoint, plus the
     # filter_keys partial load the FPD student uses) round-trip through the drop-in modules of all three families
     import os, tempfile, torch

@@ -70,7 +70,7 @@ def test_train_forward_backward_matches_reference_golden():
     assert abs(loss.item() - float(g["loss"])) < TOL * abs(float(g["loss"]))
     loss.backward()
     # Train-mode gradients of this network are ill-conditioned at the default init: the reference's own fp32
-    # gradients differ from an fp64 evaluation by up to 5e-2 per tensor (tools/diag_grad.py on B200), so the
+    # gradients differ from an fp64 evaluation by up to 5e-2 per tensor (tools/diag_grad.py), so the
     # whole-gradient relative L2 error is the meaningful check here; exact backward arithmetic is pinned per op in
     # test_ops_gpu.py and at network level in eval mode below.
     num = den = 0.0

@@ -1,6 +1,5 @@
-"""CPU suite (no GPU): pins the oracle (oracle/) against golden vectors produced by the real reference
-(tests/golden/make_golden.py) and -- when /root/reference exists -- against the live reference modules."""
-import importlib.util
+"""CPU suite (no GPU): pins the oracle (oracle/) and the drop-in modules against golden vectors produced by the real
+reference (tests/golden/make_golden.py)."""
 import os
 import sys
 import types
@@ -13,7 +12,6 @@ from oracle import decode_oracle as D
 from oracle import hourglass_oracle as O
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-REF = "/root/reference"
 
 
 def _load(name):
@@ -52,7 +50,7 @@ def test_oracle_forward_loss_grads_match_reference_golden(train_gold):
     worst = 0.0
     for k, p in params.items():
         worst = max(worst, _rel(p.grad, g["grad/" + k]))
-    assert worst < 2e-3, worst   # fp32 round-off through ~60 train-mode BN layers (see DESIGN.md on conditioning)
+    assert worst < 2e-3, worst   # fp32 round-off through ~60 train-mode BN layers (see the conditioning notes in tests/_parity.py)
     # running statistics are updated like nn.BatchNorm2d does
     assert _rel(sd["bn1.running_mean"], g["after/bn1.running_mean"]) < 1e-6
     assert _rel(sd["fc.1.1.running_var"], g["after/fc.1.1.running_var"]) < 1e-6
@@ -102,28 +100,29 @@ def test_decode_and_nms_match_reference_golden():
     assert D.nms(np.zeros((0, 5), np.float32), 0.5) == []
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="live reference only exists in the build container")
-def test_oracle_matches_live_reference_module():
+def test_oracle_matches_reference_module_golden():
+    """The reference hourglass (s1 f64) for seed 3, train and eval mode (tests/golden/layout.npz): the drop-in builds
+    its parameters in the reference's order, so the same seed gives the same weights (checked by a digest)."""
     torch.set_num_threads(4)
-    spec = importlib.util.spec_from_file_location("ref_hg_live", os.path.join(REF, "lib/models/hourglass.py"))
-    m = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(m)
+    import fpd_b200  # noqa: F401
+    from fpd_b200.lib.models import hourglass as H
+    g = _load("layout.npz")
     NS = types.SimpleNamespace
     cfg = NS(MODEL=NS(EXTRA=NS(NUM_FEATURES=64, NUM_STACKS=1, NUM_BLOCKS=1), NUM_JOINTS=16))
     torch.manual_seed(3)
-    net = m.get_pose_net(cfg, True)
-    x = torch.randn(2, 3, 64, 64)
-    for training in (True, False):
-        net.train(training)
-        sd = {k: v.clone() for k, v in net.state_dict().items()}
-        with torch.no_grad():
-            ref = net(x)
+    sd = {k: v.clone() for k, v in H.get_pose_net(cfg, True).state_dict().items()}
+    assert list(sd.keys()) == [str(k) for k in g["hg/w_keys"]]
+    sums = np.array([v.double().abs().sum().item() for v in sd.values()])
+    assert np.allclose(sums, g["hg/w_sums"], rtol=1e-6, atol=0)
+    x = torch.from_numpy(g["hg/x"])
+    for training, key in ((True, "hg/out_train"), (False, "hg/out_eval")):
+        with torch.no_grad():   # the train-mode pass updates the running statistics the eval-mode pass then uses
             got = O.hourglass_net(sd, x, num_stacks=1, training=training)
-        assert _rel(got[0], ref[0]) < 1e-5
+        assert _rel(got[0], g[key]) < 1e-5, key
 
 
 def test_dropin_module_state_dict_matches_reference_keys(train_gold):
-    """Boundary (SURVEY 8b): same state_dict keys/shapes as the reference => strict=True checkpoint loading."""
+    """Boundary: same state_dict keys/shapes as the reference => strict=True checkpoint loading."""
     import fpd_b200  # noqa: F401
     from fpd_b200.lib.models import hourglass as H
     NS = types.SimpleNamespace
@@ -253,30 +252,29 @@ def test_resnet_dropin_matches_reference_layout_and_refuses_cpu():
     assert type(net.deconv_layers[0]).__name__ == "ConvTranspose2d" and net.deconv_layers[0].bias is None
     with pytest.raises(RuntimeError, match="no CPU fallback|CUDA"):
         net(torch.zeros(1, 3, 64, 64))
-    if os.path.isdir(REF):        # live reference: every depth of resnet_spec has the same keys / shapes
-        spec = importlib.util.spec_from_file_location("ref_pose_resnet_t", os.path.join(REF, "lib/models/pose_resnet.py"))
-        R = importlib.util.module_from_spec(spec)
-        spec.loader.exec_module(R)
-        from fpd_b200.lib.models import pose_resnet as M
-        assert {k: v[1] for k, v in M.resnet_spec.items()} == {k: v[1] for k, v in R.resnet_spec.items()}
-        for tag in ("r18", "r50"):
-            a = R.get_pose_net(_resnet_cfg(tag), is_train=False).state_dict()
-            b = M.get_pose_net(_resnet_cfg(tag), is_train=False).state_dict()
-            assert list(a.keys()) == list(b.keys()) and all(a[k].shape == b[k].shape for k in a)
-        for depth in (34, 101, 152):          # the shipped d256x3 head on the remaining depths of resnet_spec
-            cfg = _resnet_cfg("r50")
-            cfg.MODEL.EXTRA.NUM_LAYERS = depth
-            cfg.MODEL.EXTRA.NUM_DECONV_FILTERS = [256, 256, 256]
-            a = R.get_pose_net(cfg, is_train=False).state_dict()
-            b = M.get_pose_net(cfg, is_train=False).state_dict()
-            assert list(a.keys()) == list(b.keys()) and all(a[k].shape == b[k].shape for k in a), depth
-        # init_weights without a checkpoint (pose_resnet.py:229-247): N(0, 0.001) convs / deconvs, unit BatchNorm
-        cfg = _resnet_cfg("r18")
-        cfg.MODEL.INIT_WEIGHTS = True
-        net = M.get_pose_net(cfg, is_train=True)
-        assert 5e-4 < net.layer2[0].conv1.weight.std().item() < 2e-3
-        assert 5e-4 < net.deconv_layers[0].weight.std().item() < 2e-3 and float(net.deconv_layers[0].bias.detach().abs().max()) == 0.0
-        assert torch.equal(net.deconv_layers[1].weight, torch.ones_like(net.deconv_layers[1].weight))
+    # every depth of resnet_spec has the reference's keys / shapes (tests/golden/layout.npz)
+    from fpd_b200.lib.models import pose_resnet as M
+    g = _load("layout.npz")
+    assert sorted(M.resnet_spec) == g["resnet/spec_depths"].tolist()
+    assert [list(M.resnet_spec[d][1]) for d in sorted(M.resnet_spec)] == g["resnet/spec_layers"].tolist()
+    cases = {"r18": _resnet_cfg("r18"), "r50": _resnet_cfg("r50")}
+    for depth in (34, 101, 152):          # the shipped d256x3 head on the remaining depths of resnet_spec
+        cfg = _resnet_cfg("r50")
+        cfg.MODEL.EXTRA.NUM_LAYERS = depth
+        cfg.MODEL.EXTRA.NUM_DECONV_FILTERS = [256, 256, 256]
+        cases["d%d" % depth] = cfg
+    for name, cfg in cases.items():
+        b = M.get_pose_net(cfg, is_train=False).state_dict()
+        assert list(b.keys()) == [str(k) for k in g["resnet/%s/keys" % name]], name
+        shapes = [list(v.shape) + [-1] * (4 - v.dim()) for v in b.values()]
+        assert shapes == g["resnet/%s/shapes" % name].tolist(), name
+    # init_weights without a checkpoint (pose_resnet.py:229-247): N(0, 0.001) convs / deconvs, unit BatchNorm
+    cfg = _resnet_cfg("r18")
+    cfg.MODEL.INIT_WEIGHTS = True
+    net = M.get_pose_net(cfg, is_train=True)
+    assert 5e-4 < net.layer2[0].conv1.weight.std().item() < 2e-3
+    assert 5e-4 < net.deconv_layers[0].weight.std().item() < 2e-3 and float(net.deconv_layers[0].bias.detach().abs().max()) == 0.0
+    assert torch.equal(net.deconv_layers[1].weight, torch.ones_like(net.deconv_layers[1].weight))
 
 
 @pytest.mark.parametrize("k,pad,outpad", [(4, 1, 0), (3, 1, 1), (2, 0, 0)])

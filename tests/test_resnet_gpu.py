@@ -217,7 +217,7 @@ def test_resnet_forward_matches_oracle_at_shipped_sizes(layers, J, H, W, trainin
     assert tuple(got.shape) == (2, J, H // 4, W // 4)
     if P.rel_max(got, ref) < TOL:
         return
-    with torch.no_grad():     # fp64 on the host cores (seconds; B200's fp64 convolutions take minutes at this size)
+    with torch.no_grad():     # fp64 on the host cores (seconds; the GPU's fp64 convolutions take minutes at this size)
         ref64 = RO.resnet(P.cast_sd(sd, torch.float64, device="cpu"), x.double().cpu(), training=training)
     # 1e-3 of the reference's fp32 result (north_star), or -- where batch statistics over 2 x 8 x 6 values per channel
     # through 33 blocks put the reference's own fp32 arithmetic further than that from the exact result (ResNet-101) --

@@ -1,7 +1,7 @@
-"""Thread-count sweep of the CPU legs (the reference's own modules, oracle/_ref) on the GPU box's host, so that
+"""Thread-count sweep of the CPU legs (the reference's own modules, oracle/_ref) on the GPU host, so that
 `cpu_baseline` / `--impl reference` use the thread count the reference actually runs fastest with on that machine.
 
-    python tools/cpu_thread_sweep.py > gpurun_out/cpu_thread_sweep.txt      # summarised in profiles/r2_cpu_thread_sweep.txt
+    python tools/cpu_thread_sweep.py > cpu_thread_sweep.txt
 """
 import os
 import subprocess

@@ -1,4 +1,4 @@
-"""Gradient parity report on a GPU box: worst per-parameter relative error (max|d|/max|ref|) of the CUDA path's
+"""Gradient parity report on a GPU host: worst per-parameter relative error (max|d|/max|ref|) of the CUDA path's
 parameter gradients vs the oracle in fp64, next to the oracle's own fp32-vs-fp64 noise floor."""
 import os
 import sys

@@ -1,4 +1,4 @@
-"""Error report for the network-level parity on a GPU box: per-stack relative error of the CUDA path vs the
+"""Error report for the network-level parity on a GPU host: per-stack relative error of the CUDA path vs the
 oracle (fp32 and fp64), plus the oracle-fp32-vs-fp64 noise floor, for several configs / precision modes."""
 import os
 import sys

@@ -60,7 +60,7 @@ def main():
             out.append("  %8.1f us %5.1f%% x%-3d avg %7.1f us  in[%d,%d,%d,%d] Cout=%d k=%d  %.1f GF/launch -> %.0f TF/s alg" % (
                 v[1], 100 * v[1] / tot, v[0], v[1] / v[0], B, Hh, Ww, Cin, Cout, k, gf, gf / (v[1] / v[0]) * 1e-3 * 1e3))
     text = "\n".join(out)
-    path = os.path.join(ROOT, "gpurun_out", "profile_convs.txt")
+    path = os.path.join(ROOT, "profile_out", "profile_convs.txt")
     os.makedirs(os.path.dirname(path), exist_ok=True)
     open(path, "w").write(text + "\n")
     print(text)

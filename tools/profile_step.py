@@ -2,7 +2,7 @@
 
     python tools/profile_step.py                 # torch.profiler (CUPTI) table, warm caches
     ncu --metrics gpu__time_duration.sum --clock-control none --profile-from-start off --csv \
-        --log-file gpurun_out/launches.csv python tools/profile_step.py --ncu      # launch list for profiles/
+        --log-file profile_out/launches.csv python tools/profile_step.py --ncu      # per-launch kernel durations
 """
 import argparse
 import os
@@ -20,7 +20,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--ncu", action="store_true")
     ap.add_argument("--batch", type=int, default=32)
-    ap.add_argument("--out", default=os.path.join(ROOT, "gpurun_out", "profile_step.txt"))
+    ap.add_argument("--out", default=os.path.join(ROOT, "profile_out", "profile_step.txt"))
     args = ap.parse_args()
     import fpd_b200  # noqa: F401
     from fpd_b200.lib.models import hourglass as H

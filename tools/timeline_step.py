@@ -3,10 +3,10 @@ SMs the resident kernels can cover, and where the step's wall time goes.
 
     python tools/timeline_step.py [--batch 32] [--tag r2a]
 
-Writes gpurun_out/timeline_<tag>.csv.gz (name, stream, start_us, dur_us, grid) and gpurun_out/timeline_<tag>.txt:
+Writes profile_out/timeline_<tag>.csv.gz (name, stream, start_us, dur_us, grid) and profile_out/timeline_<tag>.txt:
   * span of the step, per-stream busy time,
-  * "SM cover": integral over time of min(148, sum of grid sizes of the kernels running) / (148 x span) -- an upper
-    bound on how much of the chip the launched grids could occupy (persistent kernels: grid <= 148),
+  * "SM cover": integral over time of min(132, sum of grid sizes of the kernels running) / (132 x span) -- an upper
+    bound on how much of the chip the launched grids could occupy (persistent kernels: grid <= 132),
   * time split by how many SMs the running kernels cover (<25 %, 25-50 %, 50-100 %, full),
   * per kernel family: launches, summed duration, duration-weighted mean grid.
 CUPTI timestamps under a profiler: use the SHARES, not the absolute step time (bench.py is the step time)."""
@@ -75,7 +75,7 @@ def main():
     t0 = ev[0][0]
     t1 = max(s + d for s, d, _, _, _ in ev)
     span = t1 - t0
-    out_dir = os.path.join(ROOT, "gpurun_out")
+    out_dir = os.path.join(ROOT, "profile_out")
     os.makedirs(out_dir, exist_ok=True)
     with gzip.open(os.path.join(out_dir, "timeline_%s.csv.gz" % args.tag), "wt") as fh:
         fh.write("name,stream,start_us,dur_us,grid\n")
@@ -95,9 +95,9 @@ def main():
     for tt, dg, dn in pts:
         dt = tt - last
         if dt > 0:
-            c = min(148, cur_g)
+            c = min(132, cur_g)
             cover += dt * c
-            k = "idle" if cur_n == 0 else "<25%" if c < 37 else "25-50%" if c < 74 else "50-100%" if c < 148 else "full"
+            k = "idle" if cur_n == 0 else "<25%" if c < 33 else "25-50%" if c < 66 else "50-100%" if c < 132 else "full"
             buckets[k] += dt
             conc[min(cur_n, 6)] += dt
         cur_g += dg
@@ -110,18 +110,18 @@ def main():
         f = fam[short(n)]
         f[0] += 1
         f[1] += d
-        f[2] += d * min(g, 148)
-        f[3] += 1 if g < 148 else 0
+        f[2] += d * min(g, 132)
+        f[3] += 1 if g < 132 else 0
     lines = []
     lines.append("config %s" % args.config)
     lines.append("one %s FPD step, B=%d: %d kernels, span %.3f ms, summed kernel time %.3f ms" % (
         "eager" if args.eager else "graph-replayed", args.batch, len(ev), span / 1e3, sum(e[1] for e in ev) / 1e3))
-    lines.append("SM cover (time-integral of min(148, sum of running grids)) = %.3f of 148 x span" % (cover / (148 * span)))
+    lines.append("SM cover (time-integral of min(132, sum of running grids)) = %.3f of 132 x span" % (cover / (132 * span)))
     lines.append("time by SM cover of the running kernels: " + ", ".join("%s %.2f ms" % (k, v / 1e3) for k, v in buckets.items()))
     lines.append("time by number of concurrently running kernels: " + ", ".join(
         "%s%d: %.2f ms" % (">=" if k == 6 else "", k, v / 1e3) for k, v in sorted(conc.items())))
     lines.append("per stream busy ms: " + ", ".join("s%d %.2f" % (k, v / 1e3) for k, v in sorted(streams.items(), key=lambda kv: -kv[1])))
-    lines.append("%-58s %6s %9s %9s %7s" % ("kernel", "n", "sum ms", "mean grid", "n<148"))
+    lines.append("%-58s %6s %9s %9s %7s" % ("kernel", "n", "sum ms", "mean grid", "n<132"))
     for k, f in sorted(fam.items(), key=lambda kv: -kv[1][1]):
         lines.append("%-58s %6d %9.3f %9.1f %7d" % (k, f[0], f[1] / 1e3, f[2] / max(f[1], 1e-9), f[3]))
     txt = "\n".join(lines)
