@@ -14,7 +14,7 @@ OUT = os.path.join(HERE, "libfpd_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
          "--expt-relaxed-constexpr", "-Xptxas", "-v"]
-SOURCES = ["api.cu", "conv_wgmma.cu", "conv_simt.cu", "elementwise.cu", "loss.cu", "decode.cu", "nms.cu", "adam.cu"]
+SOURCES = ["api.cu", "conv_wgmma.cu", "conv_simt.cu", "elementwise.cu", "loss.cu", "decode.cu", "nms.cu", "adam.cu", "augment.cu"]
 
 
 def _newer(a, b):

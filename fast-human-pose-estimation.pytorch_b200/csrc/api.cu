@@ -353,6 +353,13 @@ int fpd_gaussian_targets(const float* joints, const float* joints_vis, const flo
                           image_h, sigma, S(stream));
 }
 
+int fpd_crop_affine_normalize(const uint8_t* src, size_t src_bytes, const int64_t* desc, const double* inv,
+                              const int64_t* desc_host, const double* inv_host, const float* mean_std_host, float* out,
+                              int N, int out_h, int out_w, fpd_stream_t stream) {
+  return crop_affine_normalize(src, src_bytes, desc, inv, desc_host, inv_host, mean_std_host, out, N, out_h, out_w,
+                               S(stream));
+}
+
 int fpd_adam_flat(float* param, const float* grad, float* m, float* v, int64_t n, float lr, float b1, float b2,
                   float eps, float wd, int step, float grad_scale, fpd_stream_t stream) {
   return adam_flat(param, grad, m, v, n, lr, b1, b2, eps, wd, step, grad_scale, S(stream));

@@ -179,6 +179,15 @@ int gaussian_targets(const float* joints, const float* joints_vis, const float* 
                      float* target, float* target_weight, int N, int J, int H, int W, int image_w, int image_h, int sigma,
                      cudaStream_t stream);
 
+// ---- augment.cu ----
+// Affine crop + ToTensor/Normalize of N uint8 HWC source regions packed in src (see fpd_crop_affine_normalize):
+// desc int64 [N, kCropDescLen], inv float64 [N, 6] on the device, the same arrays on the host for validation,
+// mean_std_host = {mean[3], std[3]}; out fp32 [N, 3, out_h, out_w].
+constexpr int kCropDescLen = 7;   // byte offset, region x, y, w, h, image w, h
+int crop_affine_normalize(const uint8_t* src, size_t src_bytes, const int64_t* desc, const double* inv,
+                          const int64_t* desc_host, const double* inv_host, const float* mean_std_host, float* out, int N,
+                          int out_h, int out_w, cudaStream_t stream);
+
 // ---- adam.cu ----
 int adam_flat(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, int64_t n, float lr, float beta1,
               float beta2, float eps, float weight_decay, int step, float grad_scale, cudaStream_t stream);

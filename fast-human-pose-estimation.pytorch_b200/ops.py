@@ -661,26 +661,68 @@ def oks_rescore(kpts, box_score, in_vis_thre):
     return out
 
 
+def gaussian_table(sigma, device):
+    """The un-normalised Gaussian patch gaussian_targets stamps, as a device tensor [(6 sigma + 1)^2]."""
+    import numpy as np
+    # the reference's own expression (float32 numpy), so the stamped patch is bit-identical: JointsDataset.py:266-272
+    size = 2 * (sigma * 3) + 1
+    xs = np.arange(0, size, 1, np.float32)
+    ys = xs[:, np.newaxis]
+    x0 = y0 = size // 2
+    g = np.exp(- ((xs - x0) ** 2 + (ys - y0) ** 2) / (2 * sigma ** 2))
+    return torch.from_numpy(np.ascontiguousarray(g, dtype=np.float32)).to(device)
+
+
 def gaussian_targets(joints, joints_vis, heatmap_size, image_size, sigma=2, joints_weight=None, gauss_table=None):
     """Batch form of JointsDataset.generate_target (lib/dataset/JointsDataset.py:233-289). joints / joints_vis: CUDA float32
     [N,J,3]; heatmap_size / image_size: (w, h). Returns (target [N,J,h,w], target_weight [N,J,1])."""
-    import numpy as np
     _chk(joints, "joints")
     _chk(joints_vis, "joints_vis")
     n, J = joints.shape[0], joints.shape[1]
     W, H = int(heatmap_size[0]), int(heatmap_size[1])
     dev = joints.device
     if gauss_table is None:
-        # the reference's own expression (float32 numpy), so the stamped patch is bit-identical: JointsDataset.py:266-272
-        size = 2 * (sigma * 3) + 1
-        xs = np.arange(0, size, 1, np.float32)
-        ys = xs[:, np.newaxis]
-        x0 = y0 = size // 2
-        g = np.exp(- ((xs - x0) ** 2 + (ys - y0) ** 2) / (2 * sigma ** 2))
-        gauss_table = torch.from_numpy(np.ascontiguousarray(g, dtype=np.float32)).to(dev)
+        gauss_table = gaussian_table(sigma, dev)
     target = torch.empty((n, J, H, W), dtype=torch.float32, device=dev)
     tw = torch.empty((n, J, 1), dtype=torch.float32, device=dev)
     jw = None if joints_weight is None else joints_weight.to(dev).float().contiguous().reshape(-1)
     N.check(N.lib().fpd_gaussian_targets(_p(joints), _p(joints_vis), _p(jw), _p(gauss_table), _p(target), _p(tw), n, J, H, W,
                                          int(image_size[0]), int(image_size[1]), int(sigma), _stream()), "gaussian_targets")
     return target, tw
+
+
+CROP_DESC_LEN = 7   # desc columns: byte offset, region x, y, w, h, image w, h (include/fpd_b200.h)
+
+
+def crop_affine_normalize(src, desc, inv, out_size, mean, std, desc_host=None, inv_host=None, out=None):
+    """Batched cv2.warpAffine(INTER_LINEAR, BORDER_CONSTANT=0) + ToTensor + Normalize, bit-exact (fpd_crop_affine_normalize).
+    src: CUDA uint8 buffer of packed HWC regions; desc: CUDA int64 [N,7]; inv: CUDA float64 [N,6] (or [N,2,3]) inverse
+    matrices; out_size: (w, h); mean / std: 3 values each. desc_host / inv_host: CPU copies of desc / inv (the arguments
+    are validated on the host; when omitted they are copied back, which synchronises). Returns out fp32 [N,3,h,w]."""
+    import numpy as np
+    W, H = int(out_size[0]), int(out_size[1])
+    if not (src.is_cuda and src.dtype == torch.uint8 and src.is_contiguous()):
+        raise ValueError("src must be a contiguous uint8 CUDA tensor")
+    if not (desc.is_cuda and desc.dtype == torch.int64 and desc.is_contiguous() and desc.dim() == 2
+            and desc.shape[1] == CROP_DESC_LEN):
+        raise ValueError("desc must be a contiguous int64 CUDA tensor [N, %d]" % CROP_DESC_LEN)
+    n = desc.shape[0]
+    if not (inv.is_cuda and inv.dtype == torch.float64 and inv.is_contiguous() and inv.numel() == 6 * n):
+        raise ValueError("inv must be a contiguous float64 CUDA tensor [N, 6]")
+    desc_host = (desc if desc_host is None else desc_host).cpu().contiguous()
+    inv_host = (inv if inv_host is None else inv_host).cpu().contiguous()
+    if desc_host.dtype != torch.int64 or desc_host.shape != desc.shape or inv_host.dtype != torch.float64 \
+            or inv_host.numel() != inv.numel():
+        raise ValueError("desc_host / inv_host must match desc / inv")
+    ms = np.ascontiguousarray(np.concatenate([np.asarray(mean, np.float32).reshape(3),
+                                              np.asarray(std, np.float32).reshape(3)]))
+    if out is None:
+        out = torch.empty((n, 3, max(H, 0), max(W, 0)), dtype=torch.float32, device=src.device)
+    else:
+        _chk(out, "out")
+        if tuple(out.shape) != (n, 3, H, W):
+            raise ValueError("out must be [N, 3, h, w] = %s" % ((n, 3, H, W),))
+    N.check(N.lib().fpd_crop_affine_normalize(_p(src) if src.numel() else None, src.numel(), _p(desc), _p(inv),
+                                              _p(desc_host), _p(inv_host), ms.ctypes.data_as(ctypes.c_void_p), _p(out), n,
+                                              H, W, _stream()), "crop_affine_normalize")
+    return out

@@ -17,9 +17,13 @@ class TargetGenerator:
         self.device = torch.device(device)
         self.joints_weight = None if joints_weight is None else torch.as_tensor(joints_weight, dtype=torch.float32).to(
             self.device)
+        self.gauss_table = None   # built on first use; kept so that calls on device tensors copy nothing (graph capture)
 
     def __call__(self, joints, joints_vis):
         """joints, joints_vis: [B,J,3] (CUDA or host tensors / arrays) -> (target [B,J,h,w], target_weight [B,J,1]) on the device."""
         j = torch.as_tensor(joints, dtype=torch.float32).to(self.device, non_blocking=True).contiguous()
         v = torch.as_tensor(joints_vis, dtype=torch.float32).to(self.device, non_blocking=True).contiguous()
-        return ops.gaussian_targets(j, v, self.heatmap_size, self.image_size, self.sigma, self.joints_weight)
+        if self.gauss_table is None:
+            self.gauss_table = ops.gaussian_table(self.sigma, self.device)
+        return ops.gaussian_targets(j, v, self.heatmap_size, self.image_size, self.sigma, self.joints_weight,
+                                    self.gauss_table)

@@ -303,6 +303,22 @@ int fpd_gaussian_targets(const float* joints, const float* joints_vis, const flo
                          int sigma, fpd_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------
+ * Input crop. Replaces the per-sample cv2.warpAffine(INTER_LINEAR) + ToTensor + Normalize of
+ * lib/dataset/JointsDataset.py:177-184 (transform of tools/fpd_train.py:182-184) for a whole batch, bit-exact with
+ * cv2 4.x on 8-bit images and torchvision's two fp32 divisions.
+ * src: device uint8, src_bytes long, holding per sample a packed HWC 3-channel region of its source image (already
+ * mirrored / in the channel order the model wants). desc: device int64[N,7] = {byte offset into src, region x, region y,
+ * region w, region h, image w, image h}; the region must hold every pixel of the image the crop reads (taps outside the
+ * image read 0). inv: device double[N,6], the row-major 2x3 map from output to image coordinates
+ * (cv2.invertAffineTransform of the forward matrix). desc_host / inv_host: the same arrays in host memory, checked before
+ * the launch (region bounds, and matrices whose 1/1024-pixel fixed-point coordinates would overflow int32 are refused);
+ * mean_std_host: host float[6] = {mean[3], std[3]}. out: device float[N,3,out_h,out_w]. N = 0 does nothing.
+ * ------------------------------------------------------------------------------------------------- */
+int fpd_crop_affine_normalize(const uint8_t* src, size_t src_bytes, const int64_t* desc, const double* inv,
+                              const int64_t* desc_host, const double* inv_host, const float* mean_std_host, float* out,
+                              int N, int out_h, int out_w, fpd_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------------
  * Optimizer. Replaces torch.optim.Adam as configured by lib/utils/utils.py:69-73, stepped at
  * lib/core/function.py:147, over one flat parameter buffer.
  * ------------------------------------------------------------------------------------------------- */
