@@ -14,6 +14,8 @@
 //   Split operands: acc += A_lo * B_hi + A_hi * B_lo + A_hi * B_hi (the lo * lo term is below fp32 rounding).
 //   Optional epilogue statistics: per output channel {sum (y - pivot), sum (y - pivot)^2} in fp64, per-warp shared
 //   accumulators merged in a fixed order (deterministic), one [Cout][2] block per CTA for bn_finalize_sums.
+//   3x3 with 3xFP16 operands (conv_halo_kernel, selected by conv_launch where it fits in shared memory): the same GEMM
+//   with the A operand of a tile loaded and transformed once into a halo in shared memory and fed from registers.
 //
 // Weight gradient (wgrad_tc_*):
 //   dW[co][ci][tap] = scale * sum_{pixels p} dY[p][co] * A[p (+) tap][ci],  A = relu?((x - mean) * scale + shift)
@@ -156,31 +158,117 @@ struct ConvParams {
   const float* in_scale;       // nullable device float[2] {S, 1/S}: operands are x * S, the epilogue multiplies by 1/S
   double* stat_part;           // nullable [gridDim.x][Cout][2] = {sum (y - pivot), sum (y - pivot)^2}
   const float* stat_pivot;     // nullable [Cout]
+  int halo_rows;               // conv_halo_kernel: kTileM + 2 W + 2 pixel rows + one zero row per channel block
 };
+
+// Weights of K step ks for output columns [n0, n0 + nt): nt K-major rows of 128 bytes (one tap, kCB input channels)
+// under the 128-byte swizzle, hi at `b`, lo at `b + b_lo_off`, by cp.async (one commit group); channels >= Cin are zeros.
+template <bool kF16>
+__device__ __forceinline__ void conv_load_b(const ConvParams& p, int ks, int n0, uint32_t b, uint32_t b_lo_off) {
+  constexpr int kCB = kF16 ? 64 : 32;
+  constexpr int kChunkEl = kF16 ? 8 : 4;    // weight elements per 16-byte chunk
+  constexpr int kEl = kF16 ? 2 : 4;
+  const bool split = p.passes == 3;
+  const char* wh = reinterpret_cast<const char*>(p.w_hi);
+  const char* wl = reinterpret_cast<const char*>(p.w_lo ? p.w_lo : p.w_hi);
+  const int tap = ks / p.ncb, cb = ks - tap * p.ncb;
+  for (int idx = threadIdx.x; idx < p.nt * 8; idx += kThreads) {
+    const int n = idx >> 3, jj = idx & 7;
+    const int c = cb * kCB + jj * kChunkEl;
+    const bool ok = c < p.Cin;
+    const size_t off = ((((size_t)tap * p.Cout + n0 + n) * p.Cin) + (ok ? c : 0)) * kEl;
+    const uint32_t dst = b + (uint32_t)n * 128u + ((uint32_t)(jj ^ (n & 7)) << 4);
+    cp_async16(dst, wh + off, ok);
+    if (split) cp_async16(dst + b_lo_off, wl + off, ok);
+  }
+  cp_async_commit();
+}
+
+__device__ __forceinline__ void conv_stats_init(const ConvParams& p, double* s_stat) {
+  if (p.stat_part) {
+    for (int i = threadIdx.x; i < 8 * p.Cout * 2; i += kThreads) s_stat[i] = 0.0;
+  }
+}
+
+// Epilogue of one 128 x kN tile: y = acc * oscale (+ bias) (+ residual) (ReLU mask), and the per-warp fp64 statistics.
+// Fragment row g (+8), columns 8 i + 2 t (+1) of this warp's 16 rows.
+template <int kN>
+__device__ __forceinline__ void conv_epilogue(const ConvParams& p, const float (&acc)[kN / 2], int m0, int n0,
+                                              float oscale, double* s_stat) {
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
+  const bool stats = p.stat_part != nullptr;
+  const int g = lane >> 2, t = lane & 3;
+  const int mrow = m0 + wg * 64 + (warp & 3) * 16 + g;
+  double* my_stat = s_stat + (size_t)warp * p.Cout * 2;
+#pragma unroll
+  for (int i = 0; i < kN / 8; ++i) {
+    const int col = n0 + i * 8 + 2 * t;
+    float2 b2 = make_float2(0.f, 0.f), pv = make_float2(0.f, 0.f);
+    if (p.bias) b2 = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+    if (stats && p.stat_pivot) pv = __ldg(reinterpret_cast<const float2*>(p.stat_pivot + col));
+    double s1a = 0.0, s1b = 0.0, s2a = 0.0, s2b = 0.0;
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+      const int m = mrow + rr * 8;
+      if (m >= p.P) continue;
+      const size_t off = (size_t)m * p.Cout + col;
+      float2 o = make_float2(acc[4 * i + 2 * rr] * oscale + b2.x, acc[4 * i + 2 * rr + 1] * oscale + b2.y);
+      if (p.residual) {
+        const float2 r2 = __ldg(reinterpret_cast<const float2*>(p.residual + off));
+        o.x += r2.x; o.y += r2.y;
+      }
+      if (p.relu_mask) {
+        const float2 k = __ldg(reinterpret_cast<const float2*>(p.relu_mask + off));
+        o.x = k.x > 0.f ? o.x : 0.f; o.y = k.y > 0.f ? o.y : 0.f;
+      }
+      *reinterpret_cast<float2*>(p.y + off) = o;
+      if (stats) {
+        const double d0 = (double)(o.x - pv.x), d1 = (double)(o.y - pv.y);
+        s1a += d0; s2a += d0 * d0; s1b += d1; s2b += d1 * d1;
+      }
+    }
+    if (stats) {
+#pragma unroll
+      for (int sh = 4; sh < 32; sh <<= 1) {
+        s1a += __shfl_xor_sync(0xffffffffu, s1a, sh); s2a += __shfl_xor_sync(0xffffffffu, s2a, sh);
+        s1b += __shfl_xor_sync(0xffffffffu, s1b, sh); s2b += __shfl_xor_sync(0xffffffffu, s2b, sh);
+      }
+      if (g == 0) {   // lanes 0..3 own two distinct columns each: no conflicts, no atomics
+        my_stat[(size_t)col * 2 + 0] += s1a; my_stat[(size_t)col * 2 + 1] += s2a;
+        my_stat[(size_t)col * 2 + 2] += s1b; my_stat[(size_t)col * 2 + 3] += s2b;
+      }
+    }
+  }
+}
+
+// One [Cout][2] statistics block per CTA: the eight per-warp accumulators merged in a fixed order (deterministic).
+__device__ __forceinline__ void conv_stats_flush(const ConvParams& p, const double* s_stat) {
+  if (p.stat_part) {
+    __syncthreads();
+    for (int i = threadIdx.x; i < p.Cout * 2; i += kThreads) {
+      double v = 0.0;
+      for (int w8 = 0; w8 < 8; ++w8) v += s_stat[(size_t)w8 * p.Cout * 2 + i];   // fixed order
+      p.stat_part[(size_t)blockIdx.x * p.Cout * 2 + i] = v;
+    }
+  }
+}
 
 template <bool kF16, int kN>
 __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const ConvParams p) {
   constexpr int kCB = kF16 ? 64 : 32;       // input channels per K step (one 128-byte operand row)
   constexpr int kV = kF16 ? 2 : 1;          // raw float4 per thread, row and K step
-  constexpr int kChunkEl = kF16 ? 8 : 4;    // weight elements per 16-byte chunk
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   double* s_stat = reinterpret_cast<double*>(smem + (size_t)kStages * p.stage_bytes);
   const uint32_t smem_a = smem_u32(smem);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
+  const int tid = threadIdx.x, wg = tid >> 7;
   const bool split = p.passes == 3;
-  const bool stats = p.stat_part != nullptr;
   const float in_s = p.in_scale ? __ldg(p.in_scale) : 1.f;
   const float oscale = p.in_scale ? p.out_scale * __ldg(p.in_scale + 1) : p.out_scale;
   const uint32_t a_lo_off = split ? (uint32_t)kATileBytes : 0u;
   const uint32_t b_off = (split ? 2u : 1u) * (uint32_t)kATileBytes;
   const uint32_t b_lo_off = split ? (uint32_t)p.b_tile_bytes : 0u;
-  const char* wh = reinterpret_cast<const char*>(p.w_hi);
-  const char* wl = reinterpret_cast<const char*>(p.w_lo ? p.w_lo : p.w_hi);
-  constexpr int kEl = kF16 ? 2 : 4;
-  if (stats) {
-    for (int i = tid; i < 8 * p.Cout * 2; i += kThreads) s_stat[i] = 0.0;
-  }
+  conv_stats_init(p, s_stat);
   __syncthreads();
 
   // A tile: thread -> 16-byte chunk j of rows r0 + 32 i
@@ -250,25 +338,11 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const ConvParam
         if (split) sts128u(dst + a_lo_off, ol);
       }
     };
-    auto load_b = [&](int ks, uint32_t st) {
-      const int tap = ks / p.ncb, cb = ks - tap * p.ncb;
-      for (int idx = tid; idx < p.nt * 8; idx += kThreads) {
-        const int n = idx >> 3, jj = idx & 7;
-        const int c = cb * kCB + jj * kChunkEl;
-        const bool ok = c < p.Cin;
-        const size_t off = ((((size_t)tap * p.Cout + n0 + n) * p.Cin) + (ok ? c : 0)) * kEl;
-        const uint32_t dst = st + b_off + (uint32_t)n * 128u + ((uint32_t)(jj ^ (n & 7)) << 4);
-        cp_async16(dst, wh + off, ok);
-        if (split) cp_async16(dst + b_lo_off, wl + off, ok);
-      }
-      cp_async_commit();
-    };
-
     // one partial for all terms here: a separate cross-term partial would push the fp16 N = 128 form past 255 registers
     float acc[kN / 2], part[kN / 2];
     zero_acc(acc);
     zero_acc(part);
-    load_b(0, smem_a);
+    conv_load_b<kF16>(p, 0, n0, smem_a + b_off, b_lo_off);
     load_a(0);
     for (int ks = 0; ks < p.ksteps; ++ks) {
       const uint32_t st = smem_a + (uint32_t)((ks % kStages) * p.stage_bytes);
@@ -281,7 +355,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const ConvParam
       fence_proxy_async_smem();
       __syncthreads();
       if (ks + 1 < p.ksteps) {
-        load_b(ks + 1, smem_a + (uint32_t)(((ks + 1) % kStages) * p.stage_bytes));
+        conv_load_b<kF16>(p, ks + 1, n0, smem_a + (uint32_t)(((ks + 1) % kStages) * p.stage_bytes) + b_off, b_lo_off);
         load_a(ks + 1);
       }
       wgmma_fence();
@@ -293,58 +367,162 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const ConvParam
     add_part(acc, part);
     __syncthreads();   // every warpgroup is done with every stage: the next tile may refill them
 
-    // ---- epilogue: fragment row g (+8), columns 8 i + 2 t (+1) of this warp's 16 rows ----
-    const int g = lane >> 2, t = lane & 3;
-    const int mrow = m0 + wg * 64 + (warp & 3) * 16 + g;
-    double* my_stat = s_stat + (size_t)warp * p.Cout * 2;
+    conv_epilogue<kN>(p, acc, m0, n0, oscale, s_stat);
+  }
+  conv_stats_flush(p, s_stat);
+}
+
+// ================================================ forward, 3x3 halo ================================================
+// conv_halo_kernel: the 3x3, 3xFP16 case of conv_wgmma_kernel<true, kN> with the A operand prepared once per tile instead
+// of once per K step. Tiles, K order (tap-major, then channel block) and products are those of conv_wgmma_kernel, so every
+// output is bit-identical to it; only where A comes from differs.
+//   Halo: the tile's nine taps read pixels [m0 - W - 1, m0 + 128 + W + 1) of the flattened B*H*W sequence, one contiguous
+//   NHWC range. Every thread loads its share once per tile, applies the affine + ReLU, in_scale and the fp16 hi/lo split
+//   exactly as store_a does, and stores fp16 hi and lo planes in shared memory: [channel block][row][128 B], 16-byte
+//   chunks XOR-swizzled by row & 7 (ldmatrix over 8 consecutive rows is conflict-free). Pixels outside [0, P) and
+//   channels >= Cin are zeros; row halo_rows - 1 of every channel block is all zero.
+//   Step ks (tap = ks / ncb, cb = ks % ncb): output pixel m reads the halo row of pixel m + dh W + dw, or the zero row when
+//   that neighbour lies outside m's image (or m >= P). ldmatrix.x4 loads each warp's 16 rows x k16 (hi and lo) straight
+//   into the register-A fragment of wgmma; B comes from the swizzled weight stage as before. (Shifted shared-memory A
+//   descriptors cannot do this: at dw = +-1 the pixel past a row end is a real pixel of the next image row, not zero, and
+//   an odd row shift breaks the 128-byte swizzle phase.)
+//   Per k16: lo * hi, hi * lo, hi * hi into `part` (mma_row's order), `acc += part` once per step.
+//   Weights stream through two cp.async stages: stage (ks + 1) & 1 is refilled after the step-ks barrier, by which time
+//   every warpgroup has retired the step ks - 1 group that read it; the refill overlaps the MMAs of step ks. The A
+//   registers are rewritten only after wgmma_wait<0>.
+constexpr int kHaloStages = 2;
+constexpr int kHaloBatch = 8;   // halo chunks per thread in flight (2 x float4 each)
+
+__device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], uint32_t addr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr)
+               : "memory");
+}
+
+template <int kN>
+__global__ void __launch_bounds__(kThreads, 1) conv_halo_kernel(const ConvParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  const int R = p.halo_rows;
+  const uint32_t lo_plane = (uint32_t)p.ncb * (uint32_t)R * 128u;
+  const uint32_t smem_b = smem_u32(smem);                                  // kHaloStages x {B hi, B lo}
+  const uint32_t halo = smem_b + (uint32_t)(kHaloStages * p.stage_bytes);   // hi plane, then lo plane
+  double* s_stat = reinterpret_cast<double*>(smem + (size_t)kHaloStages * p.stage_bytes + 2 * (size_t)lo_plane);
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
+  const float in_s = p.in_scale ? __ldg(p.in_scale) : 1.f;
+  const float oscale = p.in_scale ? p.out_scale * __ldg(p.in_scale + 1) : p.out_scale;
+  const uint32_t b_lo_off = (uint32_t)p.b_tile_bytes;
+  conv_stats_init(p, s_stat);
+  for (int i = tid; i < p.ncb * 8; i += kThreads) {   // the zero rows: never overwritten by the halo loads
+    const uint32_t dst = halo + (uint32_t)((i >> 3) * R + R - 1) * 128u + ((uint32_t)(i & 7) << 4);
+    sts128u(dst, make_uint4(0u, 0u, 0u, 0u));
+    sts128u(dst + lo_plane, make_uint4(0u, 0u, 0u, 0u));
+  }
+
+  const int HW = p.H * p.W;
+  // this lane's ldmatrix.x4 row among the tile's 128 and its k half: matrices {rows 0-7, rows 8-15} x {k 0-7, k 8-15}
+  // of the warp's 16 rows, in the order of the A fragment registers
+  const int lr = wg * 64 + (warp & 3) * 16 + (lane & 7) + (lane & 8);
+  const uint32_t khalf = (uint32_t)(lane >> 4);
+  const int items = p.ncb * (R - 1) * 8;   // 16-byte chunks of one halo plane, zero rows excluded
+
+  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+    const int m0 = (tile / p.n_tiles) * kTileM;
+    const int n0 = (tile % p.n_tiles) * p.nt;
+    const int hs = m0 - p.W - 1;   // pixel of halo row 0
+    conv_load_b<true>(p, 0, n0, smem_b, b_lo_off);
+
+    // ---- halo: chunk idx = (row * ncb + cb) * 8 + jj covers channels cb * 64 + 8 jj .. + 7 of pixel hs + row, so
+    // consecutive threads read consecutive 32-byte pieces of the NHWC span
+    for (int base = tid; base < items; base += kThreads * kHaloBatch) {
+      float4 v[kHaloBatch][2];
 #pragma unroll
-    for (int i = 0; i < kN / 8; ++i) {
-      const int col = n0 + i * 8 + 2 * t;
-      float2 b2 = make_float2(0.f, 0.f), pv = make_float2(0.f, 0.f);
-      if (p.bias) b2 = __ldg(reinterpret_cast<const float2*>(p.bias + col));
-      if (stats && p.stat_pivot) pv = __ldg(reinterpret_cast<const float2*>(p.stat_pivot + col));
-      double s1a = 0.0, s1b = 0.0, s2a = 0.0, s2b = 0.0;
-#pragma unroll
-      for (int rr = 0; rr < 2; ++rr) {
-        const int m = mrow + rr * 8;
-        if (m >= p.P) continue;
-        const size_t off = (size_t)m * p.Cout + col;
-        float2 o = make_float2(acc[4 * i + 2 * rr] * oscale + b2.x, acc[4 * i + 2 * rr + 1] * oscale + b2.y);
-        if (p.residual) {
-          const float2 r2 = __ldg(reinterpret_cast<const float2*>(p.residual + off));
-          o.x += r2.x; o.y += r2.y;
-        }
-        if (p.relu_mask) {
-          const float2 k = __ldg(reinterpret_cast<const float2*>(p.relu_mask + off));
-          o.x = k.x > 0.f ? o.x : 0.f; o.y = k.y > 0.f ? o.y : 0.f;
-        }
-        *reinterpret_cast<float2*>(p.y + off) = o;
-        if (stats) {
-          const double d0 = (double)(o.x - pv.x), d1 = (double)(o.y - pv.y);
-          s1a += d0; s2a += d0 * d0; s1b += d1; s2b += d1 * d1;
+      for (int u = 0; u < kHaloBatch; ++u) {
+        const int idx = base + u * kThreads;
+        const int jj = idx & 7, rc = idx >> 3;
+        const int r = rc / p.ncb, cb = rc - r * p.ncb;
+        const int q = hs + r, c = cb * 64 + jj * 8;
+        v[u][0] = v[u][1] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (idx < items && q >= 0 && q < p.P && c < p.Cin) {
+          const float4* src = reinterpret_cast<const float4*>(p.x + (size_t)q * p.Cin + c);
+          v[u][0] = __ldg(src);
+          v[u][1] = __ldg(src + 1);
         }
       }
-      if (stats) {
 #pragma unroll
-        for (int sh = 4; sh < 32; sh <<= 1) {
-          s1a += __shfl_xor_sync(0xffffffffu, s1a, sh); s2a += __shfl_xor_sync(0xffffffffu, s2a, sh);
-          s1b += __shfl_xor_sync(0xffffffffu, s1b, sh); s2b += __shfl_xor_sync(0xffffffffu, s2b, sh);
+      for (int u = 0; u < kHaloBatch; ++u) {
+        const int idx = base + u * kThreads;
+        if (idx >= items) continue;
+        const int jj = idx & 7, rc = idx >> 3;
+        const int r = rc / p.ncb, cb = rc - r * p.ncb;
+        const int q = hs + r, c = cb * 64 + jj * 8;
+        uint4 oh = make_uint4(0u, 0u, 0u, 0u), ol = make_uint4(0u, 0u, 0u, 0u);
+        if (q >= 0 && q < p.P && c < p.Cin) {
+          float4 a0 = affine_relu4(v[u][0], p.pre_mean, p.pre_scale, p.pre_shift, c, p.pre_relu);
+          float4 a1 = affine_relu4(v[u][1], p.pre_mean, p.pre_scale, p.pre_shift, c + 4, p.pre_relu);
+          a0.x *= in_s; a0.y *= in_s; a0.z *= in_s; a0.w *= in_s;
+          a1.x *= in_s; a1.y *= in_s; a1.z *= in_s; a1.w *= in_s;
+          split_f16x2(a0.x, a0.y, oh.x, ol.x);
+          split_f16x2(a0.z, a0.w, oh.y, ol.y);
+          split_f16x2(a1.x, a1.y, oh.z, ol.z);
+          split_f16x2(a1.z, a1.w, oh.w, ol.w);
         }
-        if (g == 0) {   // lanes 0..3 own two distinct columns each: no conflicts, no atomics
-          my_stat[(size_t)col * 2 + 0] += s1a; my_stat[(size_t)col * 2 + 1] += s2a;
-          my_stat[(size_t)col * 2 + 2] += s1b; my_stat[(size_t)col * 2 + 3] += s2b;
-        }
+        const uint32_t dst = halo + (uint32_t)(cb * R + r) * 128u + ((uint32_t)(jj ^ (r & 7)) << 4);
+        sts128u(dst, oh);
+        sts128u(dst + lo_plane, ol);
       }
     }
-  }
-  if (stats) {
-    __syncthreads();
-    for (int i = tid; i < p.Cout * 2; i += kThreads) {
-      double v = 0.0;
-      for (int w8 = 0; w8 < 8; ++w8) v += s_stat[(size_t)w8 * p.Cout * 2 + i];   // fixed order
-      p.stat_part[(size_t)blockIdx.x * p.Cout * 2 + i] = v;
+
+    const int m = m0 + lr;
+    const int pn = m < p.P ? m / HW : p.B;   // pn == B marks a row past the last pixel
+    const int ph = (m % HW) / p.W, pw = m % p.W;
+    float acc[kN / 2], part[kN / 2];
+    zero_acc(acc);
+    zero_acc(part);
+    for (int ks = 0; ks < p.ksteps; ++ks) {
+      const uint32_t st = smem_b + (uint32_t)((ks & 1) * p.stage_bytes);
+      if (ks > 0) {
+        wgmma_wait<0>();
+        add_part(acc, part);
+      }
+      cp_async_wait_all();
+      fence_proxy_async_smem();
+      __syncthreads();   // the weights of step ks (at ks = 0 also the halo) are visible; stage (ks + 1) & 1 is free
+      if (ks + 1 < p.ksteps)
+        conv_load_b<true>(p, ks + 1, n0, smem_b + (uint32_t)(((ks + 1) & 1) * p.stage_bytes), b_lo_off);
+      const int tap = ks / p.ncb, cb = ks - tap * p.ncb;
+      const int dh = tap / 3 - 1, dw = tap % 3 - 1;
+      const int hh = ph + dh, ww = pw + dw;
+      const bool ok = pn < p.B && hh >= 0 && hh < p.H && ww >= 0 && ww < p.W;
+      const int hr = ok ? lr + (dh + 1) * p.W + dw + 1 : R - 1;
+      const uint32_t row = halo + (uint32_t)(cb * R + hr) * 128u;
+      const uint32_t sw = (uint32_t)(hr & 7);
+      uint32_t ah[4][4], al[4][4];
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {
+        const uint32_t a = row + (((2u * kk + khalf) ^ sw) << 4);
+        ldsm_x4(ah[kk], a);
+        ldsm_x4(al[kk], a + lo_plane);
+      }
+      wgmma_fence();
+      const uint64_t dbh = gmma_desc_sw128(st), dbl = gmma_desc_sw128(st + b_lo_off);
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {
+        const uint64_t o = (uint64_t)(kk * 2);
+        WgmmaRA<kN>::f16(part, al[kk], dbh + o, kk > 0 ? 1 : 0);
+        WgmmaRA<kN>::f16(part, ah[kk], dbl + o, 1);
+        WgmmaRA<kN>::f16(part, ah[kk], dbh + o, 1);
+      }
+      wgmma_commit();
     }
+    wgmma_wait<0>();
+    add_part(acc, part);
+    __syncthreads();   // every warpgroup is done with the halo and both stages: the next tile may refill them
+
+    conv_epilogue<kN>(p, acc, m0, n0, oscale, s_stat);
   }
+  conv_stats_flush(p, s_stat);
 }
 
 bool conv_shape_ok(int Cin, int Cout, int ksize, int f16, int max_cin, int max_cout) {
@@ -378,6 +556,30 @@ int launch_n(const ConvParams& p, int grid, size_t smem, cudaStream_t stream) {
   conv_wgmma_kernel<kF16, kN><<<grid, kThreads, smem, stream>>>(p);
   FPD_LAUNCH_CHECK();
   return FPD_OK;
+}
+
+template <int kN>
+int launch_halo_n(const ConvParams& p, int grid, size_t smem, cudaStream_t stream) {
+  static std::atomic<uint64_t> done{0};
+  if (int rc = allow_smem(conv_halo_kernel<kN>, done)) return rc;
+  conv_halo_kernel<kN><<<grid, kThreads, smem, stream>>>(p);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int launch_halo(const ConvParams& p, int grid, size_t smem, cudaStream_t stream) {
+  switch (p.nt) {
+    case 16: return launch_halo_n<16>(p, grid, smem, stream);
+    case 32: return launch_halo_n<32>(p, grid, smem, stream);
+    case 48: return launch_halo_n<48>(p, grid, smem, stream);
+    case 64: return launch_halo_n<64>(p, grid, smem, stream);
+    case 80: return launch_halo_n<80>(p, grid, smem, stream);
+    case 96: return launch_halo_n<96>(p, grid, smem, stream);
+    case 112: return launch_halo_n<112>(p, grid, smem, stream);
+    case 128: return launch_halo_n<128>(p, grid, smem, stream);
+  }
+  set_last_error("conv_halo: no kernel for a %d-column slice", p.nt);
+  return FPD_ERR_UNSUPPORTED;
 }
 
 template <bool kF16>
@@ -421,9 +623,18 @@ int conv_launch(const float* x, const float* pre_mean, const float* pre_scale, c
   p.out_scale = f16 ? out_scale * (1.0f / (float)(1 << kF16WeightScaleLog2)) : out_scale;
   p.in_scale = in_scale;
   p.stat_part = stat_part; p.stat_pivot = stat_pivot;
-  const size_t smem = 1024 + (size_t)kStages * p.stage_bytes + (stat_part ? (size_t)8 * Cout * 2 * sizeof(double) : 0);
-  FPD_REQUIRE(smem <= (size_t)kSmemLimit, "conv_wgmma: shared memory plan %zu B too large", smem);
+  const size_t stat_bytes = stat_part ? (size_t)8 * Cout * 2 * sizeof(double) : 0;
   const int grid = p.num_tiles < num_sms ? p.num_tiles : num_sms;
+  if (f16 && p.passes == 3 && ksize == 3) {
+    // 3x3 3xFP16: the halo-resident kernel wherever the halo, two weight stages and the statistics scratch fit
+    ConvParams h = p;
+    h.halo_rows = kTileM + 2 * W + 3;
+    h.stage_bytes = 2 * p.b_tile_bytes;
+    const size_t smem = 1024 + (size_t)kHaloStages * h.stage_bytes + 2 * (size_t)h.ncb * h.halo_rows * 128 + stat_bytes;
+    if (smem <= (size_t)kSmemLimit) return launch_halo(h, grid, smem, stream);
+  }
+  const size_t smem = 1024 + (size_t)kStages * p.stage_bytes + stat_bytes;
+  FPD_REQUIRE(smem <= (size_t)kSmemLimit, "conv_wgmma: shared memory plan %zu B too large", smem);
   return f16 ? launch_f<true>(p, grid, smem, stream) : launch_f<false>(p, grid, smem, stream);
 }
 
