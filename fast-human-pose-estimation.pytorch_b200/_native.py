@@ -84,6 +84,8 @@ _SIGNATURES = {
     "fpd_joints_mse": (c_int, [P, P, P, P, P, c_int, c_int, c_int, P, c_size_t, P]),
     "fpd_flip_merge_argmax": (c_int, [P, P, P, c_int, P, P, P, c_int, c_int, c_int, c_int, P]),
     "fpd_argmax_nchw": (c_int, [P, P, P, c_int, c_int, P]),
+    "fpd_final_preds": (c_int, [P, P, P, P, c_int, P, c_int, c_int, c_int, c_int, P]),
+    "fpd_pck_counts": (c_int, [P, P, P, P, P, c_int, c_int, c_int, c_int, P]),
     "fpd_nms_workspace_bytes": (c_size_t, [c_int]),
     "fpd_nms_device": (c_int, [P, c_int, c_int, c_float, P, P, P, c_size_t, P]),
     "fpd_nms_host": (c_int, [P, P, P, c_int, c_int, c_float, c_int]),

@@ -274,6 +274,14 @@ int fpd_flip_merge_argmax(const float* hm, const float* hm_flip, const int* perm
 int fpd_argmax_nchw(const float* hm, int* idx, float* maxval, int BJ, int hw, fpd_stream_t stream) {
   return argmax_nchw(hm, idx, maxval, BJ, hw, S(stream));
 }
+int fpd_final_preds(const float* avg_nhwc, const int* idx, const float* maxval, const double* inv, int post_process,
+                    float* preds, int B, int J, int h, int w, fpd_stream_t stream) {
+  return final_preds(avg_nhwc, idx, maxval, inv, post_process, preds, B, J, h, w, S(stream));
+}
+int fpd_pck_counts(const int* idx, const float* maxval, const float* target_nchw, int* counts, float* pred_hm, int B,
+                   int J, int h, int w, fpd_stream_t stream) {
+  return pck_counts(idx, maxval, target_nchw, counts, pred_hm, B, J, h, w, S(stream));
+}
 
 size_t fpd_nms_workspace_bytes(int n) { return nms_workspace_bytes(n); }
 int fpd_nms_device(const float* boxes, int n, int box_dim, float thresh, int* keep, int* num_keep, void* ws,

@@ -159,6 +159,12 @@ int joints_mse(const float* out_nchw, const float* target_nchw, const float* tw,
 int flip_merge_argmax(const float* hm, const float* hm_flip, const int* flip_perm, int shift, float* avg_nchw,
                       int* idx, float* maxval, int B, int J, int h, int w, cudaStream_t stream);
 int argmax_nchw(const float* hm, int* idx, float* maxval, int BJ, int hw, cudaStream_t stream);
+// get_final_preds from the merged NHWC map and its arg-max: inv double[B,6] heat-map -> image, preds float[B,J,3]
+int final_preds(const float* avg_nhwc, const int* idx, const float* maxval, const double* inv, int post_process,
+                float* preds, int B, int J, int h, int w, cudaStream_t stream);
+// accuracy() counts: counts int32[J,2] = {valid, hit} (zeroed here), pred_hm float[B,J,2] optional
+int pck_counts(const int* idx, const float* maxval, const float* target_nchw, int* counts, float* pred_hm, int B, int J,
+               int h, int w, cudaStream_t stream);
 
 // ---- nms.cu ----
 size_t nms_workspace_bytes(int n);

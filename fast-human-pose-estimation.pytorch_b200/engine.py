@@ -657,6 +657,10 @@ class Engine:
         low3 = self.residual_seq(ctx, low2, "%s.%d.2" % (prefix, n - 1), nblocks)
         if done is not None:
             torch.cuda.current_stream().wait_event(done)
+            # up1's memory belongs to the branch stream. Branch streams come from torch's stream pool, so the same stream
+            # can be another concurrent forward's main stream (the flip-test forward's level-n branch may be the graph
+            # capture stream); without this, that forward may reuse the block while this stream still reads it.
+            up1.data.record_stream(torch.cuda.current_stream())
         return self.upsample_add(ctx, up1, low3)
 
     def _branch_stream(self, main, level):

@@ -28,6 +28,27 @@ def pck_from_preds(pred, target, h, w, thr=0.5):
     return acc, avg, cnt
 
 
+def pck_from_counts(counts):
+    """counts int [J,2] = {valid, hit} per joint (ops.pck_counts, threshold 0.5) -> (acc[J+1], avg, cnt), the same
+    float64 operations in the same order as pck_from_preds, hence the same values."""
+    counts = np.asarray(counts)
+    J = counts.shape[0]
+    acc = np.zeros(J + 1)
+    total, cnt = 0.0, 0
+    for j in range(J):
+        n = int(counts[j, 0])
+        if n > 0:
+            acc[j + 1] = float(int(counts[j, 1])) / n
+            total += acc[j + 1]
+            cnt += 1
+        else:
+            acc[j + 1] = -1
+    avg = total / cnt if cnt else 0
+    if cnt:
+        acc[0] = avg
+    return acc, avg, cnt
+
+
 def accuracy(output, target, hm_type='gaussian', thr=0.5):
     """output/target: CUDA tensors or numpy [B,J,h,w]. Returns (acc[J+1], avg_acc, cnt, pred) like the reference."""
     assert hm_type == 'gaussian'

@@ -9,6 +9,9 @@ What changes underneath:
     model / criterion combination takes the generic autograd route, statement for statement like the reference.
   * per-iteration accuracy() and validate()'s flip test / decode run on the device; only [B,J] indices cross PCIe
     (the reference ships the full heat-maps to numpy every iteration: function.py:154-156, 218-240, 263).
+  * validate: for the fpd_b200 models with JointsMSELoss, each batch is one CUDA graph replay (infer_step.
+    FlipTestInference with its decode stage: both forwards, flip merge, loss, keypoints, PCK counts); the results are
+    copied to pinned host buffers asynchronously and the host waits only to log and at the end of the epoch.
 """
 import logging
 import os
@@ -17,8 +20,8 @@ import time
 import numpy as np
 import torch
 
-from .evaluate import accuracy, pck_from_preds
-from .inference import get_final_preds, preds_from_argmax
+from .evaluate import accuracy, pck_from_counts, pck_from_preds
+from .inference import get_final_preds, inverse_affines, preds_from_argmax
 
 logger = logging.getLogger(__name__)
 
@@ -256,6 +259,57 @@ def fpd_train(config, train_loader, model, tmodel, pose_criterion, kd_pose_crite
             _debug_images(config, input, meta, target, pred, last_out, '{}_{}'.format(os.path.join(output_dir, 'train'), i))
 
 
+# validate() replays one CUDA graph per batch where it can; False forces the eager fused route (the graph route's
+# reference in the tests)
+_VALIDATE_GRAPH = True
+
+
+def _validate_graph_ok(config, criterion, target):
+    """The graph route computes exactly what the eager fused route does, for the batches its kernels take."""
+    dbg = getattr(config, "DEBUG", None)
+    _, J, h, w = target.shape
+    return (_VALIDATE_GRAPH and _is_fpd_criterion(criterion) and not (dbg is not None and getattr(dbg, "DEBUG", False))
+            and J <= 64 and _loss_shape_ok(config, J, h, w))
+
+
+class _GraphValidation:
+    """validate()'s per-batch work as FlipTestInference(decode=True) replays. The device results go to pinned host
+    buffers with non-blocking copies; `flush` waits for them and applies the meter updates in batch order."""
+
+    def __init__(self, config, net, val_dataset, criterion, num_samples, num_batches, J):
+        from fpd_b200.infer_step import FlipTestInference
+        self.runner = FlipTestInference(net, val_dataset.flip_pairs, shift_heatmap=bool(config.TEST.SHIFT_HEATMAP),
+                                        flip_test=bool(config.TEST.FLIP_TEST), decode=True)
+        self.use_tw = criterion.use_target_weight
+        self.post_process = bool(config.TEST.POST_PROCESS)
+        self.preds = torch.empty((num_samples, J, 3), dtype=torch.float32, pin_memory=True)
+        self.loss = torch.empty(num_batches, dtype=torch.float32, pin_memory=True)
+        self.counts = torch.empty((num_batches, J, 2), dtype=torch.int32, pin_memory=True)
+        self.done = torch.cuda.Event()
+        self.pending = []          # (batch, num_images) not yet applied to the meters
+        self.applied = 0           # samples whose predictions are in all_preds
+
+    def run(self, i, input, target, target_weight, c, s, idx):
+        B, _, h, w = target.shape
+        r = self.runner(input, inv=inverse_affines(c, s, [w, h]), target=target, target_weight=target_weight,
+                        use_target_weight=self.use_tw, post_process=self.post_process)
+        self.preds[idx:idx + B].copy_(r["preds"], non_blocking=True)
+        self.loss[i:i + 1].copy_(r["loss3"][:1], non_blocking=True)
+        self.counts[i].copy_(r["pck"], non_blocking=True)
+        self.pending.append((i, B))
+
+    def flush(self, losses, acc, all_preds, upto):
+        self.done.record()
+        self.done.synchronize()
+        for i, n in self.pending:
+            losses.update(float(self.loss[i]), n)
+            _, avg_acc, cnt = pck_from_counts(self.counts[i].numpy())
+            acc.update(avg_acc, cnt)
+        self.pending = []
+        all_preds[self.applied:upto] = self.preds[self.applied:upto].numpy()
+        self.applied = upto
+
+
 def validate(config, val_loader, val_dataset, model, criterion, output_dir, tb_log_dir, writer_dict=None):
     """Evaluation epoch (reference function.py:189-333) with the flip test, shift, average, arg-max on the device."""
     from fpd_b200 import ops
@@ -268,9 +322,32 @@ def validate(config, val_loader, val_dataset, model, criterion, output_dir, tb_l
     idx = 0
     fpd_net = _is_fpd_net(model)
     perm_cache = {}
+    graph = None
     with torch.no_grad():
         end = time.time()
         for i, (input, target, target_weight, meta) in enumerate(val_loader):
+            if fpd_net and i == 0 and _validate_graph_ok(config, criterion, target):
+                graph = _GraphValidation(config, _unwrap(model), val_dataset, criterion, num_samples, len(val_loader),
+                                         target.shape[1])
+            if graph is not None:
+                num_images = input.size(0)
+                c = meta['center'].numpy()
+                s = meta['scale'].numpy()
+                score = meta['score'].numpy()
+                graph.run(i, input, target, target_weight, c, s, idx)
+                batch_time.update(time.time() - end)
+                end = time.time()
+                all_boxes[idx:idx + num_images, 0:2] = c[:, 0:2]
+                all_boxes[idx:idx + num_images, 2:4] = s[:, 0:2]
+                all_boxes[idx:idx + num_images, 4] = np.prod(s * 200, 1)
+                all_boxes[idx:idx + num_images, 5] = score
+                image_path.extend(meta['image'])
+                idx += num_images
+                if i % config.PRINT_FREQ == 0:
+                    graph.flush(losses, acc, all_preds, idx)
+                    logger.info('Test: [%d/%d]\tTime %.3f (%.3f)\tLoss %.4f (%.4f)\tAccuracy %.3f (%.3f)' % (
+                        i, len(val_loader), batch_time.val, batch_time.avg, losses.val, losses.avg, acc.val, acc.avg))
+                continue
             x = input.cuda(non_blocking=True).float().contiguous()
             if fpd_net:
                 net = _unwrap(model)
@@ -323,6 +400,8 @@ def validate(config, val_loader, val_dataset, model, criterion, output_dir, tb_l
                 logger.info('Test: [%d/%d]\tTime %.3f (%.3f)\tLoss %.4f (%.4f)\tAccuracy %.3f (%.3f)' % (
                     i, len(val_loader), batch_time.val, batch_time.avg, losses.val, losses.avg, acc.val, acc.avg))
                 _debug_images(config, input, meta, target, pred, output, '{}_{}'.format(os.path.join(output_dir, 'val'), i))
+        if graph is not None:
+            graph.flush(losses, acc, all_preds, idx)
         name_values, perf_indicator = val_dataset.evaluate(config, all_preds, output_dir, all_boxes, image_path,
                                                            filenames, imgnums)
         model_name = config.MODEL.NAME

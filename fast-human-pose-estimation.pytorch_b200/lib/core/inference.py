@@ -54,6 +54,31 @@ def _inverse_affine(center, scale, output_size):
     return np.linalg.solve(a, src.astype(np.float64)).T          # maps heat-map (dst) coordinates to image (src)
 
 
+def inverse_affines(center, scale, output_size):
+    """_inverse_affine for a whole batch: center, scale [B,2] -> float64 [B,6], row b the row-major 2x3 matrix of sample
+    b, equal bit for bit to _inverse_affine(center[b], scale[b], output_size) (the same float32 point arithmetic, the
+    same LAPACK solve per sample). This is the `inv` that ops.final_preds takes."""
+    c = np.asarray(center, np.float32).reshape(-1, 2)
+    src_w = np.asarray(scale, np.float32).reshape(-1, 2)[:, 0] * np.float32(200.0)
+    B = c.shape[0]
+    dst_w, dst_h = output_size[0], output_size[1]
+    src = np.zeros((B, 3, 2), np.float32)
+    dst = np.zeros((3, 2), np.float32)
+    src[:, 0] = c
+    shift = np.zeros((B, 2))
+    shift[:, 1] = (src_w * np.float32(-0.5)).astype(np.float64)
+    src[:, 1] = c.astype(np.float64) + shift
+    dst[0] = [dst_w * 0.5, dst_h * 0.5]
+    dst[1] = np.array([dst_w * 0.5, dst_h * 0.5]) + np.array([0, dst_w * -0.5], np.float32)
+    d = src[:, 0] - src[:, 1]
+    src[:, 2] = src[:, 1] + np.stack([-d[:, 1], d[:, 0]], 1)
+    d = dst[0] - dst[1]
+    dst[2] = dst[1] + np.array([-d[1], d[0]], np.float32)
+    a = np.concatenate([dst.astype(np.float64), np.ones((3, 1))], 1)
+    t = np.linalg.solve(np.broadcast_to(a, (B, 3, 3)), src.astype(np.float64))     # [B,3,2]
+    return np.ascontiguousarray(t.transpose(0, 2, 1).reshape(B, 6))
+
+
 def transform_preds(coords, center, scale, output_size):
     """lib/utils/transforms.py:49-54 for the whole [J,2] array at once (rot = 0 is the only call the hot path makes)."""
     coords = np.asarray(coords, dtype=np.float64)

@@ -607,6 +607,33 @@ def argmax_nchw(hm):
     return idx, maxval
 
 
+def final_preds(avg_nhwc, idx, maxval, inv, post_process, out=None):
+    """get_final_preds on the device (csrc/decode.cu). avg_nhwc: [B,h,w,J] merged heat-maps; idx int32 / maxval [B,J]
+    from flip_merge_argmax; inv: CUDA float64 [B,6] heat-map -> image matrices (lib.core.inference.inverse_affines).
+    Returns preds [B,J,3] = (x, y, maxval) in image coordinates."""
+    _chk(avg_nhwc, "avg_nhwc")
+    B, h, w, J = avg_nhwc.shape
+    if not (inv.is_cuda and inv.dtype == torch.float64 and inv.is_contiguous() and tuple(inv.shape) == (B, 6)):
+        raise ValueError("inv must be a contiguous float64 CUDA tensor of shape (%d, 6)" % B)
+    preds = out if out is not None else torch.empty((B, J, 3), dtype=torch.float32, device=avg_nhwc.device)
+    N.check(N.lib().fpd_final_preds(_p(avg_nhwc), _p(idx), _p(maxval), _p(inv), int(bool(post_process)), _p(preds), B, J,
+                                    h, w, _stream()), "final_preds")
+    return preds
+
+
+def pck_counts(idx, maxval, target_nchw, want_pred_hm=False, out=None):
+    """accuracy() counts on the device (csrc/decode.cu): int32 [J,2] = {valid, hit} per joint, plus the prediction in
+    heat-map coordinates [B,J,2] when want_pred_hm (else None). lib.core.evaluate.pck_from_counts turns the counts into
+    accuracy()'s (acc, avg_acc, cnt)."""
+    _chk(target_nchw, "target")
+    B, J, h, w = target_nchw.shape
+    counts = out if out is not None else torch.empty((J, 2), dtype=torch.int32, device=target_nchw.device)
+    pred_hm = torch.empty((B, J, 2), dtype=torch.float32, device=target_nchw.device) if want_pred_hm else None
+    N.check(N.lib().fpd_pck_counts(_p(idx), _p(maxval), _p(target_nchw), _p(counts), _p(pred_hm), B, J, h, w, _stream()),
+            "pck_counts")
+    return counts, pred_hm
+
+
 def nms_device(boxes_sorted, thresh):
     n, d = boxes_sorted.shape
     dev = boxes_sorted.device

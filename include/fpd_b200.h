@@ -264,6 +264,19 @@ int fpd_joints_mse(const float* out_nchw, const float* target_nchw, const float*
 int fpd_flip_merge_argmax(const float* hm, const float* hm_flip, const int* flip_perm, int shift, float* avg_nhwc,
                           int* idx, float* maxval, int B, int J, int h, int w, fpd_stream_t stream);
 int fpd_argmax_nchw(const float* hm_nchw, int* idx, float* maxval, int BJ, int hw, fpd_stream_t stream);
+/* get_final_preds, lib/core/inference.py:49-79 (+ transform_preds, lib/utils/transforms.py:49-54), from the merged map
+ * avg_nhwc [B,h,w,J] and its arg-max idx / maxval [B,J] (fpd_flip_merge_argmax). post_process != 0 nudges each
+ * coordinate a quarter pixel toward the higher neighbour (needs h, w >= 3). inv: device double[B,6], the row-major 2x3
+ * heat-map -> image matrix per sample (the convention of fpd_crop_affine_normalize). preds: float[B,J,3] = (x, y,
+ * maxval). J <= 64. */
+int fpd_final_preds(const float* avg_nhwc, const int* idx, const float* maxval, const double* inv, int post_process,
+                    float* preds, int B, int J, int h, int w, fpd_stream_t stream);
+/* accuracy(), lib/core/evaluate.py:16-71, as per-joint counts: the arg-max of each target map target_nchw [B,J,h,w]
+ * against the prediction's idx / maxval [B,J]. counts: device int32[J,2] = {joints whose target lies at x > 1 and
+ * y > 1, those of them within 0.5 of the target after normalising x by h/10 and y by w/10}; zeroed by the call.
+ * pred_hm: optional float[B,J,2], the prediction in heat-map coordinates. J <= 64. */
+int fpd_pck_counts(const int* idx, const float* maxval, const float* target_nchw, int* counts, float* pred_hm, int B,
+                   int J, int h, int w, fpd_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------
  * NMS. Replaces lib/nms/nms_kernel.cu:33-77 (nms_kernel) and :90-143 (_nms), declared in
