@@ -266,6 +266,21 @@ int fpd_joints_mse(const float* out, const float* target, const float* tw, float
                    int hw, void* ws, size_t wsb, fpd_stream_t stream) {
   return joints_mse(out, target, tw, loss3, grad, 1.f, B, J, hw, ws, wsb, S(stream));
 }
+size_t fpd_loss_ohkm_workspace_bytes(int Sn, int B, int J, int h, int w) {
+  return fpd::fpd_loss_ohkm_workspace_bytes(Sn, B, J, h, w);
+}
+int fpd_loss_ohkm_fused(const float* const* outs_host, int Sn, const float* target_nchw, const float* teacher_nhwc,
+                        const float* tw, float alpha, float* const* grads_host, float grad_scale, float* losses, int B,
+                        int J, int h, int w, int pose_topk, int kd_topk, void* ws, size_t wsb, fpd_stream_t stream) {
+  FPD_REQUIRE(outs_host != nullptr, "fpd_loss_ohkm_fused: outs_host is NULL");
+  return fpd::fpd_loss_ohkm(outs_host, Sn, target_nchw, teacher_nhwc, tw, alpha, grads_host, grad_scale, losses, B, J,
+                            h, w, pose_topk, kd_topk, ws, wsb, S(stream));
+}
+size_t fpd_joints_ohkm_workspace_bytes(int B, int J) { return joints_ohkm_workspace_bytes(B, J); }
+int fpd_joints_ohkm(const float* out, const float* target, const float* tw, int topk, float* loss3, float* grad, int B,
+                    int J, int hw, void* ws, size_t wsb, fpd_stream_t stream) {
+  return joints_ohkm(out, target, tw, topk, loss3, grad, B, J, hw, ws, wsb, S(stream));
+}
 
 int fpd_flip_merge_argmax(const float* hm, const float* hm_flip, const int* perm, int shift, float* avg_nhwc,
                           int* idx, float* maxval, int B, int J, int h, int w, fpd_stream_t stream) {

@@ -153,6 +153,15 @@ int fpd_loss(const float* const* outs_dev_ptrs_host, int S, const float* target_
 // reference-compatible single JointsMSELoss on NCHW tensors (lib/core/loss.py:21-39)
 int joints_mse(const float* out_nchw, const float* target_nchw, const float* tw, float* loss, float* grad_out,
                float grad_scale_unused, int B, int J, int hw, void* workspace, size_t ws_bytes, cudaStream_t stream);
+// online hard keypoint mining (lib/core/loss.py:42-87): the fused FPD form with a topk per term (0 = JointsMSELoss) and
+// the NCHW module form (loss[0] is the value, grad optional)
+size_t fpd_loss_ohkm_workspace_bytes(int S, int B, int J, int h, int w);
+int fpd_loss_ohkm(const float* const* outs_dev_ptrs_host, int S, const float* target_nchw, const float* teacher_nhwc,
+                  const float* tw, float alpha, float* const* grads_host, float grad_scale, float* losses, int B, int J,
+                  int h, int w, int pose_topk, int kd_topk, void* workspace, size_t ws_bytes, cudaStream_t stream);
+size_t joints_ohkm_workspace_bytes(int B, int J);
+int joints_ohkm(const float* out_nchw, const float* target_nchw, const float* tw, int topk, float* loss, float* grad_out,
+                int B, int J, int hw, void* workspace, size_t ws_bytes, cudaStream_t stream);
 
 // ---- decode.cu ----
 // flip-test merge + arg-max: hm/hm_flip NHWC [B,h,w,J]; out avg NCHW (optional), idx[B,J] int32, maxval[B,J]

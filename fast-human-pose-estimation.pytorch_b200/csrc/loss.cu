@@ -169,4 +169,354 @@ int joints_mse(const float* out_nchw, const float* target_nchw, const float* tw,
   return FPD_OK;
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Online hard keypoint mining (reference lib/core/loss.py:42-87, JointsOHKMMSELoss):
+//   l[b,j] = 0.5 * mean_p (w[b,j]*o - w[b,j]*g)^2 ;  L = 1/B * sum_b 1/topk * sum_{j in S_b} l[b,j]
+//   S_b = the topk joints with the largest fp32-rounded l[b,.]; on exact ties the lower joint index wins
+//   dL/do = [j in S_b] * w^2 * (o - g) / (B * topk * hw)
+// The gradient depends on a per-sample selection, so the heat-maps are read twice: (1) per-(stack, sample, joint)
+// sums of squares, fp32 partials added in fp64 in a fixed order; (2) one warp per (stack, term, sample) ranks the J
+// values and turns the selection into per-(s, b, j) gradient coefficients (zero for joints left out); (3) one pass
+// writes every gradient element. A topk of 0 makes a term plain JointsMSELoss (coefficient 1/(J*B*hw) for every
+// joint), so the fused FPD form covers all four pose / kd combinations. No floating-point atomics: deterministic and
+// graph-capturable.
+//
+// Workspace: part double [B][nch][S][2][J] | contrib double [B][S][2] | coef float [B][S][2][J]
+// (nch = 64-pixel chunks per sample on the fused NHWC form, 1 on the NCHW module form).
+namespace {
+
+constexpr int kMaxJ = 64;
+
+// a ranks ahead of b: larger value first (NaN above everything, as torch.topk orders it), then the lower index
+__device__ __forceinline__ bool ohkm_ahead(float a, int ia, float b, int ib) {
+  const bool an = isnan(a), bn = isnan(b);
+  if (an || bn) return an && (!bn || ia < ib);
+  return a > b || (a == b && ia < ib);
+}
+
+// Bit j set <=> joint j is among the k first of v[0..J) in ohkm_ahead order. One warp, J <= 64; every lane gets the
+// same mask. Ranking by counting is a total order, so exactly min(k, J) bits are set.
+__device__ __forceinline__ unsigned long long warp_topk_mask(const float* v, int J, int k, int lane) {
+  bool sel[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int j = lane + 32 * h;
+    sel[h] = false;
+    if (j < J) {
+      const float x = v[j];
+      int rank = 0;
+      for (int jj = 0; jj < J; ++jj) rank += ohkm_ahead(v[jj], jj, x, j) ? 1 : 0;
+      sel[h] = rank < k;
+    }
+  }
+  const unsigned lo = __ballot_sync(0xffffffffu, sel[0]);
+  const unsigned hi = __ballot_sync(0xffffffffu, sel[1]);
+  return (unsigned long long)lo | ((unsigned long long)hi << 32);
+}
+
+// (1) fused form: per (sample, 64-pixel chunk) block, sums over the chunk of (o_s - g)^2 and (o_s - t)^2 for every
+// (s, j). Thread (pl, j) owns joint j and pixels pl, pl + L, ... (L = pixel lanes), so the reduction needs no atomics.
+__global__ void __launch_bounds__(kThreads)
+ohkm_sums_nhwc_kernel(StackPtrs sp, int S, const float* __restrict__ target, const float* __restrict__ teacher, int J,
+                      int hw, double* __restrict__ part) {
+  extern __shared__ float sm[];
+  float* tgt = sm;                        // [J][kPix+1]
+  float* red = sm + J * (kPix + 1);       // [S*2][L*J]
+  const int nch = hw / kPix;
+  const int b = blockIdx.x / nch;
+  const int p0 = (blockIdx.x % nch) * kPix;
+  for (int i = threadIdx.x; i < J * kPix; i += kThreads) {
+    const int j = i / kPix, px = i % kPix;
+    tgt[j * (kPix + 1) + px] = __ldg(target + ((int64_t)b * J + j) * hw + p0 + px);
+  }
+  __syncthreads();
+  const int L = min(kPix, kThreads / J);
+  const int active = L * J;
+  if (threadIdx.x < active) {
+    const int j = threadIdx.x % J, pl = threadIdx.x / J;
+    float ap[kMaxStacks], ak[kMaxStacks];
+#pragma unroll
+    for (int s = 0; s < kMaxStacks; ++s) ap[s] = ak[s] = 0.f;
+    const int64_t base = ((int64_t)b * hw + p0) * J + j;
+    for (int px = pl; px < kPix; px += L) {
+      const int64_t e = base + (int64_t)px * J;
+      const float g = tgt[j * (kPix + 1) + px];
+      const float t = teacher ? __ldg(teacher + e) : 0.f;
+#pragma unroll
+      for (int s = 0; s < kMaxStacks; ++s) {
+        if (s < S) {
+          const float o = __ldg(sp.out[s] + e);
+          const float dp = o - g, dk = o - t;
+          ap[s] = fmaf(dp, dp, ap[s]);
+          ak[s] = fmaf(dk, dk, ak[s]);
+        }
+      }
+    }
+#pragma unroll
+    for (int s = 0; s < kMaxStacks; ++s) {
+      if (s < S) {
+        red[(2 * s) * active + threadIdx.x] = ap[s];
+        red[(2 * s + 1) * active + threadIdx.x] = teacher ? ak[s] : 0.f;
+      }
+    }
+  }
+  __syncthreads();
+  double* dst = part + (size_t)blockIdx.x * S * 2 * J;
+  for (int q = threadIdx.x; q < S * 2 * J; q += kThreads) {
+    const int st = q / J, j = q % J;
+    double acc = 0.0;
+    for (int pl = 0; pl < L; ++pl) acc += (double)red[st * active + pl * J + j];
+    dst[q] = acc;
+  }
+}
+
+// (1) module form: one block per NCHW (b, j) map; part[b][0][0][0][j] = sum_p (o - g)^2, the kd slot is zero
+__global__ void __launch_bounds__(kThreads)
+ohkm_sums_nchw_kernel(const float* __restrict__ out, const float* __restrict__ target, int J, int hw,
+                      double* __restrict__ part) {
+  const int b = blockIdx.x / J, j = blockIdx.x % J;
+  const float* o = out + (int64_t)blockIdx.x * hw;
+  const float* g = target + (int64_t)blockIdx.x * hw;
+  float acc = 0.f;
+  double dacc = 0.0;
+  int inner = 0;
+  for (int p = threadIdx.x; p < hw; p += kThreads) {
+    const float d = __ldg(o + p) - __ldg(g + p);
+    acc = fmaf(d, d, acc);
+    if (++inner == 32) { dacc += (double)acc; acc = 0.f; inner = 0; }
+  }
+  dacc += (double)acc;
+  __shared__ double red[kThreads / 32];
+  dacc = warp_sum(dacc);
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  if (lane == 0) red[wid] = dacc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+    for (int i = 0; i < kThreads / 32; ++i) s += red[i];
+    part[(size_t)b * 2 * J + j] = s;
+    part[(size_t)b * 2 * J + J + j] = 0.0;
+  }
+}
+
+// (2) one block per sample: per-(s, term, j) losses l = 0.5 * w^2 * sum / hw, then one warp per (s, term) selects and
+// writes the sample's share of the term (selected sum / topk, or sum / J for plain MSE) and the gradient
+// coefficients grad_scale * {1-alpha | alpha | 1} * w^2 / (B * {topk | J} * hw) of the selected joints.
+__global__ void __launch_bounds__(kThreads)
+ohkm_select_kernel(const double* __restrict__ part, int nch, int S, int J, int hw, int B, const float* __restrict__ tw,
+                   int has_teacher, int pose_topk, int kd_topk, float alpha, float grad_scale,
+                   double* __restrict__ contrib, float* __restrict__ coef) {
+  __shared__ double ld[kMaxStacks * 2][kMaxJ];
+  __shared__ float lf[kMaxStacks * 2][kMaxJ];
+  const int b = blockIdx.x;
+  const int SJ2 = S * 2 * J;
+  for (int q = threadIdx.x; q < SJ2; q += kThreads) {
+    const int st = q / J, j = q % J;
+    double acc = 0.0;
+    for (int c = 0; c < nch; ++c) acc += part[((size_t)b * nch + c) * SJ2 + q];
+    const double w = tw ? (double)__ldg(tw + (size_t)b * J + j) : 1.0;
+    const double l = 0.5 * (w * w) * acc / (double)hw;
+    ld[st][j] = l;
+    lf[st][j] = (float)l;
+  }
+  __syncthreads();
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  for (int st = wid; st < S * 2; st += kThreads / 32) {
+    const int s = st >> 1, term = st & 1;
+    float* cf = coef + (((size_t)b * S + s) * 2 + term) * J;
+    double* ct = contrib + ((size_t)b * S + s) * 2 + term;
+    if (term == 1 && !has_teacher) {
+      for (int j = lane; j < J; j += 32) cf[j] = 0.f;
+      if (lane == 0) *ct = 0.0;
+      continue;
+    }
+    const int k = term ? kd_topk : pose_topk;
+    const unsigned long long mask = k > 0 ? warp_topk_mask(lf[st], J, k, lane)
+                                          : (J == 64 ? ~0ull : ((1ull << J) - 1ull));
+    const int cnt = k > 0 ? k : J;
+    const double factor = has_teacher ? (term ? (double)alpha : 1.0 - (double)alpha) : 1.0;
+    const double scale = (double)grad_scale * factor / ((double)B * (double)cnt * (double)hw);
+    for (int j = lane; j < J; j += 32) {
+      const double w = tw ? (double)__ldg(tw + (size_t)b * J + j) : 1.0;
+      cf[j] = ((mask >> j) & 1ull) ? (float)(scale * w * w) : 0.f;
+    }
+    if (lane == 0) {
+      double sum = 0.0;
+      for (int j = 0; j < J; ++j)
+        if ((mask >> j) & 1ull) sum += ld[st][j];
+      *ct = sum / (double)cnt;
+    }
+  }
+}
+
+// (2') losses[3] = {pose, kd, total}: term_s = 1/B sum_b share[b][s][term], pose / kd = sum over stacks in order
+__global__ void ohkm_final_kernel(const double* __restrict__ contrib, int B, int S, int has_teacher, float alpha,
+                                  float* __restrict__ losses) {
+  __shared__ double crit[kMaxStacks * 2];
+  const int st = threadIdx.x;
+  if (st < S * 2) {
+    double a = 0.0;
+    for (int b = 0; b < B; ++b) a += contrib[(size_t)b * S * 2 + st];
+    crit[st] = a / (double)B;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double pose = 0.0, kd = 0.0;
+    for (int s = 0; s < S; ++s) { pose += crit[2 * s]; kd += crit[2 * s + 1]; }
+    losses[0] = (float)pose;
+    losses[1] = (float)kd;
+    losses[2] = has_teacher ? (float)((1.0 - (double)alpha) * pose + (double)alpha * kd) : (float)pose;
+  }
+}
+
+// (3) fused form: grad_s = c_pose[s,b,j] * (o_s - g) + c_kd[s,b,j] * (o_s - t) for every element
+__global__ void __launch_bounds__(kThreads)
+ohkm_grad_nhwc_kernel(StackPtrs sp, int S, const float* __restrict__ target, const float* __restrict__ teacher,
+                      const float* __restrict__ coef, int J, int hw) {
+  extern __shared__ float sm[];
+  float* tgt = sm;                        // [J][kPix+1]
+  float* cs = sm + J * (kPix + 1);        // [S][2][J] of this sample
+  const int nch = hw / kPix;
+  const int b = blockIdx.x / nch;
+  const int p0 = (blockIdx.x % nch) * kPix;
+  for (int i = threadIdx.x; i < J * kPix; i += kThreads) {
+    const int j = i / kPix, px = i % kPix;
+    tgt[j * (kPix + 1) + px] = __ldg(target + ((int64_t)b * J + j) * hw + p0 + px);
+  }
+  for (int i = threadIdx.x; i < S * 2 * J; i += kThreads) cs[i] = __ldg(coef + (size_t)b * S * 2 * J + i);
+  __syncthreads();
+  const int64_t base = ((int64_t)b * hw + p0) * J;
+  for (int i = threadIdx.x; i < J * kPix; i += kThreads) {
+    const int px = i / J, j = i % J;
+    const float g = tgt[j * (kPix + 1) + px];
+    const float t = teacher ? __ldg(teacher + base + i) : 0.f;
+#pragma unroll
+    for (int s = 0; s < kMaxStacks; ++s) {
+      if (s < S) {
+        // each term rounded on its own, then added (no FMA), as autograd adds the gradients of the two module-form
+        // criteria: the same bits whenever alpha and 1 - alpha are powers of two (alpha = 0.5)
+        const float o = __ldg(sp.out[s] + base + i);
+        float gr = __fmul_rn(cs[(2 * s) * J + j], o - g);
+        if (teacher) gr = __fadd_rn(gr, __fmul_rn(cs[(2 * s + 1) * J + j], o - t));
+        sp.grad[s][base + i] = gr;
+      }
+    }
+  }
+}
+
+// (3) module form: one block per NCHW (b, j) map; joints left out (coefficient 0) get zeros without reading the maps
+__global__ void __launch_bounds__(kThreads)
+ohkm_grad_nchw_kernel(const float* __restrict__ out, const float* __restrict__ target, const float* __restrict__ coef,
+                      int J, int hw, float* __restrict__ grad) {
+  const int b = blockIdx.x / J, j = blockIdx.x % J;
+  const float c = __ldg(coef + (size_t)b * 2 * J + j);
+  const int64_t off = (int64_t)blockIdx.x * hw;
+  if (c == 0.f) {
+    for (int p = threadIdx.x; p < hw; p += kThreads) grad[off + p] = 0.f;
+    return;
+  }
+  for (int p = threadIdx.x; p < hw; p += kThreads) grad[off + p] = c * (__ldg(out + off + p) - __ldg(target + off + p));
+}
+
+size_t ohkm_ws_bytes(int64_t B, int64_t nch, int64_t S, int64_t J) {
+  return (size_t)((B * nch * S * 2 * J + B * S * 2) * (int64_t)sizeof(double) + B * S * 2 * J * (int64_t)sizeof(float));
+}
+
+struct OhkmWs {
+  double* part;
+  double* contrib;
+  float* coef;
+};
+
+OhkmWs ohkm_ws_split(void* ws, int64_t B, int64_t nch, int64_t S, int64_t J) {
+  OhkmWs r;
+  r.part = (double*)ws;
+  r.contrib = r.part + B * nch * S * 2 * J;
+  r.coef = (float*)(r.contrib + B * S * 2);
+  return r;
+}
+
+}  // namespace
+
+size_t fpd_loss_ohkm_workspace_bytes(int S, int B, int J, int h, int w) {
+  const int64_t hw = (int64_t)h * w;
+  if (S < 1 || B < 1 || J < 1 || hw < 1) return 0;
+  return ohkm_ws_bytes(B, (hw + kPix - 1) / kPix, S, J);
+}
+
+size_t joints_ohkm_workspace_bytes(int B, int J) {
+  if (B < 1 || J < 1) return 0;
+  return ohkm_ws_bytes(B, 1, 1, J);
+}
+
+int fpd_loss_ohkm(const float* const* outs, int S, const float* target_nchw, const float* teacher_nhwc, const float* tw,
+                  float alpha, float* const* grads, float grad_scale, float* losses, int B, int J, int h, int w,
+                  int pose_topk, int kd_topk, void* workspace, size_t ws_bytes, cudaStream_t stream) {
+  FPD_REQUIRE(S >= 1 && S <= kMaxStacks, "fpd_loss_ohkm: S=%d out of range [1,%d]", S, kMaxStacks);
+  FPD_REQUIRE(B >= 1, "fpd_loss_ohkm: B=%d (an empty batch has no loss)", B);
+  FPD_REQUIRE(h >= 1 && w >= 1, "fpd_loss_ohkm: empty heat-map %dx%d", h, w);
+  const int64_t hw64 = (int64_t)h * w;
+  FPD_REQUIRE(hw64 % kPix == 0 && hw64 <= (1 << 30), "fpd_loss_ohkm: h*w=%lld must be a multiple of %d",
+              (long long)hw64, kPix);
+  const int hw = (int)hw64;
+  FPD_REQUIRE(J >= 1 && J <= kMaxJ, "fpd_loss_ohkm: J=%d out of range [1,%d]", J, kMaxJ);
+  FPD_REQUIRE(pose_topk >= 0 && pose_topk <= J, "fpd_loss_ohkm: pose_topk=%d out of range [0,J=%d]", pose_topk, J);
+  FPD_REQUIRE(kd_topk >= 0 && kd_topk <= J, "fpd_loss_ohkm: kd_topk=%d out of range [0,J=%d]", kd_topk, J);
+  FPD_REQUIRE(teacher_nhwc != nullptr || kd_topk == 0, "fpd_loss_ohkm: kd_topk=%d without a teacher", kd_topk);
+  FPD_REQUIRE(target_nchw != nullptr && losses != nullptr, "fpd_loss_ohkm: target or losses is NULL");
+  FPD_REQUIRE(tw != nullptr, "fpd_loss_ohkm: target_weight is required (pass ones for use_target_weight=False)");
+  const int64_t nch = hw / kPix;
+  FPD_REQUIRE((int64_t)B * nch <= 0x7fffffff, "fpd_loss_ohkm: B * h*w/%d too large", kPix);
+  FPD_REQUIRE(workspace != nullptr && ws_bytes >= ohkm_ws_bytes(B, nch, S, J), "fpd_loss_ohkm: workspace too small");
+  StackPtrs sp{};
+  for (int s = 0; s < S; ++s) {
+    FPD_REQUIRE(outs[s] != nullptr, "fpd_loss_ohkm: outs[%d] is NULL", s);
+    sp.out[s] = outs[s];
+    sp.grad[s] = grads ? grads[s] : nullptr;
+    FPD_REQUIRE(grads == nullptr || grads[s] != nullptr, "fpd_loss_ohkm: grads[%d] is NULL", s);
+  }
+  const OhkmWs ws = ohkm_ws_split(workspace, B, nch, S, J);
+  const int L = kThreads / J < kPix ? kThreads / J : kPix;
+  const size_t smem1 = ((size_t)J * (kPix + 1) + (size_t)S * 2 * L * J) * sizeof(float);
+  ohkm_sums_nhwc_kernel<<<(int)(B * nch), kThreads, smem1, stream>>>(sp, S, target_nchw, teacher_nhwc, J, hw, ws.part);
+  FPD_LAUNCH_CHECK();
+  const int has_teacher = teacher_nhwc != nullptr;
+  ohkm_select_kernel<<<B, kThreads, 0, stream>>>(ws.part, (int)nch, S, J, hw, B, tw, has_teacher, pose_topk, kd_topk,
+                                                 alpha, grad_scale, ws.contrib, ws.coef);
+  FPD_LAUNCH_CHECK();
+  ohkm_final_kernel<<<1, 32, 0, stream>>>(ws.contrib, B, S, has_teacher, alpha, losses);
+  FPD_LAUNCH_CHECK();
+  if (grads) {
+    const size_t smem3 = ((size_t)J * (kPix + 1) + (size_t)S * 2 * J) * sizeof(float);
+    ohkm_grad_nhwc_kernel<<<(int)(B * nch), kThreads, smem3, stream>>>(sp, S, target_nchw, teacher_nhwc, ws.coef, J, hw);
+    FPD_LAUNCH_CHECK();
+  }
+  return FPD_OK;
+}
+
+int joints_ohkm(const float* out_nchw, const float* target_nchw, const float* tw, int topk, float* loss3,
+                float* grad_out, int B, int J, int hw, void* workspace, size_t ws_bytes, cudaStream_t stream) {
+  FPD_REQUIRE(out_nchw != nullptr && target_nchw != nullptr && loss3 != nullptr,
+              "joints_ohkm: out, target or loss3 is NULL");
+  FPD_REQUIRE(B >= 1, "joints_ohkm: B=%d (an empty batch has no loss)", B);
+  FPD_REQUIRE(hw >= 1, "joints_ohkm: hw=%d (empty heat-map)", hw);
+  FPD_REQUIRE(J >= 1 && J <= kMaxJ, "joints_ohkm: J=%d out of range [1,%d]", J, kMaxJ);
+  FPD_REQUIRE(topk >= 1 && topk <= J, "joints_ohkm: topk=%d out of range [1,J=%d]", topk, J);
+  FPD_REQUIRE((int64_t)B * J <= 0x7fffffff, "joints_ohkm: B*J too large");
+  FPD_REQUIRE(workspace != nullptr && ws_bytes >= ohkm_ws_bytes(B, 1, 1, J), "joints_ohkm: workspace too small");
+  const OhkmWs ws = ohkm_ws_split(workspace, B, 1, 1, J);
+  ohkm_sums_nchw_kernel<<<B * J, kThreads, 0, stream>>>(out_nchw, target_nchw, J, hw, ws.part);
+  FPD_LAUNCH_CHECK();
+  ohkm_select_kernel<<<B, kThreads, 0, stream>>>(ws.part, 1, 1, J, hw, B, tw, 0, topk, 0, 0.f, 1.f, ws.contrib,
+                                                 ws.coef);
+  FPD_LAUNCH_CHECK();
+  ohkm_final_kernel<<<1, 32, 0, stream>>>(ws.contrib, B, 1, 0, 0.f, loss3);
+  FPD_LAUNCH_CHECK();
+  if (grad_out) {
+    ohkm_grad_nchw_kernel<<<B * J, kThreads, 0, stream>>>(out_nchw, target_nchw, ws.coef, J, hw, grad_out);
+    FPD_LAUNCH_CHECK();
+  }
+  return FPD_OK;
+}
+
 }  // namespace fpd

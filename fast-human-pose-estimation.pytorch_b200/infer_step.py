@@ -8,8 +8,9 @@ one pixel, average, D2H of the merged heat-maps, numpy arg-max. Here, per batch:
                    forward (eval BN, cached 3xFP16 weights)      | second stream: forward of the mirrored image
                    fused flip_back + shift + average + arg-max -> idx[B,J], maxval[B,J] (+ merged heat-maps)
                    [optional box NMS of the detector boxes that produced the crops: lib/nms, csrc/nms.cu]
-                   [decode=True: merged map -> NCHW -> JointsMSELoss (loss3), get_final_preds (preds), accuracy()
-                    counts (pck), all on the device, bit-identical to lib/core/function.py's eager route] }
+                   [decode=True: merged map -> NCHW -> JointsMSELoss or JointsOHKMMSELoss (loss3), get_final_preds
+                    (preds), accuracy() counts (pck), all on the device, bit-identical to lib/core/function.py's eager
+                    route] }
 
 Only [B,J] indices and maxima (or [B,J,3] predictions, 3 loss floats and [J,2] counts) need to cross PCIe. The module must be one of fpd_b200.lib.models (hourglass / pose_hrnet).
 """
@@ -76,17 +77,20 @@ class FlipTestInference:
         res = {"idx": idx, "maxval": maxval, "avg_nhwc": avg, "nms_keep": keep, "nms_num": num}
         out_nchw = None
         if self.decode:
-            # the loss validate() computes: JointsMSELoss on the NCHW merged map (same kernel, same summation order)
+            # the loss validate() computes: the criterion on the NCHW merged map (same kernel, same summation order)
             out_nchw = ops.nhwc_to_nchw(avg)
             B, J = idx.shape
             tw = extra["target_weight"].reshape(B, J) if extra["use_target_weight"] else None
-            res["loss3"], _ = ops.joints_mse(out_nchw, extra["target"], tw, want_grad=False)
+            if extra["topk"]:
+                res["loss3"], _ = ops.joints_ohkm_mse(out_nchw, extra["target"], tw, extra["topk"], want_grad=False)
+            else:
+                res["loss3"], _ = ops.joints_mse(out_nchw, extra["target"], tw, want_grad=False)
             res["preds"] = ops.final_preds(avg, idx, maxval, extra["inv"], extra["post_process"])
             res["pck"], _ = ops.pck_counts(idx, maxval, extra["target"])
         self._keep = (ctx, ctx_f, nhwc, out_nchw)      # every intermediate stays referenced: the graph pool never recycles them
         return res
 
-    def _extra(self, inv, target, target_weight, use_target_weight, post_process, static):
+    def _extra(self, inv, target, target_weight, use_target_weight, post_process, topk, static):
         """The decode stage's inputs on the device: fresh copies, or refills of the graph's static buffers."""
         if not self.decode:
             return None
@@ -100,7 +104,8 @@ class FlipTestInference:
                 return torch.empty(tuple(t.shape), dtype=dtype, device=dev).copy_(t)
             return {"inv": own(inv, torch.float64), "target": own(target, torch.float32),
                     "target_weight": own(target_weight, torch.float32),
-                    "use_target_weight": bool(use_target_weight), "post_process": bool(post_process)}
+                    "use_target_weight": bool(use_target_weight), "post_process": bool(post_process),
+                    "topk": int(topk)}
         static["inv"].copy_(inv, non_blocking=True)
         static["target"].copy_(target, non_blocking=True)
         static["target_weight"].copy_(target_weight, non_blocking=True)
@@ -132,12 +137,13 @@ class FlipTestInference:
         self._staged_for = next_x
 
     def __call__(self, x, boxes_sorted=None, nms_thresh=0.6, next_x=None, inv=None, target=None, target_weight=None,
-                 use_target_weight=True, post_process=True):
+                 use_target_weight=True, post_process=True, topk=0):
         """x: [B,3,H,W] fp32, CUDA or pinned host. boxes_sorted: optional device [n,5] detector boxes sorted by score.
         next_x: optional pinned host tensor = the NEXT batch (its H2D copy overlaps this batch; pass it as `x` next time).
         With decode=True: inv host float64 [B,6] heat-map -> image matrices (lib.core.inference.inverse_affines of the
         batch's centres / scales), target [B,J,h,w] and target_weight [B,J,1] (host or device), use_target_weight (the
-        criterion's), post_process (config.TEST.POST_PROCESS).
+        criterion's), post_process (config.TEST.POST_PROCESS) and topk (the JointsOHKMMSELoss criterion's topk; 0 for
+        JointsMSELoss).
         Returns a dict of DEVICE tensors (static across calls in graph mode): idx int32 [B,J] (flat arg-max, first maximum),
         maxval [B,J], avg_nhwc [B,h,w,J] merged heat-maps, nms_keep / nms_num; with decode=True also preds [B,J,3]
         (get_final_preds: x, y, maxval), loss3 [3] (loss3[0] = the criterion's value) and pck int32 [J,2] (per joint:
@@ -146,17 +152,18 @@ class FlipTestInference:
         if not self.use_graph:
             xd = x.cuda(non_blocking=True).float().contiguous()
             return self._body(xd, boxes_sorted, self._extra(inv, target, target_weight, use_target_weight, post_process,
-                                                            None))
+                                                            topk, None))
         shape = (tuple(x.shape), None if boxes_sorted is None else tuple(boxes_sorted.shape), self.nms_thresh)
         if self.decode:
-            shape += (tuple(target.shape), tuple(target_weight.shape), bool(use_target_weight), bool(post_process))
+            shape += (tuple(target.shape), tuple(target_weight.shape), bool(use_target_weight), bool(post_process),
+                      int(topk))
         gen = self.net.engine().generation
         if self.graph is None or shape != self._shape or gen != self._gen:
             xd = x.cuda(non_blocking=True).float().contiguous()
             self.static_x = torch.empty_like(xd)
             self.static_x.copy_(xd)
             self.static_boxes = None if boxes_sorted is None else boxes_sorted.clone()
-            self.static_extra = self._extra(inv, target, target_weight, use_target_weight, post_process, None)
+            self.static_extra = self._extra(inv, target, target_weight, use_target_weight, post_process, topk, None)
             side = torch.cuda.Stream()
             side.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(side):
@@ -174,7 +181,7 @@ class FlipTestInference:
         self._stage(x)
         if boxes_sorted is not None:
             self.static_boxes.copy_(boxes_sorted, non_blocking=True)
-        self._extra(inv, target, target_weight, use_target_weight, post_process, self.static_extra)
+        self._extra(inv, target, target_weight, use_target_weight, post_process, topk, self.static_extra)
         self.graph.replay()
         self._prefetch(next_x)
         return self.result

@@ -7,9 +7,10 @@ What changes underneath:
     FPD loss+gradient kernel, the explicit backward tape -- and the gradients are handed to the caller's
     optimizer through .grad, so `optimizer.step()`, LR schedulers and checkpointing keep working. Any other
     model / criterion combination takes the generic autograd route, statement for statement like the reference.
+    The criteria may be JointsMSELoss or JointsOHKMMSELoss (online hard keypoint mining, any mix of the two under FPD).
   * per-iteration accuracy() and validate()'s flip test / decode run on the device; only [B,J] indices cross PCIe
     (the reference ships the full heat-maps to numpy every iteration: function.py:154-156, 218-240, 263).
-  * validate: for the fpd_b200 models with JointsMSELoss, each batch is one CUDA graph replay (infer_step.
+  * validate: for the fpd_b200 models with JointsMSELoss or JointsOHKMMSELoss, each batch is one CUDA graph replay (infer_step.
     FlipTestInference with its decode stage: both forwards, flip merge, loss, keypoints, PCK counts); the results are
     copied to pinned host buffers asynchronously and the host waits only to log and at the end of the epoch.
 """
@@ -71,11 +72,17 @@ def _is_fpd_net(model):
 
 
 def _is_fpd_criterion(c):
-    from .loss import JointsMSELoss
-    return isinstance(c, JointsMSELoss)
+    from .loss import JointsMSELoss, JointsOHKMMSELoss
+    return isinstance(c, (JointsMSELoss, JointsOHKMMSELoss))
 
 
-def _fused_step(model, tmodel, input, target, target_weight, alpha, use_tw):
+def _criterion_topk(c):
+    """The fused loss kernels' term selector: the criterion's topk for JointsOHKMMSELoss, 0 for JointsMSELoss."""
+    from .loss import JointsOHKMMSELoss
+    return c.topk if isinstance(c, JointsOHKMMSELoss) else 0
+
+
+def _fused_step(model, tmodel, input, target, target_weight, alpha, use_tw, pose_topk=0, kd_topk=0):
     """student fwd -> teacher fwd -> fused loss+grad -> backward tape; returns (losses[3] dev, last output NHWC)."""
     from fpd_b200 import ops
     net = _unwrap(model)
@@ -88,7 +95,8 @@ def _fused_step(model, tmodel, input, target, target_weight, alpha, use_tw):
         t_last = _unwrap(tmodel).forward_nhwc(x, training=False)[-1]
     B, _, _, J = outs[0].shape
     tw = target_weight.reshape(B, J) if use_tw else torch.ones(B, J, device=x.device)
-    losses, grads = ops.fpd_loss(outs, target.contiguous().float(), t_last, tw.contiguous().float(), alpha)
+    losses, grads = ops.fpd_loss(outs, target.contiguous().float(), t_last, tw.contiguous().float(), alpha,
+                                 pose_topk=pose_topk, kd_topk=kd_topk)
     pg = eng.backward(ctx, grads)
     params = [p for p in net.parameters() if p.requires_grad]      # frozen parameters keep whatever .grad they had
     glist = []
@@ -154,7 +162,7 @@ def _log_train(config, writer_dict, epoch, i, n_batches, batch_time, data_time, 
 
 
 def train(config, train_loader, model, criterion, optimizer, epoch, output_dir, tb_log_dir, writer_dict):
-    """Plain heat-map regression epoch (reference function.py:28-96): loss = sum over stacks of JointsMSELoss."""
+    """Plain heat-map regression epoch (reference function.py:28-96): loss = sum over stacks of the criterion."""
     batch_time, data_time, losses, acc = AverageMeter(), AverageMeter(), AverageMeter(), AverageMeter()
     model.train()
     fused = _is_fpd_net(model) and _is_fpd_criterion(criterion)
@@ -169,7 +177,8 @@ def train(config, train_loader, model, criterion, optimizer, epoch, output_dir, 
             shape_checked = True
         if fused:
             optimizer.zero_grad()
-            l3, out_nhwc = _fused_step(model, None, input, target, target_weight, 0.0, criterion.use_target_weight)
+            l3, out_nhwc = _fused_step(model, None, input, target, target_weight, 0.0, criterion.use_target_weight,
+                                       pose_topk=_criterion_topk(criterion))
             optimizer.step()
             losses.update(float(l3[2]), input.size(0))
             avg_acc, cnt, pred = _device_accuracy(out_nhwc, target)
@@ -222,7 +231,8 @@ def fpd_train(config, train_loader, model, tmodel, pose_criterion, kd_pose_crite
         if fused:
             optimizer.zero_grad()
             l3, out_nhwc = _fused_step(model, tmodel, input, target, target_weight, alpha,
-                                       pose_criterion.use_target_weight)
+                                       pose_criterion.use_target_weight, pose_topk=_criterion_topk(pose_criterion),
+                                       kd_topk=_criterion_topk(kd_pose_criterion))
             optimizer.step()
             pose_v, kd_v, loss_v = [float(v) for v in l3.cpu()]
             avg_acc, cnt, pred = _device_accuracy(out_nhwc, target)
@@ -281,6 +291,7 @@ class _GraphValidation:
         self.runner = FlipTestInference(net, val_dataset.flip_pairs, shift_heatmap=bool(config.TEST.SHIFT_HEATMAP),
                                         flip_test=bool(config.TEST.FLIP_TEST), decode=True)
         self.use_tw = criterion.use_target_weight
+        self.topk = _criterion_topk(criterion)
         self.post_process = bool(config.TEST.POST_PROCESS)
         self.preds = torch.empty((num_samples, J, 3), dtype=torch.float32, pin_memory=True)
         self.loss = torch.empty(num_batches, dtype=torch.float32, pin_memory=True)
@@ -292,7 +303,7 @@ class _GraphValidation:
     def run(self, i, input, target, target_weight, c, s, idx):
         B, _, h, w = target.shape
         r = self.runner(input, inv=inverse_affines(c, s, [w, h]), target=target, target_weight=target_weight,
-                        use_target_weight=self.use_tw, post_process=self.post_process)
+                        use_target_weight=self.use_tw, post_process=self.post_process, topk=self.topk)
         self.preds[idx:idx + B].copy_(r["preds"], non_blocking=True)
         self.loss[i:i + 1].copy_(r["loss3"][:1], non_blocking=True)
         self.counts[i].copy_(r["pck"], non_blocking=True)

@@ -554,9 +554,16 @@ def add(a, b, out=None):
     return o
 
 
+def _check_topk(topk, J, lo, name):
+    if int(topk) != topk or not lo <= topk <= J:
+        raise ValueError("%s=%r out of range [%d, J=%d]" % (name, topk, lo, J))
+    return int(topk)
+
+
 def fpd_loss(outs_nhwc, target_nchw, teacher_nhwc, target_weight, alpha, want_grads=True, grad_scale=1.0,
-             grads_out=None, losses_out=None):
-    """Fused FPD loss. outs_nhwc: list of [B,h,w,J]; returns (losses[3] device tensor, grads list or None)."""
+             grads_out=None, losses_out=None, pose_topk=0, kd_topk=0):
+    """Fused FPD loss. outs_nhwc: list of [B,h,w,J]; returns (losses[3] device tensor, grads list or None).
+    pose_topk / kd_topk > 0 make that term JointsOHKMMSELoss(topk) instead of JointsMSELoss (fpd_loss_ohkm_fused)."""
     S = len(outs_nhwc)
     B, h, w, J = outs_nhwc[0].shape
     dev = outs_nhwc[0].device
@@ -567,6 +574,16 @@ def fpd_loss(outs_nhwc, target_nchw, teacher_nhwc, target_weight, alpha, want_gr
         grads = grads_out if grads_out is not None else [torch.empty_like(o) for o in outs_nhwc]
     outs_arr = (ctypes.c_void_p * S)(*[o.data_ptr() for o in outs_nhwc])
     grads_arr = (ctypes.c_void_p * S)(*[g.data_ptr() for g in grads]) if grads is not None else None
+    if pose_topk or kd_topk:
+        pose_topk = _check_topk(pose_topk, J, 0, "pose_topk")
+        kd_topk = _check_topk(kd_topk, J, 0, "kd_topk")
+        for t in list(outs_nhwc) + [target_nchw, teacher_nhwc, tw]:
+            _chk(t, "fpd_loss argument")
+        ws = _ws.get(N.lib().fpd_loss_ohkm_workspace_bytes(S, B, J, h, w), dev)
+        N.check(N.lib().fpd_loss_ohkm_fused(outs_arr, S, _p(target_nchw), _p(teacher_nhwc), _p(tw), float(alpha),
+                                            grads_arr, float(grad_scale), _p(losses), B, J, h, w, pose_topk, kd_topk,
+                                            _p(ws), ws.numel(), _stream()), "loss_ohkm_fused")
+        return losses, grads
     ws = _ws.get(N.lib().fpd_loss_workspace_bytes(B, J, h, w), dev)
     N.check(N.lib().fpd_loss_fused(outs_arr, S, _p(target_nchw), _p(teacher_nhwc), _p(tw), float(alpha), grads_arr,
                                    float(grad_scale), _p(losses), B, J, h, w, _p(ws), ws.numel(), _stream()),
@@ -584,6 +601,28 @@ def joints_mse(out_nchw, target_nchw, target_weight=None, want_grad=True):
     ws = _ws.get(1 << 16, dev)
     N.check(N.lib().fpd_joints_mse(_p(out_nchw), _p(target_nchw), _p(tw), _p(loss3), _p(grad), B, J, hw, _p(ws),
                                    ws.numel(), _stream()), "joints_mse")
+    return loss3, grad
+
+
+def joints_ohkm_mse(out_nchw, target_nchw, target_weight=None, topk=8, want_grad=True):
+    """JointsOHKMMSELoss (lib/core/loss.py:42-87) on NCHW tensors: per sample the mean of the topk largest per-joint
+    losses, averaged over the batch. Returns (loss3 device tensor, loss3[0] the value; grad [B,J,h,w] or None)."""
+    _chk(out_nchw, "out")
+    _chk(target_nchw, "target")
+    if out_nchw.dim() < 3 or out_nchw.shape[0] * out_nchw.shape[1] == 0 or target_nchw.shape != out_nchw.shape:
+        raise ValueError("out / target must be non-empty [B,J,...] tensors of one shape (got %s, %s)"
+                         % (tuple(out_nchw.shape), tuple(target_nchw.shape)))
+    B, J = out_nchw.shape[:2]
+    topk = _check_topk(topk, J, 1, "topk")
+    hw = out_nchw.numel() // (B * J)
+    dev = out_nchw.device
+    loss3 = torch.empty(3, dtype=torch.float32, device=dev)
+    grad = torch.empty_like(out_nchw) if want_grad else None
+    tw = None if target_weight is None else target_weight.reshape(B, J).contiguous()
+    _chk(tw, "target_weight")
+    ws = _ws.get(N.lib().fpd_joints_ohkm_workspace_bytes(B, J), dev)
+    N.check(N.lib().fpd_joints_ohkm(_p(out_nchw), _p(target_nchw), _p(tw), topk, _p(loss3), _p(grad), B, J, hw, _p(ws),
+                                    ws.numel(), _stream()), "joints_ohkm")
     return loss3, grad
 
 

@@ -254,6 +254,27 @@ int fpd_loss_fused(const float* const* outs_host, int S, const float* target_nch
 int fpd_joints_mse(const float* out_nchw, const float* target_nchw, const float* target_weight, float* loss3,
                    float* grad, int B, int J, int hw, void* workspace, size_t workspace_bytes, fpd_stream_t stream);
 
+/* Online hard keypoint mining, lib/core/loss.py:42-87 (JointsOHKMMSELoss): per joint
+ * l[b,j] = 0.5 * mean_p (w*out - w*ref)^2, per sample the mean of the topk largest l[b,.], averaged over the batch
+ * (no division by J). Joints are ranked by the fp32-rounded l; on exact ties the lower joint index wins. Joints
+ * left out get an exactly zero gradient. Needs 1 <= J <= 64 and B >= 1 (B = 1 works; the reference's squeeze()
+ * fails there). Deterministic: fixed-order fp64 sums, no floating-point atomics.
+ *
+ * Fused FPD form: the arguments of fpd_loss_fused plus pose_topk / kd_topk, each in [0, J]; 0 makes that term plain
+ * JointsMSELoss. kd_topk > 0 needs a teacher. losses[3] = {pose, kd, total} with pose = sum_s crit(out_s, target).
+ * Same shape limits as fpd_loss_fused (h*w % 64 == 0, J <= 64, S <= 8). */
+size_t fpd_loss_ohkm_workspace_bytes(int S, int B, int J, int h, int w);
+int fpd_loss_ohkm_fused(const float* const* outs_host, int S, const float* target_nchw, const float* teacher_nhwc,
+                        const float* target_weight, float alpha, float* const* grads_host, float grad_scale,
+                        float* losses, int B, int J, int h, int w, int pose_topk, int kd_topk, void* workspace,
+                        size_t workspace_bytes, fpd_stream_t stream);
+/* Module form on NCHW tensors, like fpd_joints_mse: topk in [1, J]; loss3 (device, 3 floats, [0] is the loss);
+ * grad (optional) = dloss/dout, written everywhere; target_weight NULL = use_target_weight False. */
+size_t fpd_joints_ohkm_workspace_bytes(int B, int J);
+int fpd_joints_ohkm(const float* out_nchw, const float* target_nchw, const float* target_weight, int topk,
+                    float* loss3, float* grad, int B, int J, int hw, void* workspace, size_t workspace_bytes,
+                    fpd_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------------------
  * Decode. Replaces the numpy round-trips of lib/core/function.py:218-240 (flip test),
  * lib/utils/transforms.py:15-29 (flip_back) and lib/core/inference.py:18-46 (get_max_preds).
