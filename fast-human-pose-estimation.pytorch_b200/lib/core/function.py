@@ -10,6 +10,11 @@ What changes underneath:
     The criteria may be JointsMSELoss or JointsOHKMMSELoss (online hard keypoint mining, any mix of the two under FPD).
   * per-iteration accuracy() and validate()'s flip test / decode run on the device; only [B,J] indices cross PCIe
     (the reference ships the full heat-maps to numpy every iteration: function.py:154-156, 218-240, 263).
+  * train / fpd_train: on the fused route each batch of the epoch's batch shape is one CUDA graph replay (train_step.
+    FPDTrainStep in its external-optimizer mode: student forward, teacher forward on a side stream, loss, backward tape
+    with the weight gradients on their own stream, PCK counts); the caller's optimizer then steps on the gradients. Losses
+    and counts go to pinned host buffers asynchronously; the host waits only to log and at the end of the epoch. Other
+    batch shapes (the short last batch) and config.DEBUG.DEBUG take the eager fused route, which gives the same bits.
   * validate: for the fpd_b200 models with JointsMSELoss or JointsOHKMMSELoss, each batch is one CUDA graph replay (infer_step.
     FlipTestInference with its decode stage: both forwards, flip merge, loss, keypoints, PCK counts); the results are
     copied to pinned host buffers asynchronously and the host waits only to log and at the end of the epoch.
@@ -82,8 +87,12 @@ def _criterion_topk(c):
     return c.topk if isinstance(c, JointsOHKMMSELoss) else 0
 
 
-def _fused_step(model, tmodel, input, target, target_weight, alpha, use_tw, pose_topk=0, kd_topk=0):
-    """student fwd -> teacher fwd -> fused loss+grad -> backward tape; returns (losses[3] dev, last output NHWC)."""
+def _fused_step(model, tmodel, input, target, target_weight, alpha, use_tw, graph=None, pose_topk=0, kd_topk=0):
+    """student fwd -> teacher fwd -> fused loss+grad -> backward tape; returns (losses[3] dev, last output NHWC).
+    graph: a _GraphTraining whose batch shape this batch has -- the same step is then one replay of its graph, and the
+    last output is None (the PCK counts come out of the graph instead)."""
+    if graph is not None:
+        return graph.step(input, target, target_weight), None
     from fpd_b200 import ops
     net = _unwrap(model)
     x = input.cuda(non_blocking=True).float().contiguous()
@@ -111,6 +120,78 @@ def _fused_step(model, tmodel, input, target, target_weight, alpha, use_tw, pose
     for p, g in zip(params, glist):
         p.grad = g
     return losses, outs[-1]
+
+
+# train() / fpd_train() replay one CUDA graph per batch where they can; False forces the eager fused route (the graph
+# route's reference in the tests)
+_TRAIN_GRAPH = True
+_train_step_cache = {}      # key -> FPDTrainStep: one captured step, reused across epochs (it keeps the networks alive)
+
+
+def _train_route(config, model, tmodel, criteria, target_shape):
+    """'graph', 'fused' or 'generic' for a train (tmodel None, one criterion) / fpd_train epoch whose first batch has
+    targets of `target_shape`. The graph route replays exactly the eager fused route's kernels; debug images need the
+    heat-maps on the host every logged step, so config.DEBUG.DEBUG keeps the eager fused route."""
+    fused = (_is_fpd_net(model) and (tmodel is None or _is_fpd_net(tmodel)) and all(_is_fpd_criterion(c) for c in criteria)
+             and len({c.use_target_weight for c in criteria}) == 1
+             and _loss_shape_ok(config, target_shape[1], target_shape[2], target_shape[3]))
+    if not fused:
+        return "generic"
+    dbg = getattr(config, "DEBUG", None)
+    return "graph" if _TRAIN_GRAPH and not (dbg is not None and getattr(dbg, "DEBUG", False)) else "fused"
+
+
+class _GraphTraining:
+    """train()/fpd_train()'s per-batch work as replays of one FPDTrainStep(fused_adam=False, accuracy=True), which is
+    cached across calls keyed on the networks, the batch shapes, alpha and the topks. Losses and PCK counts go to pinned
+    host buffers with non-blocking copies; `flush` waits for them and applies the meter updates in batch order."""
+
+    def __init__(self, model, tmodel, alpha, use_tw, pose_topk, kd_topk, input, target, target_weight, num_batches):
+        from fpd_b200.train_step import FPDTrainStep
+        net = _unwrap(model)
+        tnet = _unwrap(tmodel) if tmodel is not None else None
+        self.shapes = (tuple(input.shape), tuple(target.shape), tuple(target_weight.shape))
+        alpha = float(alpha) if tnet is not None else 0.0
+        key = (id(net), id(tnet), self.shapes, alpha, pose_topk, kd_topk)
+        step = _train_step_cache.get(key)
+        if step is None:
+            _train_step_cache.clear()          # one graph pool at a time
+            step = _train_step_cache[key] = FPDTrainStep(net, tnet, alpha=alpha, pose_topk=pose_topk, kd_topk=kd_topk,
+                                                         fused_adam=False, accuracy=True)
+        self.train_step = step
+        self.trainable = [(p, g) for p, g in zip(step.params, step.grad_views) if p.requires_grad]
+        B, J = target.shape[0], target.shape[1]
+        self.ones = None if use_tw else torch.ones(B, J, device=target.device)
+        self.loss = torch.empty((num_batches, 3), dtype=torch.float32, pin_memory=True)
+        self.counts = torch.empty((num_batches, J, 2), dtype=torch.int32, pin_memory=True)
+        self.done = torch.cuda.Event()
+        self.pending = []          # (batch, num_images) not yet applied to the meters
+
+    def accepts(self, input, target, target_weight):
+        return (tuple(input.shape), tuple(target.shape), tuple(target_weight.shape)) == self.shapes
+
+    def step(self, input, target, target_weight):
+        """Replay (gradients all-reduced when there are several ranks) and hand the gradients to the parameters'
+        .grad, as _fused_step does; returns the device losses[3]."""
+        l3 = self.train_step.step(input, target, target_weight if self.ones is None else self.ones)
+        for p, g in self.trainable:     # frozen parameters keep whatever .grad they had
+            p.grad = g
+        return l3
+
+    def record(self, i, l3, num_images):
+        """Queue batch i's losses and PCK counts for the host (call after the optimizer step)."""
+        self.loss[i].copy_(l3, non_blocking=True)
+        self.counts[i].copy_(self.train_step.counts, non_blocking=True)
+        self.pending.append((i, num_images))
+
+    def flush(self, apply):
+        """apply(losses[3] as floats, avg_acc, cnt, num_images) for every pending batch, in batch order."""
+        self.done.record()
+        self.done.synchronize()
+        for i, n in self.pending:
+            _, avg_acc, cnt = pck_from_counts(self.counts[i].numpy())
+            apply([float(v) for v in self.loss[i]], avg_acc, cnt, n)
+        self.pending = []
 
 
 def _device_accuracy(out_nhwc, target_nchw):
@@ -168,18 +249,39 @@ def train(config, train_loader, model, criterion, optimizer, epoch, output_dir, 
     fused = _is_fpd_net(model) and _is_fpd_criterion(criterion)
     end = time.time()
     shape_checked = False
+    graph = None
+
+    def apply(l3, avg_acc, cnt, n):
+        losses.update(l3[2], n)
+        acc.update(avg_acc, cnt)
     for i, (input, target, target_weight, meta) in enumerate(train_loader):
         data_time.update(time.time() - end)
         target = target.cuda(non_blocking=True)
         target_weight = target_weight.cuda(non_blocking=True)
         if fused and not shape_checked:
-            fused = _loss_shape_ok(config, target.shape[1], target.shape[2], target.shape[3])
+            route = _train_route(config, model, None, [criterion], target.shape)
+            fused = route != "generic"
             shape_checked = True
+            if route == "graph":
+                graph = _GraphTraining(model, None, 0.0, criterion.use_target_weight, _criterion_topk(criterion), 0,
+                                       input, target, target_weight, len(train_loader))
+        replay = graph if graph is not None and graph.accepts(input, target, target_weight) else None
+        if graph is not None and replay is None:
+            graph.flush(apply)          # meter updates stay in batch order
         if fused:
             optimizer.zero_grad()
             l3, out_nhwc = _fused_step(model, None, input, target, target_weight, 0.0, criterion.use_target_weight,
-                                       pose_topk=_criterion_topk(criterion))
+                                       replay, pose_topk=_criterion_topk(criterion))
             optimizer.step()
+            if replay is not None:
+                replay.record(i, l3, input.size(0))
+                batch_time.update(time.time() - end)
+                end = time.time()
+                if i % config.PRINT_FREQ == 0:
+                    replay.flush(apply)
+                    _log_train(config, writer_dict, epoch, i, len(train_loader), batch_time, data_time,
+                               [('Loss', losses, '%.5f'), ('Accuracy', acc, '%.3f')], input.size(0))
+                continue
             losses.update(float(l3[2]), input.size(0))
             avg_acc, cnt, pred = _device_accuracy(out_nhwc, target)
             output = out_nhwc
@@ -205,6 +307,8 @@ def train(config, train_loader, model, criterion, optimizer, epoch, output_dir, 
             _log_train(config, writer_dict, epoch, i, len(train_loader), batch_time, data_time,
                        [('Loss', losses, '%.5f'), ('Accuracy', acc, '%.3f')], input.size(0))
             _debug_images(config, input, meta, target, pred, output.detach(), '{}_{}'.format(os.path.join(output_dir, 'train'), i))
+    if graph is not None:
+        graph.flush(apply)
 
 
 def fpd_train(config, train_loader, model, tmodel, pose_criterion, kd_pose_criterion, optimizer, epoch,
@@ -221,19 +325,45 @@ def fpd_train(config, train_loader, model, tmodel, pose_criterion, kd_pose_crite
              and pose_criterion.use_target_weight == kd_pose_criterion.use_target_weight)
     end = time.time()
     shape_checked = False
+    graph = None
+    meters = [('POSE_Loss', pose_losses, '%.5f'), ('KD_POSE_Loss', kd_pose_losses, '%.5f'), ('Loss', losses, '%.5f'),
+              ('Accuracy', acc, '%.3f')]
+
+    def apply(l3, avg_acc, cnt, n):
+        pose_losses.update(l3[0], n)
+        kd_pose_losses.update(l3[1], n)
+        losses.update(l3[2], n)
+        acc.update(avg_acc, cnt)
     for i, (input, target, target_weight, meta) in enumerate(train_loader):
         data_time.update(time.time() - end)
         target = target.cuda(non_blocking=True)
         target_weight = target_weight.cuda(non_blocking=True)
         if fused and not shape_checked:
-            fused = _loss_shape_ok(config, target.shape[1], target.shape[2], target.shape[3])
+            route = _train_route(config, model, tmodel, [pose_criterion, kd_pose_criterion], target.shape)
+            fused = route != "generic"
             shape_checked = True
+            if route == "graph":
+                graph = _GraphTraining(model, tmodel, alpha, pose_criterion.use_target_weight,
+                                       _criterion_topk(pose_criterion), _criterion_topk(kd_pose_criterion),
+                                       input, target, target_weight, len(train_loader))
+        replay = graph if graph is not None and graph.accepts(input, target, target_weight) else None
+        if graph is not None and replay is None:
+            graph.flush(apply)          # meter updates stay in batch order
         if fused:
             optimizer.zero_grad()
             l3, out_nhwc = _fused_step(model, tmodel, input, target, target_weight, alpha,
-                                       pose_criterion.use_target_weight, pose_topk=_criterion_topk(pose_criterion),
+                                       pose_criterion.use_target_weight, replay, pose_topk=_criterion_topk(pose_criterion),
                                        kd_topk=_criterion_topk(kd_pose_criterion))
             optimizer.step()
+            if replay is not None:
+                replay.record(i, l3, input.size(0))
+                batch_time.update(time.time() - end)
+                end = time.time()
+                if i % config.PRINT_FREQ == 0:
+                    replay.flush(apply)
+                    _log_train(config, writer_dict, epoch, i, len(train_loader), batch_time, data_time, meters,
+                               input.size(0))
+                continue
             pose_v, kd_v, loss_v = [float(v) for v in l3.cpu()]
             avg_acc, cnt, pred = _device_accuracy(out_nhwc, target)
             last_out = out_nhwc
@@ -263,10 +393,10 @@ def fpd_train(config, train_loader, model, tmodel, pose_criterion, kd_pose_crite
         batch_time.update(time.time() - end)
         end = time.time()
         if i % config.PRINT_FREQ == 0:
-            _log_train(config, writer_dict, epoch, i, len(train_loader), batch_time, data_time,
-                       [('POSE_Loss', pose_losses, '%.5f'), ('KD_POSE_Loss', kd_pose_losses, '%.5f'),
-                        ('Loss', losses, '%.5f'), ('Accuracy', acc, '%.3f')], input.size(0))
+            _log_train(config, writer_dict, epoch, i, len(train_loader), batch_time, data_time, meters, input.size(0))
             _debug_images(config, input, meta, target, pred, last_out, '{}_{}'.format(os.path.join(output_dir, 'train'), i))
+    if graph is not None:
+        graph.flush(apply)
 
 
 # validate() replays one CUDA graph per batch where it can; False forces the eager fused route (the graph route's

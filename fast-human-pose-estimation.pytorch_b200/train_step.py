@@ -9,6 +9,11 @@ eager ATen launches plus a DataParallel replicate/scatter/gather. Here the same 
     [NCCL all-reduce of the flat gradient buffer when world_size > 1]
     one fused Adam launch over the flat parameter buffer
 
+With fused_adam=False the step stops after the all-reduce: the parameters keep their own storage and the caller's
+optimizer (any torch.optim optimizer, its state dict, LR schedules) steps on the per-parameter views of the flat gradient
+buffer -- lib/core/function.py's train / fpd_train run this way. pose_topk / kd_topk select JointsOHKMMSELoss for a term;
+accuracy=True adds accuracy()'s PCK counts of the last stack to the graph.
+
 The teacher is forward-only (its gradients never influence the student update; the reference's teacher
 backward is wasted work). `plain=True` drops the teacher (function.train semantics,
 function.py:44-63).
@@ -26,9 +31,10 @@ SHARE_STEM = os.environ.get("FPD_SHARE_STEM", "1") != "0"   # student + teacher 
 class FlatParams:
     """Re-homes a module's parameters as views into one flat fp32 buffer (needed for the single all-reduce and the
     single Adam launch). Parameter objects are preserved (only .data changes), so optimizers / state_dict keep
-    working."""
+    working. rehome=False keeps the parameters' own storage and builds only the flat gradient buffer (`flat` is then
+    None)."""
 
-    def __init__(self, net):
+    def __init__(self, net, rehome=True):
         self.params = [p for p in net.parameters()]
         dev = self.params[0].device
         sizes = [p.numel() for p in self.params]
@@ -39,33 +45,57 @@ class FlatParams:
             self.offsets.append(off)
             off += (n + 3) // 4 * 4
         self.numel = off
-        self.flat = torch.zeros(off, dtype=torch.float32, device=dev)
+        self.flat = torch.zeros(off, dtype=torch.float32, device=dev) if rehome else None
         self.grad = torch.zeros(off, dtype=torch.float32, device=dev)
         self.grad_views = []
         for p, o in zip(self.params, self.offsets):
-            v = self.flat[o:o + p.numel()].view(p.shape)
-            v.copy_(p.data)
-            p.data = v
+            if rehome:
+                v = self.flat[o:o + p.numel()].view(p.shape)
+                v.copy_(p.data)
+                p.data = v
             self.grad_views.append(self.grad[o:o + p.numel()].view(p.shape))
 
     def is_intact(self):
+        if self.flat is None:
+            return True
         base = self.flat.untyped_storage().data_ptr()
         return all(p.data.untyped_storage().data_ptr() == base for p in self.params)
 
 
+def _check_topk(value, name):
+    """0 = JointsMSELoss for that term, k >= 1 = JointsOHKMMSELoss(topk=k); the kernels take J <= 64 (the upper bound J
+    itself is checked against the heat-maps by ops.fpd_loss)."""
+    if isinstance(value, bool) or int(value) != value or not 0 <= value <= 64:
+        raise ValueError("%s=%r must be an integer in [0, 64] (0: JointsMSELoss)" % (name, value))
+    return int(value)
+
+
 class FPDTrainStep:
     def __init__(self, student, teacher=None, alpha=0.5, lr=2.5e-4, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0,
-                 process_group=None, use_graph=True):
+                 process_group=None, use_graph=True, pose_topk=0, kd_topk=0, fused_adam=True, accuracy=False):
+        """pose_topk / kd_topk: > 0 makes that loss term JointsOHKMMSELoss(topk) instead of JointsMSELoss.
+        fused_adam=False (external-optimizer mode): step() stops once the gradients are in the flat gradient buffer
+        (all-reduced, mean over ranks); the parameters keep their own storage and the caller's optimizer steps on
+        `grad_views`. lr / betas / eps / weight_decay are then unused.
+        accuracy=True: the step also computes accuracy()'s per-joint PCK counts of the last stack (`counts`, int32 [J,2],
+        lib.core.evaluate.pck_from_counts)."""
+        pose_topk, kd_topk = _check_topk(pose_topk, "pose_topk"), _check_topk(kd_topk, "kd_topk")
+        if kd_topk and teacher is None:
+            raise ValueError("kd_topk=%d needs a teacher" % kd_topk)
         self.student, self.teacher = student, teacher
         self.alpha = float(alpha) if teacher is not None else 0.0
         self.lr, self.betas, self.eps, self.wd = lr, betas, eps, weight_decay
+        self.pose_topk, self.kd_topk = pose_topk, kd_topk
+        self.fused_adam = bool(fused_adam)
+        self.want_accuracy = bool(accuracy)
+        self.counts = None
         self.pg = process_group
         self.world = 1
         if process_group is not None or (torch.distributed.is_available() and torch.distributed.is_initialized()):
             self.world = torch.distributed.get_world_size(process_group)
-        self.flat = FlatParams(student)
-        self.exp_avg = torch.zeros_like(self.flat.flat)
-        self.exp_avg_sq = torch.zeros_like(self.flat.flat)
+        self.flat = FlatParams(student, rehome=self.fused_adam)
+        self.exp_avg = torch.zeros_like(self.flat.flat) if self.fused_adam else None
+        self.exp_avg_sq = torch.zeros_like(self.flat.flat) if self.fused_adam else None
         self.step_count = 0
         self.use_graph = use_graph
         self.graph = None
@@ -79,6 +109,7 @@ class FPDTrainStep:
         self.x_next = self.t_cur = self.t_next = None
         self._have_next = False
         self._static_shapes = None
+        self._static_ptrs = None
         self._teacher_gen = 0
         self._stage_x = self._copy_stream = self._stage_ev = self._stage_free = None   # next batch's images, prefetched
         self._staged_for = None
@@ -109,7 +140,7 @@ class FPDTrainStep:
             self.t_next.copy_(t_ctx.outs[-1].data)
         ctx = s_eng.forward(x, True, record_tape=True)
         outs = [v.data for v in ctx.outs]
-        losses, grads = ops.fpd_loss(outs, target, self.t_cur, tw, self.alpha, losses_out=self.losses)
+        losses, grads = self._loss(outs, target, self.t_cur, tw)
         pg = s_eng.backward(ctx, grads, wgrad_stream=self._wstream)
         self._gather_grads(pg)
         main.wait_stream(self._side)
@@ -153,10 +184,28 @@ class FPDTrainStep:
                 t_last = t_ctx.outs[-1].data
         outs = [v.data for v in ctx.outs]
         self.last_outs, self.last_teacher = outs, t_last
-        losses, grads = ops.fpd_loss(outs, target, t_last, tw, self.alpha, losses_out=self.losses)
+        losses, grads = self._loss(outs, target, t_last, tw)
         pg = s_eng.backward(ctx, grads, wgrad_stream=self._wstream)
         self._gather_grads(pg)
         return losses
+
+    def _loss(self, outs, target, t_last, tw):
+        """The fused FPD loss and its gradients (+ the PCK counts of the last stack when accuracy=True)."""
+        if self.pose_topk or self.kd_topk:
+            losses, grads = ops.fpd_loss(outs, target, t_last, tw, self.alpha, losses_out=self.losses,
+                                         pose_topk=self.pose_topk, kd_topk=self.kd_topk)
+        else:
+            losses, grads = ops.fpd_loss(outs, target, t_last, tw, self.alpha, losses_out=self.losses)
+        if self.want_accuracy:
+            _, idx, maxval = ops.flip_merge_argmax(outs[-1], want_avg=False)
+            ops.pck_counts(idx, maxval, target, out=self.counts)
+        return losses, grads
+
+    def _outputs(self, target):
+        """The step's device outputs: losses[3] and, with accuracy=True, the PCK counts [J,2]."""
+        self.losses = torch.zeros(3, dtype=torch.float32, device=target.device)
+        if self.want_accuracy:
+            self.counts = torch.zeros((target.shape[1], 2), dtype=torch.int32, device=target.device)
 
     def _run_body(self):
         if self.pipeline:
@@ -167,7 +216,7 @@ class FPDTrainStep:
         self.static = (torch.empty_like(x), torch.empty_like(target), torch.empty_like(tw))
         for s, v in zip(self.static, (x, target, tw)):
             s.copy_(v)
-        self.losses = torch.zeros(3, dtype=torch.float32, device=x.device)
+        self._outputs(target)
         if self.pipeline:
             self.x_next = x.clone()
             with torch.no_grad():
@@ -187,7 +236,7 @@ class FPDTrainStep:
         self.graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.graph):
             self._run_body()
-        self.launches_per_step = int(N.lib().fpd_launch_count() - n0) + 1  # + the Adam launch
+        self.launches_per_step = int(N.lib().fpd_launch_count() - n0) + int(self.fused_adam)  # + the Adam launch
         self._restore_bn(self._saved_bn)  # capture does not execute, but keep host-side state tidy
 
     def _snapshot_bn(self):
@@ -205,19 +254,26 @@ class FPDTrainStep:
         under this step, and the following call must pass that same tensor as `x`.
         With teacher pipelining (`pipeline=True`) pass `next_x`, the NEXT step's images (what a prefetching loader has at
         hand anyway): the teacher runs on them while the student trains on `x`, and the following call must pass that
-        same batch as `x`. Without `next_x` the teacher for the following step is run up front (no overlap)."""
+        same batch as `x`. Without `next_x` the teacher for the following step is run up front (no overlap).
+        With fused_adam=False the step ends with the gradients in `grad_views` (mean over ranks); the caller's optimizer
+        does the update."""
         tw = target_weight.reshape(target_weight.shape[0], -1)
         if self.use_graph:
             shapes = (tuple(x.shape), tuple(target.shape), tuple(tw.shape))
             t_gen = self.teacher.engine().generation if self.teacher is not None else 0
-            if self.graph is not None and (shapes != self._static_shapes or t_gen != self._teacher_gen):
-                # a short last batch / a different resolution, or teacher weights reloaded after capture (the graph holds
-                # pointers to the teacher's prepared weights): capture again instead of broadcasting or using stale data
+            # fused-Adam mode owns the parameters' storage (FlatParams); otherwise the caller may give them new storage
+            ptrs = None if self.fused_adam else self._student_ptrs()
+            if self.graph is not None and (shapes != self._static_shapes or t_gen != self._teacher_gen
+                                           or ptrs != self._static_ptrs):
+                # a short last batch / a different resolution, teacher weights reloaded after capture (the graph holds
+                # pointers to the teacher's prepared weights), or a student parameter / buffer given new storage (the
+                # graph holds its old address): capture again instead of broadcasting or using stale data
                 self.graph = None
             if self.graph is None:
                 xd, td, wd = (t.cuda(non_blocking=True).float().contiguous() for t in (x, target, tw))
                 self._capture(xd, td, wd)
                 self._static_shapes = shapes
+                self._static_ptrs = ptrs
                 self._teacher_gen = self.teacher.engine().generation if self.teacher is not None else 0
                 self._have_next = False
             if self.pipeline:
@@ -243,22 +299,41 @@ class FPDTrainStep:
             losses = self.losses
         else:
             xd, td, wd = (t.cuda(non_blocking=True).float().contiguous() for t in (x, target, tw))
-            if self.losses is None:
-                self.losses = torch.zeros(3, dtype=torch.float32, device=xd.device)
+            if self.losses is None or (self.want_accuracy and self.counts.shape[0] != td.shape[1]):
+                self._outputs(td)
             n0 = N.lib().fpd_launch_count()
             losses = self._body(xd, td, wd)
-            self.launches_per_step = int(N.lib().fpd_launch_count() - n0) + 1
-        gscale = 1.0
-        if self.world > 1:
-            from .parallel import allreduce_mean_
-            gscale = allreduce_mean_(self.flat.grad, self.pg)
-        self.step_count += 1
-        ops.adam_flat(self.flat.flat, self.flat.grad, self.exp_avg, self.exp_avg_sq, self.lr, self.betas[0],
-                      self.betas[1], self.eps, self.wd, self.step_count, grad_scale=gscale)
+            self.launches_per_step = int(N.lib().fpd_launch_count() - n0) + int(self.fused_adam)
+        if self.fused_adam:
+            gscale = 1.0
+            if self.world > 1:
+                from .parallel import allreduce_mean_
+                gscale = allreduce_mean_(self.flat.grad, self.pg)
+            self.step_count += 1
+            ops.adam_flat(self.flat.flat, self.flat.grad, self.exp_avg, self.exp_avg_sq, self.lr, self.betas[0],
+                          self.betas[1], self.eps, self.wd, self.step_count, grad_scale=gscale)
+        else:
+            if self.world > 1:
+                # the same two operations as DistributedDataParallel's averaging (and lib.core.function's eager route)
+                torch.distributed.all_reduce(self.flat.grad, op=torch.distributed.ReduceOp.SUM, group=self.pg)
+                self.flat.grad.mul_(1.0 / self.world)
         # weights and running statistics were just rewritten through raw pointers (and, in graph mode, without running any
         # Python): drop the student's cached eval-mode operands so a following validation sees the new values
         self.student.engine().invalidate_eval_cache()
         return losses
+
+    @property
+    def params(self):
+        """The student's parameters, in the order of `grad_views`."""
+        return self.flat.params
+
+    @property
+    def grad_views(self):
+        """Per-parameter views of the flat gradient buffer (rewritten by every step; clone to keep one)."""
+        return self.flat.grad_views
+
+    def _student_ptrs(self):
+        return tuple(t.data_ptr() for t in self.flat.params) + tuple(b.data_ptr() for b in self.student.buffers())
 
     # ------------------------------------------------------------------ host batches: H2D of batch i+1 under step i
     def _stage_inputs(self, x, target, tw):
@@ -299,14 +374,20 @@ class FPDTrainStep:
     # ------------------------------------------------------------------ checkpointing (the reference saves
     # optimizer.state_dict() next to the model, lib/utils/utils.py:75-84 / tools/fpd_train.py:277-291)
     def state_dict(self):
+        self._need_fused_adam()
         return {"step": self.step_count, "exp_avg": self.exp_avg.clone(), "exp_avg_sq": self.exp_avg_sq.clone(),
                 "lr": self.lr, "betas": tuple(self.betas), "eps": self.eps, "weight_decay": self.wd,
                 "numel": self.flat.numel}
 
     def load_state_dict(self, sd):
+        self._need_fused_adam()
         if int(sd["numel"]) != self.flat.numel:
             raise ValueError("optimizer state is for %d flat parameters, this step has %d" % (sd["numel"], self.flat.numel))
         self.step_count = int(sd["step"])
         self.exp_avg.copy_(sd["exp_avg"])
         self.exp_avg_sq.copy_(sd["exp_avg_sq"])
         self.lr, self.betas, self.eps, self.wd = sd["lr"], tuple(sd["betas"]), sd["eps"], sd["weight_decay"]
+
+    def _need_fused_adam(self):
+        if not self.fused_adam:
+            raise RuntimeError("FPDTrainStep(fused_adam=False) has no optimizer state: checkpoint the caller's optimizer")
