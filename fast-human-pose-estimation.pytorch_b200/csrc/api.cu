@@ -61,6 +61,8 @@ int fpd_conv2d_tc_h(const float* x, const float* pre_mean, const float* pre_scal
                           out_scale, in_scale, B, H, W, Cin, Cout, ksize, device_sm_count(), S(stream));
 }
 
+int fpd_set_conv1x1(int enabled) { return set_conv1x1(enabled); }
+
 int fpd_conv2d_tc_h_stats_blocks(int B, int H, int W, int Cin, int Cout, int ksize, int f16) {
   return conv_tc_h_stats_grid(B, H, W, Cin, Cout, ksize, f16, device_sm_count());
 }

@@ -27,6 +27,9 @@ int conv_tc_h_launch(const float* x, const float* pre_mean, const float* pre_sca
 // BatchNorm statistics of the OUTPUT from the epilogue: number of per-CTA partial blocks the launch writes to
 // stat_part[blocks][Cout][2] (0: this shape cannot carry the statistics, e.g. Cout > 256)
 int conv_tc_h_stats_grid(int B, int H, int W, int Cin, int Cout, int ksize, int f16, int num_sms);
+// 1x1 3xFP16 convolutions without statistics: the weight-resident kernel (1, the default) or the staged kernel (0),
+// process-wide; returns the previous setting
+int set_conv1x1(int enabled);
 
 // ---- conv_wgmma.cu : warpgroup-MMA weight-gradient GEMM (K = pixels) reading RAW x and dY; BN-apply + ReLU + tf32 split
 //      fused into the operand staging ----

@@ -156,6 +156,23 @@ CONV_F16 = os.environ.get("FPD_CONV_F16", "1") != "0"      # 3xFP16 operands for
 CONV_F16_DGRAD = os.environ.get("FPD_CONV_F16_DGRAD", "1") != "0"   # ... and for the data-gradient convolutions (dY * 2^k)
 
 
+CONV1X1 = os.environ.get("FPD_CONV1X1", "1") != "0"   # 1x1 3xFP16 convolutions on the weight-resident kernel
+
+
+def set_conv1x1(enabled):
+    """Run 1x1 3xFP16 convolutions (without epilogue statistics) on the weight-resident kernel (True) or on the staged
+    kernel (False), process-wide, for launches made after the call. The results are bit-identical. Returns the previous
+    setting."""
+    global CONV1X1
+    prev = bool(N.lib().fpd_set_conv1x1(int(bool(enabled))))
+    CONV1X1 = bool(enabled)
+    return prev
+
+
+if not CONV1X1:
+    set_conv1x1(False)
+
+
 def conv2d_tc_h_supported(cin, cout, k, H, W, f16):
     return CONV_H and bool(N.lib().fpd_conv2d_tc_h_supported(cin, cout, k, H, W, int(f16)))
 

@@ -74,6 +74,10 @@ int fpd_conv2d_tc_h(const float* x, const float* pre_mean, const float* pre_scal
                     int pre_relu, const void* w_hi, const void* w_lo, int f16, const float* bias,
                     const float* residual, const float* relu_mask, float* y, float out_scale, const float* in_scale,
                     int B, int H, int W, int Cin, int Cout, int ksize, fpd_stream_t stream);
+/* 1x1 convolutions with 3xFP16 operands and no statistics run on a kernel that keeps the weights of its output slice in
+ * shared memory, where they fit (enabled = 1, the default), or on the staged kernel (enabled = 0). Both give bit-identical
+ * results. Process-wide; affects launches made after the call; returns the previous setting. */
+int fpd_set_conv1x1(int enabled);
 /* Forward ([tap][O][I]) and data-gradient ([taps-1-tap][I][O]) __half hi/lo forms of w * 2^8 from one read of the
  * weights: one launch per convolution and training step instead of two. */
 int fpd_weight_prep_f16_both(const float* w_oihw, void* f_hi, void* f_lo, void* d_hi, void* d_lo, int O, int I, int k,
