@@ -23,6 +23,8 @@
 //   pixel ranges. tf32 wgmma takes K-major operands only, so the transform threads write both operands transposed
 //   (channel rows of 32 pixels). Each CTA stores an fp32 partial; a second kernel reduces the partials in a fixed
 //   order (deterministic) into the OIHW gradient.
+//   Every 3x3 shape and the 1x1 shapes with Cout <= 64 run the same plan on wgrad_halo_kernel instead (input channels
+//   on M, x from registers, one staged pixel step for the three taps of a kernel row), bit-identical to it.
 #include <cuda_fp16.h>
 
 #include <atomic>
@@ -855,6 +857,8 @@ struct WgradParams {
   const float* pre_shift;
   int pre_relu;
   float* partial;   // [split][tap][Cout][Cin]
+  // wgrad_halo_kernel only
+  int h_ci, h_co_tiles, h_ci_tiles, h_rows, h_halo, h_win, h_xstride, h_stage_bytes;
 };
 
 template <int kN>
@@ -978,6 +982,211 @@ __global__ void __launch_bounds__(kThreads, 1) wgrad_wgmma_kernel(const WgradPar
   }
 }
 
+// ============================================ weight gradient, tap rows ============================================
+// wgrad_halo_kernel: the weight gradient of wgrad_wgmma_kernel with the roles of the operands swapped, so that M is
+// filled for every Cout, and with one staged pixel step serving every tap of a kernel row. Same plan (splits,
+// kt_per_split, K steps of 32 pixels, partial layout), and per output element the same chain: per K step the same
+// hi / lo values, per k8 dY_lo x_hi then dY_hi x_lo into `part_x` and dY_hi x_hi into `part` (the products are the
+// same numbers as wgrad_wgmma_kernel's, A and B only trade places), then acc += part + part_x.
+//   GEMM: M = (tap, input channel) rows, 64 per warpgroup, one tap and 16 channels per warp; N = a kN-wide slice of the
+//   output channels; one CTA = one split x one row of the 3x3 kernel (three taps; the 1x1 tap alone) x one input-channel
+//   tile of h_ci (<= 64) x one output slice. With h_ci = 32 two taps share a warpgroup; rows past the CTA's last tap
+//   (the fourth warpgroup half at h_ci = 32) compute a duplicate and are not written.
+//   Per K step (pixels p0 .. p0 + 31) the CTA stages, double-buffered:
+//     - dY as the B operand: kN K-major rows of 128 bytes under the 128-byte swizzle, hi and lo. Each thread loads 4
+//       pixels x 4 channels, transposes them in registers and writes one 16-byte chunk per channel row (8 consecutive
+//       threads write 8 chunks of one row: conflict-free).
+//     - x after the BN affine + ReLU, fp32, in its natural [pixel][channel] layout: the h_win = 32 + 2 h_halo
+//       flattened pixels p0 + dh W - h_halo .. of the kernel row dh, rows padded to h_xstride = h_ci + 8 floats so that
+//       the four k columns of a fragment load fall in distinct banks.
+//     - one word per pixel of the step: bit j set if tap j of the row reads a pixel inside the image (and p < P).
+//   Every lane then reads its A fragment for its tap from the shifted rows (zero where the mask bit is clear, the rule
+//   of wgrad_wgmma_kernel's loads), splits hi / lo in registers and issues the MMAs from registers.
+//   Stage s % 2 is rewritten at step s after the step s - 1 barrier, which follows every warpgroup's wgmma_wait<0> for
+//   step s - 2 (the last reader of that stage); the next step's global loads are in flight during the MMAs.
+constexpr int kWhMaxThreads = 384;
+constexpr int kWhXChunks = 4;   // staged x float4 chunks per thread and step, at most
+
+template <int kN, bool kSplit>
+__global__ void __launch_bounds__(kWhMaxThreads, 1) wgrad_halo_kernel(const WgradParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  const uint32_t smem_s = smem_u32(smem);
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, nthr = blockDim.x;
+  int bid = blockIdx.x;
+  const int ct = bid % p.h_co_tiles; bid /= p.h_co_tiles;
+  const int it = bid % p.h_ci_tiles; bid /= p.h_ci_tiles;
+  const int trow = bid % p.h_rows;
+  const int sp = bid / p.h_rows;
+  const int co0 = ct * kN, ci0 = it * p.h_ci;
+  const int row_taps = p.ksize == 3 ? 3 : 1;
+  const int dh = p.ksize == 3 ? trow - 1 : 0;
+  const int kt0 = sp * p.kt_per_split, kt1 = min(kt0 + p.kt_per_split, p.num_kt);
+  const uint32_t dy_lo_off = (uint32_t)kN * 128u;
+  const uint32_t x_off = 2u * dy_lo_off;
+  const uint32_t mask_off = x_off + (uint32_t)(p.h_win * p.h_xstride) * 4u;
+  const int HW = p.H * p.W;
+
+  // this warp's 16 rows: tap tl of the row, input channels cb .. cb + 15 of the tile
+  const int r0 = warp * 16;
+  int tl = r0 / p.h_ci;
+  const bool active = tl < row_taps;
+  if (!active) tl = row_taps - 1;
+  const int cb = r0 % p.h_ci;
+  const int tap = trow * row_taps + tl;
+  const int dw = p.ksize == 3 ? tl - 1 : 0;
+  const int g = lane >> 2, t = lane & 3;
+
+  // loads, one step ahead: dY item (pixel quad dq, channel quad dc) into registers for threads < 2 kN; the raw x window
+  // by cp.async straight into the stage; the tap mask
+  const int dq = tid & 7, dc = tid >> 3;
+  const bool dy_thread = tid < 2 * kN;
+  const int xq = p.h_ci / 4;                 // float4 chunks per staged pixel
+  const int x_items = p.h_win * xq;
+  const uint32_t dy_raw = mask_off + kKp * 4u + (uint32_t)((4 * dq * kN + 4 * dc) * 4);   // this thread's raw dY
+  uint32_t mbits = 0;
+  auto load = [&](int kt, uint32_t st) {
+    if (dy_thread) {
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        const int m = kt * kKp + 4 * dq + r;
+        cp_async16(st + dy_raw + (uint32_t)(r * kN * 4), p.dy + (size_t)(m < p.P ? m : 0) * p.Cout + co0 + 4 * dc,
+                   m < p.P);
+      }
+    }
+    const int qs = kt * kKp + dh * p.W - p.h_halo;
+#pragma unroll
+    for (int u = 0; u < kWhXChunks; ++u) {
+      const int idx = tid + u * nthr;
+      if (idx >= x_items) break;
+      const int j = idx / xq, c = (idx - j * xq) * 4;
+      const int q = qs + j;
+      const bool ok = q >= 0 && q < p.P;   // rows outside [0, P) are never read unmasked: zero-filled
+      cp_async16(st + x_off + (uint32_t)(j * p.h_xstride + c) * 4u, p.x + (size_t)(ok ? q : 0) * p.Cin + ci0 + c, ok);
+    }
+    cp_async_commit();
+    if (tid < kKp) {
+      const int m = kt * kKp + tid;
+      mbits = 0;
+      if (m < p.P) {
+        const int hh = (m % HW) / p.W + dh, w0 = m % p.W;
+        if (hh >= 0 && hh < p.H) {
+          for (int k = 0; k < row_taps; ++k) {
+            const int ww = w0 + (p.ksize == 3 ? k - 1 : 0);
+            if (ww >= 0 && ww < p.W) mbits |= 1u << k;
+          }
+        }
+      }
+    }
+  };
+  auto store = [&](uint32_t st) {   // after cp_async_wait_all: this thread's own raw dY copies have landed
+    if (dy_thread) {
+      float v[4][4];
+#pragma unroll
+      for (int r = 0; r < 4; ++r)
+        asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
+                     : "=f"(v[r][0]), "=f"(v[r][1]), "=f"(v[r][2]), "=f"(v[r][3])
+                     : "r"(st + dy_raw + (uint32_t)(r * kN * 4))
+                     : "memory");
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int row = 4 * dc + e;   // output channel co0 + row, pixels 4 dq .. 4 dq + 3
+        float4 h, l;
+        split_tf32x4(make_float4(v[0][e], v[1][e], v[2][e], v[3][e]), h, l);
+        const uint32_t a = st + (uint32_t)row * 128u + ((uint32_t)(dq ^ (row & 7)) << 4);
+        sts128u(a, make_uint4(__float_as_uint(h.x), __float_as_uint(h.y), __float_as_uint(h.z), __float_as_uint(h.w)));
+        if (kSplit)
+          sts128u(a + dy_lo_off,
+                  make_uint4(__float_as_uint(l.x), __float_as_uint(l.y), __float_as_uint(l.z), __float_as_uint(l.w)));
+      }
+    }
+    if (tid < kKp) asm volatile("st.shared.u32 [%0], %1;" ::"r"(st + mask_off + (uint32_t)tid * 4u), "r"(mbits) : "memory");
+  };
+
+  float acc[kN / 2], part[kN / 2], part_x[kN / 2];
+  zero_acc(acc);
+  zero_acc(part);
+  zero_acc(part_x);
+  if (kt0 < kt1) load(kt0, smem_s);
+  for (int kt = kt0; kt < kt1; ++kt) {
+    const uint32_t st = smem_s + (uint32_t)(((kt - kt0) & 1) * p.h_stage_bytes);
+    cp_async_wait_all();
+    store(st);   // overlaps the MMAs of step kt - 1
+    if (kt > kt0) {
+      wgmma_wait<0>();
+      add_part(acc, part, part_x);
+    }
+    fence_proxy_async_smem();
+    __syncthreads();
+    if (kt + 1 < kt1) load(kt + 1, smem_s + (uint32_t)(((kt + 1 - kt0) & 1) * p.h_stage_bytes));
+    // A fragments: k = 8 kk + t (+ 4), rows cb + g (+ 8); pixel k of the step reads staged row k + dw + h_halo
+    // the BN affine of this lane's two fragment channels, affine_relu4's expression applied per element
+    const int c_lane = ci0 + cb + g;
+    float mu[2] = {0.f, 0.f}, sc[2] = {1.f, 1.f}, sh[2] = {0.f, 0.f};
+    if (p.pre_scale) {
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        mu[hr] = p.pre_mean ? __ldg(p.pre_mean + c_lane + 8 * hr) : 0.f;
+        sc[hr] = __ldg(p.pre_scale + c_lane + 8 * hr);
+        sh[hr] = __ldg(p.pre_shift + c_lane + 8 * hr);
+      }
+    }
+    uint32_t ah[4][4], al[4][4];
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+      for (int hk = 0; hk < 2; ++hk) {
+        const int k = 8 * kk + t + 4 * hk;
+        uint32_t mk;
+        asm volatile("ld.shared.u32 %0, [%1];" : "=r"(mk) : "r"(st + mask_off + (uint32_t)k * 4u));
+        const bool ok = (mk >> tl) & 1u;
+        const uint32_t src = st + x_off + (uint32_t)((k + dw + p.h_halo) * p.h_xstride + cb + g) * 4u;
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          float v;
+          asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(src + (uint32_t)hr * 32u));
+          if (p.pre_scale) v = fmaf(v - mu[hr], sc[hr], sh[hr]);
+          if (p.pre_relu) v = fmaxf(v, 0.f);
+          if (!ok) v = 0.f;
+          float h, l;
+          split_tf32_fast(v, h, l);
+          // volatile moves keep the fragment writes ahead of wgmma_fence (no warpgroup.arrive between the MMAs)
+          asm volatile("mov.b32 %0, %1;" : "=r"(ah[kk][2 * hk + hr]) : "r"(__float_as_uint(h)));
+          asm volatile("mov.b32 %0, %1;" : "=r"(al[kk][2 * hk + hr]) : "r"(__float_as_uint(l)));
+        }
+      }
+    }
+    wgmma_fence();
+    const uint64_t dbh = gmma_desc_sw128(st), dbl = gmma_desc_sw128(st + dy_lo_off);
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      const uint64_t o = (uint64_t)(kk * 2);
+      const int accum = kk > 0 ? 1 : 0;
+      if (kSplit) {
+        WgmmaRATf32<kN>::mma(part_x, ah[kk], dbl + o, accum);   // dY_lo x_hi
+        WgmmaRATf32<kN>::mma(part_x, al[kk], dbh + o, 1);       // dY_hi x_lo
+      }
+      WgmmaRATf32<kN>::mma(part, ah[kk], dbh + o, accum);
+    }
+    wgmma_commit();
+  }
+  wgmma_wait<0>();
+  if (kt1 > kt0) add_part(acc, part, part_x);
+
+  if (!active) return;
+  float* out = p.partial + ((size_t)sp * p.taps + tap) * p.Cout * p.Cin;
+#pragma unroll
+  for (int rr = 0; rr < 2; ++rr) {
+    const int ci = ci0 + cb + g + rr * 8;
+#pragma unroll
+    for (int i = 0; i < kN / 8; ++i) {
+      const int co = co0 + i * 8 + 2 * t;
+      out[(size_t)co * p.Cin + ci] = acc[4 * i + 2 * rr];
+      out[(size_t)(co + 1) * p.Cin + ci] = acc[4 * i + 2 * rr + 1];
+    }
+  }
+}
+
 // dw[co][ci][tap] = scale * sum_splits partial[split][tap][co][ci]
 // Block = 32 consecutive partial elements (coalesced along ci) x 8 split groups: every thread sums splits sg, sg+8, ...
 // and the eight group sums are added in a fixed order (deterministic).
@@ -1034,6 +1243,53 @@ int wgrad_launch_n(const WgradParams& p, int grid, size_t smem, cudaStream_t str
   wgrad_wgmma_kernel<kN><<<grid, kThreads, smem, stream>>>(p);
   FPD_LAUNCH_CHECK();
   return FPD_OK;
+}
+
+std::atomic<int> g_wgrad_halo{1};
+
+// wgrad_halo_kernel takes every 3x3 shape of wgrad_tc_supported, and the 1x1 shapes whose input channels fill whole
+// 64-row warpgroups and whose Cout is 32 or 64, where wgrad_wgmma_kernel's 128-row tile is at most half used. (At
+// Cout >= 128 that tile is full, and the per-tap kernel was faster on the H100: 128 -> 128 at 64x64, batch 32, 128.5
+// against 151.9 µs.)
+bool wgrad_halo_ok(int Cin, int Cout, int ksize) {
+  if (!g_wgrad_halo.load(std::memory_order_relaxed)) return false;
+  if (ksize == 3) return true;
+  return Cin % 64 == 0 && (Cout == 32 || Cout == 64);
+}
+
+template <int kN, bool kSplit>
+int wgrad_halo_launch_n(const WgradParams& p, int grid, int threads, size_t smem, cudaStream_t stream) {
+  static std::atomic<uint64_t> done{0};
+  if (int rc = allow_smem(wgrad_halo_kernel<kN, kSplit>, done)) return rc;
+  wgrad_halo_kernel<kN, kSplit><<<grid, threads, smem, stream>>>(p);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+// The tap-row kernel for a plan of wgrad_plan (the splits are the plan's; only the CTA decomposition differs).
+int wgrad_halo_launch(WgradParams p, const WgradPlan& pl, cudaStream_t stream) {
+  const int n = p.Cout % 64 == 0 ? 64 : 32;
+  p.h_ci = p.Cin < 64 ? p.Cin : 64;
+  p.h_co_tiles = p.Cout / n;
+  p.h_ci_tiles = p.Cin / p.h_ci;
+  p.h_rows = p.ksize == 3 ? 3 : 1;
+  p.h_halo = p.ksize == 3 ? 1 : 0;
+  p.h_win = kKp + 2 * p.h_halo;
+  p.h_xstride = p.h_ci + 8;
+  const int row_taps = p.ksize == 3 ? 3 : 1;
+  const int threads = (row_taps * p.h_ci + 63) / 64 * 128;
+  // dY hi / lo tiles, the x window, the tap mask, raw dY
+  const size_t stage = 2 * (size_t)n * 128 + (size_t)p.h_win * p.h_xstride * 4 + kKp * 4 + (size_t)kKp * n * 4;
+  p.h_stage_bytes = (int)((stage + 1023) / 1024 * 1024);
+  FPD_REQUIRE(threads <= kWhMaxThreads && p.h_win * (p.h_ci / 4) <= kWhXChunks * threads,
+              "wgrad_halo: no plan for Cin=%d k=%d", p.Cin, p.ksize);
+  const size_t smem = 1024 + 2 * (size_t)p.h_stage_bytes;
+  const int grid = pl.splits * p.h_rows * p.h_ci_tiles * p.h_co_tiles;
+  if (p.passes == 3)
+    return n == 64 ? wgrad_halo_launch_n<64, true>(p, grid, threads, smem, stream)
+                   : wgrad_halo_launch_n<32, true>(p, grid, threads, smem, stream);
+  return n == 64 ? wgrad_halo_launch_n<64, false>(p, grid, threads, smem, stream)
+                 : wgrad_halo_launch_n<32, false>(p, grid, threads, smem, stream);
 }
 
 }  // namespace
@@ -1095,6 +1351,8 @@ bool wgrad_tc_supported(int Cin, int Cout, int ksize) {
   return ksize == 1 && Cout % 4 == 0 && Cin % 4 == 0 && Cin >= 4 && Cin <= 256;
 }
 
+int set_wgrad_halo(int enabled) { return g_wgrad_halo.exchange(enabled ? 1 : 0); }
+
 bool wgrad_tc3_supported(int H, int W, int Cin, int Cout, int ksize) {
   (void)H; (void)W;
   return ksize == 3 && wgrad_tc_supported(Cin, Cout, ksize);
@@ -1128,7 +1386,8 @@ int wgrad_tc_fused_launch(const float* x, const float* pre_mean, const float* pr
   p.partial = (float*)workspace;
   const size_t smem = 1024 + (size_t)kStages * p.stage_bytes;
   const int grid = pl.splits * pl.taps * pl.co_tiles * pl.ci_tiles;
-  int rc = pl.n == 32 ? wgrad_launch_n<32>(p, grid, smem, stream)
+  int rc = wgrad_halo_ok(Cin, Cout, ksize) ? wgrad_halo_launch(p, pl, stream)
+         : pl.n == 32 ? wgrad_launch_n<32>(p, grid, smem, stream)
          : pl.n == 64 ? wgrad_launch_n<64>(p, grid, smem, stream)
                       : wgrad_launch_n<128>(p, grid, smem, stream);
   if (rc) return rc;

@@ -39,6 +39,9 @@ int wgrad_tc_fused_launch(const float* x, const float* pre_mean, const float* pr
                           int pre_relu, const float* dy, int passes, float* dw_oihw, float scale, int B, int H, int W,
                           int Cin, int Cout, int ksize, void* workspace, size_t workspace_bytes, int num_sms,
                           cudaStream_t stream);
+// weight gradients on the tap-row kernel where it takes the shape (1, the default) or all on the per-tap kernel (0),
+// process-wide; returns the previous setting
+int set_wgrad_halo(int enabled);
 
 // the 3x3 shape rule of wgrad_tc_supported (fpd_conv2d_wgrad_tc3_supported)
 bool wgrad_tc3_supported(int H, int W, int Cin, int Cout, int ksize);

@@ -285,6 +285,22 @@ def conv2d_wgrad_tc_supported(cin, cout, k):
     return bool(N.lib().fpd_conv2d_wgrad_tc_supported(cin, cout, k))
 
 
+WGRAD_HALO = os.environ.get("FPD_WGRAD_HALO", "1") != "0"   # weight gradients on the tap-row kernel
+
+
+def set_wgrad_halo(enabled):
+    """Run weight gradients on the tap-row kernel where it takes the shape (True) or all on the per-tap kernel (False),
+    process-wide, for launches made after the call. The results are bit-identical. Returns the previous setting."""
+    global WGRAD_HALO
+    prev = bool(N.lib().fpd_set_wgrad_halo(int(bool(enabled))))
+    WGRAD_HALO = bool(enabled)
+    return prev
+
+
+if not WGRAD_HALO:
+    set_wgrad_halo(False)
+
+
 def conv2d_wgrad_tc_fused(x, dy, ksize, mean=None, scale=None, shift=None, relu=False, passes=3, out_scale=1.0,
                           out=None):
     """dW for y = conv(relu?((x-mean)*scale+shift)) given raw x and raw dy (operand transform inside the kernel)."""

@@ -123,6 +123,10 @@ int fpd_bn_stats_fused(const float* x, int64_t P, int C, const float* gamma, con
 /* Tensor-core weight gradient: dw_oihw[Cout,Cin,k,k] = scale * sum_pixels dy (x) a(tap-shifted). */
 int fpd_conv2d_wgrad_tc_supported(int Cin, int Cout, int ksize);
 size_t fpd_conv2d_wgrad_tc_workspace_bytes(int B, int H, int W, int Cin, int Cout, int ksize);
+/* Weight gradients run on the tap-row kernel (input channels on the MMA rows, one staged pixel step for all taps of a
+ * kernel row) where it takes the shape (enabled = 1, the default), or all on the per-tap kernel (enabled = 0). Both
+ * give bit-identical results. Process-wide; affects launches made after the call; returns the previous setting. */
+int fpd_set_wgrad_halo(int enabled);
 
 /* Weight gradient with the operand preparation fused in: x and dy are RAW fp32 NHWC tensors; the kernel applies
  * a = relu?((x - pre_mean) * pre_scale + pre_shift) (NULLs = identity), zeroes the 3x3 padding positions and does the

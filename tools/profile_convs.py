@@ -2,8 +2,9 @@
 teacher s8 f256, B=32).
 
 Every ops.conv2d_tc_h / ops.conv2d_tc_fused call (forward and data-gradient convolutions: conv_wgmma_kernel or
-conv_halo_kernel) and every ops.conv2d_wgrad_tc_fused call (wgrad_wgmma_kernel) is recorded on the host with its shape;
-the i-th kernel of each family in the CUPTI trace is matched to the i-th call, and time is aggregated per (kernel, shape).
+conv_halo_kernel) and every ops.conv2d_wgrad_tc_fused call (wgrad_halo_kernel or wgrad_wgmma_kernel) is recorded on
+the host with its shape; the i-th kernel of each family in the CUPTI trace is matched to the i-th call, and time is
+aggregated per (kernel, shape). Each weight gradient is followed by one wgrad_reduce_kernel, reported beside the family.
 The side streams (teacher overlap, hourglass branch fork, weight-gradient stream) are switched off so that each family
 runs on one stream in call order; the kernels and their shapes are the same as in the overlapped step.
 
@@ -19,7 +20,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-FAMILIES = {"conv": ("conv_wgmma_kernel", "conv_halo_kernel"), "wgrad": ("wgrad_wgmma_kernel",)}
+FAMILIES = {"conv": ("conv_wgmma_kernel", "conv_halo_kernel"), "wgrad": ("wgrad_halo_kernel", "wgrad_wgmma_kernel")}
 
 
 def kernel_label(name):
@@ -85,6 +86,11 @@ def main():
             by_kernel[s[0]] += v[1]
         for kname, us in sorted(by_kernel.items(), key=lambda kv: -kv[1]):
             out.append("  %-28s %8.2f ms" % (kname, us / 1000.0))
+        if fam == "wgrad":
+            red = [e for e in evs if "wgrad_reduce_kernel" in e.name]
+            red_us = sum(e.time_range.end - e.time_range.start for e in red)
+            out.append("  %-28s %8.2f ms (%d launches); wgrad family with the reduce: %.2f ms" % (
+                "wgrad_reduce_kernel", red_us / 1000.0, len(red), (tot + red_us) / 1000.0))
         for s, v in sorted(agg.items(), key=lambda kv: -kv[1][1])[:30]:
             kname, (B, Hh, Ww, Cin), Cout, k, prec, tag = s
             gf = 2.0 * B * Hh * Ww * Cin * Cout * k * k / 1e9
