@@ -62,6 +62,7 @@ int fpd_conv2d_tc_h(const float* x, const float* pre_mean, const float* pre_scal
 }
 
 int fpd_set_conv1x1(int enabled) { return set_conv1x1(enabled); }
+int fpd_set_conv_halo(int enabled) { return set_conv_halo(enabled); }
 int fpd_set_wgrad_halo(int enabled) { return set_wgrad_halo(enabled); }
 
 int fpd_conv2d_tc_h_stats_blocks(int B, int H, int W, int Cin, int Cout, int ksize, int f16) {

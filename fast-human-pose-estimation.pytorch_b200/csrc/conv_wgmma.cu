@@ -25,9 +25,11 @@
 //   order (deterministic) into the OIHW gradient.
 //   Every 3x3 shape and the 1x1 shapes with Cout <= 64 run the same plan on wgrad_halo_kernel instead (input channels
 //   on M, x from registers, one staged pixel step for the three taps of a kernel row), bit-identical to it.
+#include <cuda.h>
 #include <cuda_fp16.h>
 
 #include <atomic>
+#include <mutex>
 
 #include "common.cuh"
 #include "kernels.h"
@@ -161,6 +163,7 @@ struct ConvParams {
   double* stat_part;           // nullable [gridDim.x][Cout][2] = {sum (y - pivot), sum (y - pivot)^2}
   const float* stat_pivot;     // nullable [Cout]
   int halo_rows;               // conv_halo_kernel: kTileM + 2 W + 2 pixel rows + one zero row per channel block
+  int halo_stages;             // conv_halo_kernel: weight stages in the TMA ring (2 or 3)
 };
 
 // Weights of K step ks for output columns [n0, n0 + nt): nt K-major rows of 128 bytes (one tap, kCB input channels)
@@ -388,12 +391,31 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const ConvParam
 //   into the register-A fragment of wgmma; B comes from the swizzled weight stage as before. (Shifted shared-memory A
 //   descriptors cannot do this: at dw = +-1 the pixel past a row end is a real pixel of the next image row, not zero, and
 //   an odd row shift breaks the 128-byte swizzle phase.)
-//   Per k16: lo * hi, hi * lo, hi * hi into `part` (mma_row's order), `acc += part` once per step.
-//   Weights stream through two cp.async stages: stage (ks + 1) & 1 is refilled after the step-ks barrier, by which time
-//   every warpgroup has retired the step ks - 1 group that read it; the refill overlaps the MMAs of step ks. The A
-//   registers are rewritten only after wgmma_wait<0>.
-constexpr int kHaloStages = 2;
+//   Per k16: lo * hi, hi * lo, hi * hi into `part` (mma_row's order), `acc += part` once per step. The A registers are
+//   rewritten only after wgmma_wait<0>.
+//   Weights: a ring of S = halo_stages (2 or 3) stages, each {B hi, B lo} of one K step, filled by TMA from two 2-D tensor
+//   maps over the [tap][Cout][Cin] fp16 weights (rows of Cin, box 64 channels x nt rows, 128-byte swizzle: the layout
+//   mma_row's B descriptors read; channels >= Cin are zero-filled). The CTA's (tile, K step) sequence is one stream of
+//   steps s = 0, 1, ...; step s uses stage s % S, and its fill is phase s / S of full[s % S] (one arrive with expect_tx
+//   for the two boxes) and its release phase s / S of empty[s % S] (one arrive per warp, after that warp's
+//   wgmma_wait<0> has retired the step's MMAs: 8 arrivals). The ring runs across tiles, so the first S - 1 steps of the
+//   CTA's next tile load during the epilogue and the halo fill.
+//   Ping-pong: the warpgroups take turns to issue their MMAs of a step, warpgroup 0 first, through two named barriers
+//   (turn[wg] = kTurnBar + wg; a warpgroup syncs on its own turn, then arrives on the other's once its MMAs are issued;
+//   warpgroup 0 does not wait before the CTA's first step, warpgroup 1 does not hand over after the CTA's last). The
+//   tensor cores run each warpgroup's 12 MMAs of a step in issue order, so warpgroup 0's drain, accumulator adds and
+//   ldmatrix of the next step overlap warpgroup 1's MMAs and the other way round; without the turns both warpgroups
+//   stay in step (they start every tile together) and drain at the same time. A warpgroup can arrive on a turn barrier
+//   again only after the other has synced on it, so no turn phase is skipped.
+//   Producer: thread kTileM (warpgroup 1, the second to issue) fills step s + S - 1 into the stage of step s - 1 right
+//   after its warpgroup has issued the MMAs of step s. Its wait on empty[(s - 1) % S] never blocks: its own warpgroup
+//   released step s - 1 before issuing step s, and warpgroup 0 released it before issuing step s, which came before
+//   warpgroup 1's turn. So the producer never holds back a warpgroup's MMA issue, and waits on full never depend on a
+//   warpgroup the waiter is itself holding. Parity waits are unambiguous: a stage is refilled only after both
+//   warpgroups released its previous step, so no barrier runs two phases ahead of a waiter. Two CTA barriers per tile
+//   remain, around the halo fill that both warpgroups read.
 constexpr int kHaloBatch = 8;   // halo chunks per thread in flight (2 x float4 each)
+constexpr int kTurnBar = 1;     // named barriers kTurnBar + wg: warpgroup wg may issue its MMAs (0 is __syncthreads)
 
 __device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], uint32_t addr) {
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
@@ -401,20 +423,74 @@ __device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], uint32_t addr) {
                : "r"(addr)
                : "memory");
 }
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(int id, int count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
+  asm volatile(
+      "{\n.reg .pred p;\nWAIT:\n"
+      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
+      "@!p bra WAIT;\n}\n" ::"r"(bar),
+      "r"(parity)
+      : "memory");
+}
+__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint32_t bar) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
+          dst),
+      "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(bar)
+      : "memory");
+}
 
 template <int kN>
-__global__ void __launch_bounds__(kThreads, 1) conv_halo_kernel(const ConvParams p) {
+__global__ void __launch_bounds__(kThreads, 1)
+    conv_halo_kernel(const __grid_constant__ ConvParams p, const __grid_constant__ CUtensorMap w_hi_map,
+                     const __grid_constant__ CUtensorMap w_lo_map) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int R = p.halo_rows;
+  const uint32_t S = (uint32_t)p.halo_stages;
   const uint32_t lo_plane = (uint32_t)p.ncb * (uint32_t)R * 128u;
-  const uint32_t smem_b = smem_u32(smem);                                  // kHaloStages x {B hi, B lo}
-  const uint32_t halo = smem_b + (uint32_t)(kHaloStages * p.stage_bytes);   // hi plane, then lo plane
-  double* s_stat = reinterpret_cast<double*>(smem + (size_t)kHaloStages * p.stage_bytes + 2 * (size_t)lo_plane);
+  const uint32_t smem_b = smem_u32(smem);                          // S x {B hi, B lo}
+  const uint32_t halo = smem_b + S * (uint32_t)p.stage_bytes;      // hi plane, then lo plane
+  double* s_stat = reinterpret_cast<double*>(smem + (size_t)S * p.stage_bytes + 2 * (size_t)lo_plane);
+  const uint32_t full = smem_u32(s_stat) + (p.stat_part ? 16u * 8u * (uint32_t)p.Cout : 0u);   // S mbarriers
+  const uint32_t empty = full + 8u * S;                                                         // S mbarriers
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
   const float in_s = p.in_scale ? __ldg(p.in_scale) : 1.f;
   const float oscale = p.in_scale ? p.out_scale * __ldg(p.in_scale + 1) : p.out_scale;
   const uint32_t b_lo_off = (uint32_t)p.b_tile_bytes;
+  // fill of stream step s = (tile, ks): thread 0 for the first S - 1 steps (after the barrier init), then thread kTileM
+  auto load_b = [&](uint32_t s, int tile, int ks) {
+    const uint32_t st = s % S;
+    if (s >= S) mbar_wait(empty + 8u * st, (s / S - 1u) & 1u);
+    const uint32_t bar = full + 8u * st, dst = smem_b + st * (uint32_t)p.stage_bytes;
+    const int tap = ks / p.ncb, cb = ks - tap * p.ncb;
+    const int row = tap * p.Cout + (tile % p.n_tiles) * p.nt;
+    mbar_arrive_expect_tx(bar, 2u * (uint32_t)p.b_tile_bytes);
+    tma_load_2d(dst, &w_hi_map, cb * 64, row, bar);
+    tma_load_2d(dst + b_lo_off, &w_lo_map, cb * 64, row, bar);
+  };
+  if (tid == 0) {
+    for (uint32_t i = 0; i < S; ++i) {
+      mbar_init(full + 8u * i, 1);
+      mbar_init(empty + 8u * i, kThreads / 32);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    for (uint32_t s = 0; s + 1 < S; ++s) load_b(s, blockIdx.x, (int)s);   // ksteps >= 9 > S - 1
+  }
   conv_stats_init(p, s_stat);
   for (int i = tid; i < p.ncb * 8; i += kThreads) {   // the zero rows: never overwritten by the halo loads
     const uint32_t dst = halo + (uint32_t)((i >> 3) * R + R - 1) * 128u + ((uint32_t)(i & 7) << 4);
@@ -428,12 +504,12 @@ __global__ void __launch_bounds__(kThreads, 1) conv_halo_kernel(const ConvParams
   const int lr = wg * 64 + (warp & 3) * 16 + (lane & 7) + (lane & 8);
   const uint32_t khalf = (uint32_t)(lane >> 4);
   const int items = p.ncb * (R - 1) * 8;   // 16-byte chunks of one halo plane, zero rows excluded
+  uint32_t s = 0;                          // stream step
 
   for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
     const int m0 = (tile / p.n_tiles) * kTileM;
     const int n0 = (tile % p.n_tiles) * p.nt;
     const int hs = m0 - p.W - 1;   // pixel of halo row 0
-    conv_load_b<true>(p, 0, n0, smem_b, b_lo_off);
 
     // ---- halo: chunk idx = (row * ncb + cb) * 8 + jj covers channels cb * 64 + 8 jj .. + 7 of pixel hs + row, so
     // consecutive threads read consecutive 32-byte pieces of the NHWC span
@@ -476,23 +552,21 @@ __global__ void __launch_bounds__(kThreads, 1) conv_halo_kernel(const ConvParams
       }
     }
 
+    __syncthreads();   // the halo is visible
+
     const int m = m0 + lr;
     const int pn = m < p.P ? m / HW : p.B;   // pn == B marks a row past the last pixel
     const int ph = (m % HW) / p.W, pw = m % p.W;
     float acc[kN / 2], part[kN / 2];
     zero_acc(acc);
     zero_acc(part);
-    for (int ks = 0; ks < p.ksteps; ++ks) {
-      const uint32_t st = smem_b + (uint32_t)((ks & 1) * p.stage_bytes);
+    for (int ks = 0; ks < p.ksteps; ++ks, ++s) {
+      const uint32_t st = s % S;
       if (ks > 0) {
         wgmma_wait<0>();
         add_part(acc, part);
+        if (lane == 0) mbar_arrive(empty + 8u * ((s - 1u) % S));   // this warp is done with step s - 1
       }
-      cp_async_wait_all();
-      fence_proxy_async_smem();
-      __syncthreads();   // the weights of step ks (at ks = 0 also the halo) are visible; stage (ks + 1) & 1 is free
-      if (ks + 1 < p.ksteps)
-        conv_load_b<true>(p, ks + 1, n0, smem_b + (uint32_t)(((ks + 1) & 1) * p.stage_bytes), b_lo_off);
       const int tap = ks / p.ncb, cb = ks - tap * p.ncb;
       const int dh = tap / 3 - 1, dw = tap % 3 - 1;
       const int hh = ph + dh, ww = pw + dw;
@@ -507,8 +581,11 @@ __global__ void __launch_bounds__(kThreads, 1) conv_halo_kernel(const ConvParams
         ldsm_x4(ah[kk], a);
         ldsm_x4(al[kk], a + lo_plane);
       }
+      mbar_wait(full + 8u * st, (s / S) & 1u);   // the weights of step s have landed
+      if (wg == 1 || s > 0) named_bar_sync(kTurnBar + wg, kThreads);   // this warpgroup's turn to issue
       wgmma_fence();
-      const uint64_t dbh = gmma_desc_sw128(st), dbl = gmma_desc_sw128(st + b_lo_off);
+      const uint32_t b = smem_b + st * (uint32_t)p.stage_bytes;
+      const uint64_t dbh = gmma_desc_sw128(b), dbl = gmma_desc_sw128(b + b_lo_off);
 #pragma unroll
       for (int kk = 0; kk < 4; ++kk) {
         const uint64_t o = (uint64_t)(kk * 2);
@@ -517,10 +594,22 @@ __global__ void __launch_bounds__(kThreads, 1) conv_halo_kernel(const ConvParams
         WgmmaRA<kN>::f16(part, ah[kk], dbh + o, 1);
       }
       wgmma_commit();
+      if (wg == 0 || ks + 1 < p.ksteps || tile + (int)gridDim.x < p.num_tiles)
+        named_bar_arrive(kTurnBar + 1 - wg, kThreads);   // the other warpgroup's turn (none after the CTA's last step)
+      if (tid == kTileM) {   // fill step s + S - 1 into the stage of step s - 1
+        int lt = tile, lks = ks + (int)S - 1;
+        if (lks >= p.ksteps) {
+          lks -= p.ksteps;
+          lt += gridDim.x;
+        }
+        if (lt < p.num_tiles) load_b(s + S - 1u, lt, lks);
+      }
+      __syncwarp();
     }
     wgmma_wait<0>();
     add_part(acc, part);
-    __syncthreads();   // every warpgroup is done with the halo and both stages: the next tile may refill them
+    if (lane == 0) mbar_arrive(empty + 8u * ((s - 1u) % S));
+    __syncthreads();   // every warpgroup is done with the halo: the next tile may refill it
 
     conv_epilogue<kN>(p, acc, m0, n0, oscale, s_stat);
   }
@@ -731,25 +820,84 @@ int launch_n(const ConvParams& p, int grid, size_t smem, cudaStream_t stream) {
   return FPD_OK;
 }
 
+// The weights [taps][Cout][Cin] (fp16) as a 2-D tensor of taps * Cout rows of Cin channels, loaded in boxes of 64
+// channels x nt rows under the 128-byte swizzle; channels >= Cin read as zero. TMA needs a 16-byte row pitch, which
+// conv_shape_ok guarantees for fp16 (Cin % 8 == 0). cuTensorMapEncodeTiled is a driver API entry point; the library
+// links only the runtime, so it is looked up once through cudaGetDriverEntryPoint.
+using EncodeTiledFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+// A map depends only on (address, Cin, rows, nt), so the last kMapCache maps are kept and reused: a training step
+// launches the same weights many times, and reuse keeps driver calls out of the launch path.
+constexpr int kMapCache = 64;
+struct MapEntry {
+  const void* w;
+  int cin, rows, nt;
+  CUtensorMap map;
+};
+
+int halo_weight_map(CUtensorMap* map, const void* w, const ConvParams& p) {
+  static std::mutex mu;
+  static MapEntry cache[kMapCache];
+  static int cached = 0, next = 0;
+  const int rows = p.ksize * p.ksize * p.Cout;
+  std::lock_guard<std::mutex> lock(mu);
+  for (int i = 0; i < cached; ++i) {
+    const MapEntry& e = cache[i];
+    if (e.w == w && e.cin == p.Cin && e.rows == rows && e.nt == p.nt) {
+      *map = e.map;
+      return FPD_OK;
+    }
+  }
+  static std::atomic<EncodeTiledFn> encode{nullptr};
+  EncodeTiledFn fn = encode.load(std::memory_order_acquire);
+  if (!fn) {
+    void* f = nullptr;
+    cudaDriverEntryPointQueryResult q = cudaDriverEntryPointSymbolNotFound;
+    FPD_CUDA_CHECK(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q));
+    FPD_REQUIRE(q == cudaDriverEntryPointSuccess && f, "conv_halo: the driver has no cuTensorMapEncodeTiled");
+    fn = reinterpret_cast<EncodeTiledFn>(f);
+    encode.store(fn, std::memory_order_release);
+  }
+  const cuuint64_t dims[2] = {(cuuint64_t)p.Cin, (cuuint64_t)p.ksize * p.ksize * p.Cout};
+  const cuuint64_t pitch[1] = {(cuuint64_t)p.Cin * 2};
+  const cuuint32_t box[2] = {64, (cuuint32_t)p.nt};
+  const cuuint32_t elem_strides[2] = {1, 1};
+  const CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(w), dims, pitch, box, elem_strides,
+                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  FPD_REQUIRE(r == CUDA_SUCCESS, "conv_halo: cuTensorMapEncodeTiled failed (%d) for Cin=%d Cout=%d nt=%d", (int)r,
+              p.Cin, p.Cout, p.nt);
+  cache[next] = MapEntry{w, p.Cin, rows, p.nt, *map};
+  next = (next + 1) % kMapCache;
+  if (cached < kMapCache) ++cached;
+  return FPD_OK;
+}
+
 template <int kN>
-int launch_halo_n(const ConvParams& p, int grid, size_t smem, cudaStream_t stream) {
+int launch_halo_n(const ConvParams& p, const CUtensorMap& hi, const CUtensorMap& lo, int grid, size_t smem,
+                  cudaStream_t stream) {
   static std::atomic<uint64_t> done{0};
   if (int rc = allow_smem(conv_halo_kernel<kN>, done)) return rc;
-  conv_halo_kernel<kN><<<grid, kThreads, smem, stream>>>(p);
+  conv_halo_kernel<kN><<<grid, kThreads, smem, stream>>>(p, hi, lo);
   FPD_LAUNCH_CHECK();
   return FPD_OK;
 }
 
 int launch_halo(const ConvParams& p, int grid, size_t smem, cudaStream_t stream) {
+  CUtensorMap hi, lo;
+  if (int rc = halo_weight_map(&hi, p.w_hi, p)) return rc;
+  if (int rc = halo_weight_map(&lo, p.w_lo, p)) return rc;
   switch (p.nt) {
-    case 16: return launch_halo_n<16>(p, grid, smem, stream);
-    case 32: return launch_halo_n<32>(p, grid, smem, stream);
-    case 48: return launch_halo_n<48>(p, grid, smem, stream);
-    case 64: return launch_halo_n<64>(p, grid, smem, stream);
-    case 80: return launch_halo_n<80>(p, grid, smem, stream);
-    case 96: return launch_halo_n<96>(p, grid, smem, stream);
-    case 112: return launch_halo_n<112>(p, grid, smem, stream);
-    case 128: return launch_halo_n<128>(p, grid, smem, stream);
+    case 16: return launch_halo_n<16>(p, hi, lo, grid, smem, stream);
+    case 32: return launch_halo_n<32>(p, hi, lo, grid, smem, stream);
+    case 48: return launch_halo_n<48>(p, hi, lo, grid, smem, stream);
+    case 64: return launch_halo_n<64>(p, hi, lo, grid, smem, stream);
+    case 80: return launch_halo_n<80>(p, hi, lo, grid, smem, stream);
+    case 96: return launch_halo_n<96>(p, hi, lo, grid, smem, stream);
+    case 112: return launch_halo_n<112>(p, hi, lo, grid, smem, stream);
+    case 128: return launch_halo_n<128>(p, hi, lo, grid, smem, stream);
   }
   set_last_error("conv_halo: no kernel for a %d-column slice", p.nt);
   return FPD_ERR_UNSUPPORTED;
@@ -780,6 +928,7 @@ int launch_pw(const ConvParams& p, int grid, size_t smem, cudaStream_t stream) {
 }
 
 std::atomic<int> g_conv1x1{1};
+std::atomic<int> g_conv_halo{1};
 
 template <bool kF16>
 int launch_f(const ConvParams& p, int grid, size_t smem, cudaStream_t stream) {
@@ -824,13 +973,18 @@ int conv_launch(const float* x, const float* pre_mean, const float* pre_scale, c
   p.stat_part = stat_part; p.stat_pivot = stat_pivot;
   const size_t stat_bytes = stat_part ? (size_t)8 * Cout * 2 * sizeof(double) : 0;
   const int grid = p.num_tiles < num_sms ? p.num_tiles : num_sms;
-  if (f16 && p.passes == 3 && ksize == 3) {
-    // 3x3 3xFP16: the halo-resident kernel wherever the halo, two weight stages and the statistics scratch fit
+  if (f16 && p.passes == 3 && ksize == 3 && g_conv_halo.load(std::memory_order_relaxed)) {
+    // 3x3 3xFP16: the halo-resident kernel wherever the halo, the statistics scratch and a ring of three (else two)
+    // weight stages with their two mbarriers each fit
     ConvParams h = p;
     h.halo_rows = kTileM + 2 * W + 3;
     h.stage_bytes = 2 * p.b_tile_bytes;
-    const size_t smem = 1024 + (size_t)kHaloStages * h.stage_bytes + 2 * (size_t)h.ncb * h.halo_rows * 128 + stat_bytes;
-    if (smem <= (size_t)kSmemLimit) return launch_halo(h, grid, smem, stream);
+    for (int stages = 3; stages >= 2; --stages) {
+      h.halo_stages = stages;
+      const size_t smem = 1024 + (size_t)stages * h.stage_bytes + 2 * (size_t)h.ncb * h.halo_rows * 128 + stat_bytes +
+                          (size_t)stages * 2 * 8;
+      if (smem <= (size_t)kSmemLimit) return launch_halo(h, grid, smem, stream);
+    }
   }
   if (f16 && p.passes == 3 && ksize == 1 && stat_part == nullptr && g_conv1x1.load(std::memory_order_relaxed)) {
     // 1x1 3xFP16: the weight-resident kernel wherever the slice's weights and two A stages fit
@@ -1318,6 +1472,7 @@ int conv_tc_ts_launch(const float* x, const float* pre_mean, const float* pre_sc
 }
 
 int set_conv1x1(int enabled) { return g_conv1x1.exchange(enabled ? 1 : 0); }
+int set_conv_halo(int enabled) { return g_conv_halo.exchange(enabled ? 1 : 0); }
 
 bool conv_tc_h_supported(int Cin, int Cout, int ksize, int H, int W, int f16) {
   (void)H; (void)W;

@@ -30,6 +30,9 @@ int conv_tc_h_stats_grid(int B, int H, int W, int Cin, int Cout, int ksize, int 
 // 1x1 3xFP16 convolutions without statistics: the weight-resident kernel (1, the default) or the staged kernel (0),
 // process-wide; returns the previous setting
 int set_conv1x1(int enabled);
+// 3x3 3xFP16 convolutions: the halo kernel where it fits (1, the default) or the staged kernel (0), process-wide;
+// returns the previous setting
+int set_conv_halo(int enabled);
 
 // ---- conv_wgmma.cu : warpgroup-MMA weight-gradient GEMM (K = pixels) reading RAW x and dY; BN-apply + ReLU + tf32 split
 //      fused into the operand staging ----

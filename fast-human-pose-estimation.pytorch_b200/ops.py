@@ -173,6 +173,13 @@ if not CONV1X1:
     set_conv1x1(False)
 
 
+def set_conv_halo(enabled):
+    """Run 3x3 3xFP16 convolutions on the halo-resident kernel where it fits (True, the default) or on the staged
+    kernel (False), process-wide, for launches made after the call; for comparing the two, whose results are
+    bit-identical. Returns the previous setting."""
+    return bool(N.lib().fpd_set_conv_halo(int(bool(enabled))))
+
+
 def conv2d_tc_h_supported(cin, cout, k, H, W, f16):
     return CONV_H and bool(N.lib().fpd_conv2d_tc_h_supported(cin, cout, k, H, W, int(f16)))
 

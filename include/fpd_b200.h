@@ -78,6 +78,10 @@ int fpd_conv2d_tc_h(const float* x, const float* pre_mean, const float* pre_scal
  * shared memory, where they fit (enabled = 1, the default), or on the staged kernel (enabled = 0). Both give bit-identical
  * results. Process-wide; affects launches made after the call; returns the previous setting. */
 int fpd_set_conv1x1(int enabled);
+/* 3x3 convolutions with 3xFP16 operands run on the halo-resident kernel where it fits (enabled = 1, the default), or on
+ * the staged kernel (enabled = 0), for bit-identity checks between the two. Process-wide; affects launches made after
+ * the call; returns the previous setting. */
+int fpd_set_conv_halo(int enabled);
 /* Forward ([tap][O][I]) and data-gradient ([taps-1-tap][I][O]) __half hi/lo forms of w * 2^8 from one read of the
  * weights: one launch per convolution and training step instead of two. */
 int fpd_weight_prep_f16_both(const float* w_oihw, void* f_hi, void* f_lo, void* d_hi, void* d_lo, int O, int I, int k,
