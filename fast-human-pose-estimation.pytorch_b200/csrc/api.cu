@@ -61,6 +61,18 @@ int fpd_conv2d_tc_h(const float* x, const float* pre_mean, const float* pre_scal
                           out_scale, in_scale, B, H, W, Cin, Cout, ksize, device_sm_count(), S(stream));
 }
 
+int fpd_conv2d_tc_f16x1_kernel(int B, int H, int W, int Cin, int Cout, int ksize) {
+  return conv_f16x1_kernel(B, H, W, Cin, Cout, ksize);
+}
+
+int fpd_conv2d_tc_f16x1(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
+                        int pre_relu, const void* w, const float* bias, const float* residual, const float* relu_mask,
+                        float* y, float out_scale, int B, int H, int W, int Cin, int Cout, int ksize,
+                        fpd_stream_t stream) {
+  return conv_f16x1_launch(x, pre_mean, pre_scale, pre_shift, pre_relu, w, bias, residual, relu_mask, y, out_scale, B,
+                           H, W, Cin, Cout, ksize, device_sm_count(), S(stream));
+}
+
 int fpd_set_conv1x1(int enabled) { return set_conv1x1(enabled); }
 int fpd_set_conv_halo(int enabled) { return set_conv_halo(enabled); }
 int fpd_set_wgrad_halo(int enabled) { return set_wgrad_halo(enabled); }

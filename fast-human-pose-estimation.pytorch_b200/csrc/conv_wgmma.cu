@@ -16,6 +16,8 @@
 //   accumulators merged in a fixed order (deterministic), one [Cout][2] block per CTA for bn_finalize_sums.
 //   3x3 with 3xFP16 operands (conv_halo_kernel, selected by conv_launch where it fits in shared memory): the same GEMM
 //   with the A operand of a tile loaded and transformed once into a halo in shared memory and fed from registers.
+//   Single-pass FP16 for inference (conv_f16x1_launch): the halo and 1x1 weight-resident kernels with kSplit = false
+//   (conv_halo_f16x1_kernel, pw_conv_f16x1_kernel), one MMA per k16 straight into the accumulators.
 //
 // Weight gradient (wgrad_tc_*):
 //   dW[co][ci][tap] = scale * sum_{pixels p} dY[p][co] * A[p (+) tap][ci],  A = relu?((x - mean) * scale + shift)
@@ -30,6 +32,7 @@
 
 #include <atomic>
 #include <mutex>
+#include <type_traits>
 
 #include "common.cuh"
 #include "kernels.h"
@@ -104,15 +107,16 @@ __device__ __forceinline__ void zero_acc(float (&acc)[N]) {
 // The caller adds `part` into its fp32 accumulators with ordinary (round-to-nearest) additions once the group has
 // retired: the tensor core's own accumulation truncates, and over a K of thousands (3x3 convolutions over 512
 // channels, weight gradients over ~1000 pixels per split) that drifts to many times the error of an fp32 sum.
+// acc0 = 1 makes the first MMA accumulate too (the single-pass kernels accumulate straight into `acc`).
 template <bool kF16, int kN, bool kSepCross>
 __device__ __forceinline__ void mma_row(float (&part)[kN / 2], float (&part_x)[kN / 2], uint32_t a_hi, uint32_t a_lo,
-                                        uint32_t b_hi, uint32_t b_lo, bool split) {
+                                        uint32_t b_hi, uint32_t b_lo, bool split, int acc0 = 0) {
   const uint64_t dah = gmma_desc_sw128(a_hi), dal = gmma_desc_sw128(a_lo);
   const uint64_t dbh = gmma_desc_sw128(b_hi), dbl = gmma_desc_sw128(b_lo);
 #pragma unroll
   for (int kk = 0; kk < 4; ++kk) {
     const uint64_t o = (uint64_t)(kk * 2);
-    const int acc = kk > 0 ? 1 : 0;
+    const int acc = kk > 0 ? 1 : acc0;
     if (split) {
       if (kF16) {
         Wgmma<kN>::f16(part_x, dal + o, dbh + o, acc);
@@ -454,34 +458,41 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       : "memory");
 }
 
-template <int kN>
-__global__ void __launch_bounds__(kThreads, 1)
-    conv_halo_kernel(const __grid_constant__ ConvParams p, const __grid_constant__ CUtensorMap w_hi_map,
-                     const __grid_constant__ CUtensorMap w_lo_map) {
+// conv_halo_f16x1_kernel: the single-pass form (kSplit = false) of the same body. Activation operand fp16_rn(x), the
+// hi plane alone (half the halo, half the ldmatrix), weights the one box of w * 2^8 per stage. One register-A MMA per k16
+// straight into `acc` for the whole K loop: with fp16-rounded operands (relative 2^-11) the tensor core's accumulation
+// drift no longer matters, so no per-step fragment. The A fragments are double-buffered (step parity) and every step
+// ends with wgmma_wait<1>, so step s + 1 issues while step s is still in the tensor core; that wait retires step s - 1,
+// whose stage the warp releases then. The producer therefore fills step s + S - 2 into the stage of step s - 2 (both
+// warpgroups released it during step s - 1, before warpgroup 0's turn for step s), and the ring has S >= 3 stages.
+template <int kN, bool kSplit>
+__device__ __forceinline__ void conv_halo_body(const ConvParams& p, const CUtensorMap& w_hi_map,
+                                               const CUtensorMap& w_lo_map) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int R = p.halo_rows;
   const uint32_t S = (uint32_t)p.halo_stages;
+  const uint32_t ahead = kSplit ? S - 1u : S - 2u;                 // steps in the ring ahead of the one being issued
   const uint32_t lo_plane = (uint32_t)p.ncb * (uint32_t)R * 128u;
   const uint32_t smem_b = smem_u32(smem);                          // S x {B hi, B lo}
   const uint32_t halo = smem_b + S * (uint32_t)p.stage_bytes;      // hi plane, then lo plane
-  double* s_stat = reinterpret_cast<double*>(smem + (size_t)S * p.stage_bytes + 2 * (size_t)lo_plane);
+  double* s_stat = reinterpret_cast<double*>(smem + (size_t)S * p.stage_bytes + (kSplit ? 2 : 1) * (size_t)lo_plane);
   const uint32_t full = smem_u32(s_stat) + (p.stat_part ? 16u * 8u * (uint32_t)p.Cout : 0u);   // S mbarriers
   const uint32_t empty = full + 8u * S;                                                         // S mbarriers
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
   const float in_s = p.in_scale ? __ldg(p.in_scale) : 1.f;
   const float oscale = p.in_scale ? p.out_scale * __ldg(p.in_scale + 1) : p.out_scale;
   const uint32_t b_lo_off = (uint32_t)p.b_tile_bytes;
-  // fill of stream step s = (tile, ks): thread 0 for the first S - 1 steps (after the barrier init), then thread kTileM
+  // fill of stream step s = (tile, ks): thread 0 for the first `ahead` steps (after the barrier init), then thread kTileM
   auto load_b = [&](uint32_t s, int tile, int ks) {
     const uint32_t st = s % S;
     if (s >= S) mbar_wait(empty + 8u * st, (s / S - 1u) & 1u);
     const uint32_t bar = full + 8u * st, dst = smem_b + st * (uint32_t)p.stage_bytes;
     const int tap = ks / p.ncb, cb = ks - tap * p.ncb;
     const int row = tap * p.Cout + (tile % p.n_tiles) * p.nt;
-    mbar_arrive_expect_tx(bar, 2u * (uint32_t)p.b_tile_bytes);
+    mbar_arrive_expect_tx(bar, (kSplit ? 2u : 1u) * (uint32_t)p.b_tile_bytes);
     tma_load_2d(dst, &w_hi_map, cb * 64, row, bar);
-    tma_load_2d(dst + b_lo_off, &w_lo_map, cb * 64, row, bar);
+    if (kSplit) tma_load_2d(dst + b_lo_off, &w_lo_map, cb * 64, row, bar);
   };
   if (tid == 0) {
     for (uint32_t i = 0; i < S; ++i) {
@@ -489,13 +500,13 @@ __global__ void __launch_bounds__(kThreads, 1)
       mbar_init(empty + 8u * i, kThreads / 32);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    for (uint32_t s = 0; s + 1 < S; ++s) load_b(s, blockIdx.x, (int)s);   // ksteps >= 9 > S - 1
+    for (uint32_t s = 0; s < ahead; ++s) load_b(s, blockIdx.x, (int)s);   // ksteps >= 9 > ahead
   }
   conv_stats_init(p, s_stat);
   for (int i = tid; i < p.ncb * 8; i += kThreads) {   // the zero rows: never overwritten by the halo loads
     const uint32_t dst = halo + (uint32_t)((i >> 3) * R + R - 1) * 128u + ((uint32_t)(i & 7) << 4);
     sts128u(dst, make_uint4(0u, 0u, 0u, 0u));
-    sts128u(dst + lo_plane, make_uint4(0u, 0u, 0u, 0u));
+    if (kSplit) sts128u(dst + lo_plane, make_uint4(0u, 0u, 0u, 0u));
   }
 
   const int HW = p.H * p.W;
@@ -548,7 +559,7 @@ __global__ void __launch_bounds__(kThreads, 1)
         }
         const uint32_t dst = halo + (uint32_t)(cb * R + r) * 128u + ((uint32_t)(jj ^ (r & 7)) << 4);
         sts128u(dst, oh);
-        sts128u(dst + lo_plane, ol);
+        if (kSplit) sts128u(dst + lo_plane, ol);
       }
     }
 
@@ -557,8 +568,58 @@ __global__ void __launch_bounds__(kThreads, 1)
     const int m = m0 + lr;
     const int pn = m < p.P ? m / HW : p.B;   // pn == B marks a row past the last pixel
     const int ph = (m % HW) / p.W, pw = m % p.W;
-    float acc[kN / 2], part[kN / 2];
+    float acc[kN / 2];
     zero_acc(acc);
+    if constexpr (!kSplit) {
+      uint32_t ah[2][4][4];   // A fragments of steps of even / odd parity
+      // step s = (tile, ks) of the stream; `buf` (a compile-time step parity) selects its A fragments
+      auto step = [&](int ks, auto buf) {
+        constexpr int kb = decltype(buf)::value;
+        const uint32_t st = s % S;
+        const int tap = ks / p.ncb, cb = ks - tap * p.ncb;
+        const int dh = tap / 3 - 1, dw = tap % 3 - 1;
+        const int hh = ph + dh, ww = pw + dw;
+        const bool ok = pn < p.B && hh >= 0 && hh < p.H && ww >= 0 && ww < p.W;
+        const int hr = ok ? lr + (dh + 1) * p.W + dw + 1 : R - 1;
+        const uint32_t row = halo + (uint32_t)(cb * R + hr) * 128u;
+        const uint32_t sw = (uint32_t)(hr & 7);
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) ldsm_x4(ah[kb][kk], row + (((2u * kk + khalf) ^ sw) << 4));
+        mbar_wait(full + 8u * st, (s / S) & 1u);   // the weights of step s have landed
+        if (wg == 1 || s > 0) named_bar_sync(kTurnBar + wg, kThreads);   // this warpgroup's turn to issue
+        wgmma_fence();
+        const uint64_t db = gmma_desc_sw128(smem_b + st * (uint32_t)p.stage_bytes);
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) WgmmaRA<kN>::f16(acc, ah[kb][kk], db + (uint64_t)(kk * 2), 1);
+        wgmma_commit();
+        if (wg == 0 || ks + 1 < p.ksteps || tile + (int)gridDim.x < p.num_tiles)
+          named_bar_arrive(kTurnBar + 1 - wg, kThreads);   // the other warpgroup's turn (none after the CTA's last step)
+        wgmma_wait<1>();   // step s - 1 has retired: its A fragments and its weight stage are free
+        if (ks > 0 && lane == 0) mbar_arrive(empty + 8u * ((s - 1u) % S));
+        if (tid == kTileM) {   // fill step s + S - 2 into the stage of step s - 2
+          int lt = tile, lks = ks + (int)ahead;
+          if (lks >= p.ksteps) {
+            lks -= p.ksteps;
+            lt += gridDim.x;
+          }
+          if (lt < p.num_tiles) load_b(s + ahead, lt, lks);
+        }
+        __syncwarp();
+        ++s;
+      };
+      int ks = 0;
+      for (; ks + 1 < p.ksteps; ks += 2) {
+        step(ks, std::integral_constant<int, 0>());
+        step(ks + 1, std::integral_constant<int, 1>());
+      }
+      if (ks < p.ksteps) step(ks, std::integral_constant<int, 0>());
+      wgmma_wait<0>();
+      if (lane == 0) mbar_arrive(empty + 8u * ((s - 1u) % S));
+      __syncthreads();   // every warpgroup is done with the halo: the next tile may refill it
+      conv_epilogue<kN>(p, acc, m0, n0, oscale, s_stat);
+      continue;
+    }
+    float part[kN / 2];
     zero_acc(part);
     for (int ks = 0; ks < p.ksteps; ++ks, ++s) {
       const uint32_t st = s % S;
@@ -614,6 +675,19 @@ __global__ void __launch_bounds__(kThreads, 1)
     conv_epilogue<kN>(p, acc, m0, n0, oscale, s_stat);
   }
   conv_stats_flush(p, s_stat);
+}
+
+template <int kN>
+__global__ void __launch_bounds__(kThreads, 1)
+    conv_halo_kernel(const __grid_constant__ ConvParams p, const __grid_constant__ CUtensorMap w_hi_map,
+                     const __grid_constant__ CUtensorMap w_lo_map) {
+  conv_halo_body<kN, true>(p, w_hi_map, w_lo_map);
+}
+
+template <int kN>
+__global__ void __launch_bounds__(kThreads, 1)
+    conv_halo_f16x1_kernel(const __grid_constant__ ConvParams p, const __grid_constant__ CUtensorMap w_map) {
+  conv_halo_body<kN, false>(p, w_map, w_map);
 }
 
 // ============================================ forward, 1x1 resident weights ============================================
@@ -684,14 +758,27 @@ __device__ __forceinline__ void pw_epilogue(const ConvParams& p, const float (&a
   }
 }
 
-template <int kN>
-__global__ void __launch_bounds__(kThreads, 1) pw_conv_wgmma_kernel(const ConvParams p) {
-  constexpr uint32_t kAStage = 2u * kATileBytes;   // A hi, then A lo
+// pw_conv_f16x1_kernel: the single-pass form (kSplit = false): hi-only A stages and weights (16 KB per stage, so the
+// slice fits up to Cin = 640 at 128 columns), one MMA per k16 straight into `acc`. Three A stages and wgmma_wait<1>
+// before each step's barrier keep one step's MMAs in flight across it: stage s % 3 is rewritten by step s after the
+// barrier of step s - 1, which follows every warpgroup's retirement of step s - 3.
+constexpr int kPwStages1 = 3;
+
+template <bool kSplit>
+size_t pw_smem_bytes(int ncb, int nt) {
+  return 1024 + (size_t)(kSplit ? kPwStages : kPwStages1) * (kSplit ? 2 : 1) * kATileBytes +
+         (size_t)ncb * (kSplit ? 2 : 1) * nt * 128;
+}
+
+template <int kN, bool kSplit>
+__device__ __forceinline__ void pw_conv_body(const ConvParams& p) {
+  constexpr uint32_t kAStage = (kSplit ? 2u : 1u) * kATileBytes;   // A hi, then A lo
+  constexpr uint32_t kNumStages = kSplit ? kPwStages : kPwStages1;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const uint32_t smem_a = smem_u32(smem);                        // kPwStages x {A hi, A lo}
-  const uint32_t smem_w = smem_a + kPwStages * kAStage;          // ncb x {B hi, B lo}
-  const uint32_t w_step = 2u * (uint32_t)p.b_tile_bytes;
+  const uint32_t smem_a = smem_u32(smem);                        // kNumStages x {A hi, A lo}
+  const uint32_t smem_w = smem_a + kNumStages * kAStage;         // ncb x {B hi, B lo}
+  const uint32_t w_step = (kSplit ? 2u : 1u) * (uint32_t)p.b_tile_bytes;
   const int tid = threadIdx.x, wg = tid >> 7;
   const float in_s = p.in_scale ? __ldg(p.in_scale) : 1.f;
   const float oscale = p.in_scale ? p.out_scale * __ldg(p.in_scale + 1) : p.out_scale;
@@ -735,7 +822,7 @@ __global__ void __launch_bounds__(kThreads, 1) pw_conv_wgmma_kernel(const ConvPa
         split_f16x2(v[1].z, v[1].w, oh.w, ol.w);
       }
       sts128u(dst, oh);
-      sts128u(dst + (uint32_t)kATileBytes, ol);
+      if (kSplit) sts128u(dst + (uint32_t)kATileBytes, ol);
     }
   };
 
@@ -760,9 +847,11 @@ __global__ void __launch_bounds__(kThreads, 1) pw_conv_wgmma_kernel(const ConvPa
     zero_acc(acc);
     zero_acc(part);
     for (int ks = 0; ks < p.ncb; ++ks, ++s) {
-      const uint32_t st = smem_a + (s % kPwStages) * kAStage;
+      const uint32_t st = smem_a + (s % kNumStages) * kAStage;
       store_a(ks, st);   // overlaps the MMAs of step ks - 1
-      if (ks > 0) {
+      if (!kSplit) {
+        wgmma_wait<1>();   // step ks - 2 has retired
+      } else if (ks > 0) {
         wgmma_wait<0>();
         add_part(acc, part);
       }
@@ -774,17 +863,24 @@ __global__ void __launch_bounds__(kThreads, 1) pw_conv_wgmma_kernel(const ConvPa
       wgmma_fence();
       const uint32_t a_hi = st + (uint32_t)wg * 64u * 128u;
       const uint32_t b = smem_w + (uint32_t)ks * w_step;
-      mma_row<true, kN, false>(part, part, a_hi, a_hi + kATileBytes, b, b + p.b_tile_bytes, true);
+      if (kSplit) mma_row<true, kN, false>(part, part, a_hi, a_hi + kATileBytes, b, b + p.b_tile_bytes, true);
+      else mma_row<true, kN, false>(acc, acc, a_hi, a_hi, b, b, false, 1);
       wgmma_commit();
     }
     wgmma_wait<0>();
-    add_part(acc, part);
+    if (kSplit) add_part(acc, part);
     pw_epilogue<kN>(p, acc, m0, n0, oscale);
   }
 }
 
-size_t pw_smem_bytes(int ncb, int nt) {
-  return 1024 + (size_t)kPwStages * 2 * kATileBytes + (size_t)ncb * 2 * nt * 128;
+template <int kN>
+__global__ void __launch_bounds__(kThreads, 1) pw_conv_wgmma_kernel(const __grid_constant__ ConvParams p) {
+  pw_conv_body<kN, true>(p);
+}
+
+template <int kN>
+__global__ void __launch_bounds__(kThreads, 1) pw_conv_f16x1_kernel(const __grid_constant__ ConvParams p) {
+  pw_conv_body<kN, false>(p);
 }
 
 bool conv_shape_ok(int Cin, int Cout, int ksize, int f16, int max_cin, int max_cout) {
@@ -875,53 +971,69 @@ int halo_weight_map(CUtensorMap* map, const void* w, const ConvParams& p) {
   return FPD_OK;
 }
 
-template <int kN>
+template <int kN, bool kSplit>
 int launch_halo_n(const ConvParams& p, const CUtensorMap& hi, const CUtensorMap& lo, int grid, size_t smem,
                   cudaStream_t stream) {
   static std::atomic<uint64_t> done{0};
-  if (int rc = allow_smem(conv_halo_kernel<kN>, done)) return rc;
-  conv_halo_kernel<kN><<<grid, kThreads, smem, stream>>>(p, hi, lo);
+  if constexpr (kSplit) {
+    if (int rc = allow_smem(conv_halo_kernel<kN>, done)) return rc;
+    conv_halo_kernel<kN><<<grid, kThreads, smem, stream>>>(p, hi, lo);
+  } else {
+    if (int rc = allow_smem(conv_halo_f16x1_kernel<kN>, done)) return rc;
+    conv_halo_f16x1_kernel<kN><<<grid, kThreads, smem, stream>>>(p, hi);
+  }
   FPD_LAUNCH_CHECK();
   return FPD_OK;
 }
 
+template <bool kSplit>
 int launch_halo(const ConvParams& p, int grid, size_t smem, cudaStream_t stream) {
   CUtensorMap hi, lo;
   if (int rc = halo_weight_map(&hi, p.w_hi, p)) return rc;
-  if (int rc = halo_weight_map(&lo, p.w_lo, p)) return rc;
+  if (kSplit) {
+    if (int rc = halo_weight_map(&lo, p.w_lo, p)) return rc;
+  } else {
+    lo = hi;
+  }
   switch (p.nt) {
-    case 16: return launch_halo_n<16>(p, hi, lo, grid, smem, stream);
-    case 32: return launch_halo_n<32>(p, hi, lo, grid, smem, stream);
-    case 48: return launch_halo_n<48>(p, hi, lo, grid, smem, stream);
-    case 64: return launch_halo_n<64>(p, hi, lo, grid, smem, stream);
-    case 80: return launch_halo_n<80>(p, hi, lo, grid, smem, stream);
-    case 96: return launch_halo_n<96>(p, hi, lo, grid, smem, stream);
-    case 112: return launch_halo_n<112>(p, hi, lo, grid, smem, stream);
-    case 128: return launch_halo_n<128>(p, hi, lo, grid, smem, stream);
+    case 16: return launch_halo_n<16, kSplit>(p, hi, lo, grid, smem, stream);
+    case 32: return launch_halo_n<32, kSplit>(p, hi, lo, grid, smem, stream);
+    case 48: return launch_halo_n<48, kSplit>(p, hi, lo, grid, smem, stream);
+    case 64: return launch_halo_n<64, kSplit>(p, hi, lo, grid, smem, stream);
+    case 80: return launch_halo_n<80, kSplit>(p, hi, lo, grid, smem, stream);
+    case 96: return launch_halo_n<96, kSplit>(p, hi, lo, grid, smem, stream);
+    case 112: return launch_halo_n<112, kSplit>(p, hi, lo, grid, smem, stream);
+    case 128: return launch_halo_n<128, kSplit>(p, hi, lo, grid, smem, stream);
   }
   set_last_error("conv_halo: no kernel for a %d-column slice", p.nt);
   return FPD_ERR_UNSUPPORTED;
 }
 
-template <int kN>
+template <int kN, bool kSplit>
 int launch_pw_n(const ConvParams& p, int grid, size_t smem, cudaStream_t stream) {
   static std::atomic<uint64_t> done{0};
-  if (int rc = allow_smem(pw_conv_wgmma_kernel<kN>, done)) return rc;
-  pw_conv_wgmma_kernel<kN><<<grid, kThreads, smem, stream>>>(p);
+  if constexpr (kSplit) {
+    if (int rc = allow_smem(pw_conv_wgmma_kernel<kN>, done)) return rc;
+    pw_conv_wgmma_kernel<kN><<<grid, kThreads, smem, stream>>>(p);
+  } else {
+    if (int rc = allow_smem(pw_conv_f16x1_kernel<kN>, done)) return rc;
+    pw_conv_f16x1_kernel<kN><<<grid, kThreads, smem, stream>>>(p);
+  }
   FPD_LAUNCH_CHECK();
   return FPD_OK;
 }
 
+template <bool kSplit>
 int launch_pw(const ConvParams& p, int grid, size_t smem, cudaStream_t stream) {
   switch (p.nt) {
-    case 16: return launch_pw_n<16>(p, grid, smem, stream);
-    case 32: return launch_pw_n<32>(p, grid, smem, stream);
-    case 48: return launch_pw_n<48>(p, grid, smem, stream);
-    case 64: return launch_pw_n<64>(p, grid, smem, stream);
-    case 80: return launch_pw_n<80>(p, grid, smem, stream);
-    case 96: return launch_pw_n<96>(p, grid, smem, stream);
-    case 112: return launch_pw_n<112>(p, grid, smem, stream);
-    case 128: return launch_pw_n<128>(p, grid, smem, stream);
+    case 16: return launch_pw_n<16, kSplit>(p, grid, smem, stream);
+    case 32: return launch_pw_n<32, kSplit>(p, grid, smem, stream);
+    case 48: return launch_pw_n<48, kSplit>(p, grid, smem, stream);
+    case 64: return launch_pw_n<64, kSplit>(p, grid, smem, stream);
+    case 80: return launch_pw_n<80, kSplit>(p, grid, smem, stream);
+    case 96: return launch_pw_n<96, kSplit>(p, grid, smem, stream);
+    case 112: return launch_pw_n<112, kSplit>(p, grid, smem, stream);
+    case 128: return launch_pw_n<128, kSplit>(p, grid, smem, stream);
   }
   set_last_error("conv_pw: no kernel for a %d-column slice", p.nt);
   return FPD_ERR_UNSUPPORTED;
@@ -946,6 +1058,21 @@ int launch_f(const ConvParams& p, int grid, size_t smem, cudaStream_t stream) {
   return FPD_ERR_UNSUPPORTED;
 }
 
+// The shape part of a launch's parameters, staged-kernel layout (passes 3: hi and lo tiles per stage).
+ConvParams conv_shape_params(int B, int H, int W, int Cin, int Cout, int ksize, int f16, int passes) {
+  ConvParams p{};
+  p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.Cout = Cout; p.ksize = ksize; p.P = B * H * W;
+  p.passes = passes;
+  p.nt = conv_tc_ts_slice(Cout);
+  p.n_tiles = Cout / p.nt;
+  p.num_tiles = conv_num_tiles(B, H, W, Cout);
+  p.ncb = (Cin + (f16 ? 63 : 31)) / (f16 ? 64 : 32);
+  p.ksteps = ksize * ksize * p.ncb;
+  p.b_tile_bytes = p.nt * 128;
+  p.stage_bytes = (p.passes == 3 ? 2 : 1) * (kATileBytes + p.b_tile_bytes);
+  return p;
+}
+
 int conv_launch(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift, int pre_relu,
                 const void* w_hi, const void* w_lo, int f16, const float* bias, const float* residual,
                 const float* relu_mask, float* y, float out_scale, const float* in_scale, int B, int H, int W, int Cin,
@@ -955,16 +1082,7 @@ int conv_launch(const float* x, const float* pre_mean, const float* pre_scale, c
   FPD_REQUIRE((pre_scale == nullptr) == (pre_shift == nullptr), "conv_wgmma: pre_scale/pre_shift come in pairs");
   FPD_REQUIRE(pre_scale != nullptr || pre_mean == nullptr, "conv_wgmma: pre_mean needs pre_scale/pre_shift");
   FPD_REQUIRE(stat_part == nullptr || Cout <= kMaxStatCout, "conv_wgmma: statistics need Cout <= %d", kMaxStatCout);
-  ConvParams p{};
-  p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.Cout = Cout; p.ksize = ksize; p.P = B * H * W;
-  p.passes = w_lo ? 3 : 1;
-  p.nt = conv_tc_ts_slice(Cout);
-  p.n_tiles = Cout / p.nt;
-  p.num_tiles = conv_num_tiles(B, H, W, Cout);
-  p.ncb = (Cin + (f16 ? 63 : 31)) / (f16 ? 64 : 32);
-  p.ksteps = ksize * ksize * p.ncb;
-  p.b_tile_bytes = p.nt * 128;
-  p.stage_bytes = (p.passes == 3 ? 2 : 1) * (kATileBytes + p.b_tile_bytes);
+  ConvParams p = conv_shape_params(B, H, W, Cin, Cout, ksize, f16, w_lo ? 3 : 1);
   p.x = x; p.w_hi = w_hi; p.w_lo = w_lo;
   p.pre_mean = pre_mean; p.pre_scale = pre_scale; p.pre_shift = pre_shift; p.pre_relu = pre_relu;
   p.bias = bias; p.residual = residual; p.relu_mask = relu_mask; p.y = y;
@@ -983,17 +1101,47 @@ int conv_launch(const float* x, const float* pre_mean, const float* pre_scale, c
       h.halo_stages = stages;
       const size_t smem = 1024 + (size_t)stages * h.stage_bytes + 2 * (size_t)h.ncb * h.halo_rows * 128 + stat_bytes +
                           (size_t)stages * 2 * 8;
-      if (smem <= (size_t)kSmemLimit) return launch_halo(h, grid, smem, stream);
+      if (smem <= (size_t)kSmemLimit) return launch_halo<true>(h, grid, smem, stream);
     }
   }
   if (f16 && p.passes == 3 && ksize == 1 && stat_part == nullptr && g_conv1x1.load(std::memory_order_relaxed)) {
     // 1x1 3xFP16: the weight-resident kernel wherever the slice's weights and two A stages fit
-    const size_t smem = pw_smem_bytes(p.ncb, p.nt);
-    if (smem <= (size_t)kSmemLimit) return launch_pw(p, grid, smem, stream);
+    const size_t smem = pw_smem_bytes<true>(p.ncb, p.nt);
+    if (smem <= (size_t)kSmemLimit) return launch_pw<true>(p, grid, smem, stream);
   }
   const size_t smem = 1024 + (size_t)kStages * p.stage_bytes + stat_bytes;
   FPD_REQUIRE(smem <= (size_t)kSmemLimit, "conv_wgmma: shared memory plan %zu B too large", smem);
   return f16 ? launch_f<true>(p, grid, smem, stream) : launch_f<false>(p, grid, smem, stream);
+}
+
+// Single-pass FP16 (conv_f16x1_launch): which kernel takes the shape, from the shape alone. 0: unsupported; 2: 3x3 on
+// conv_halo_f16x1_kernel where the hi-only halo and a ring of four (else three) weight stages fit; 3: 1x1 on
+// pw_conv_f16x1_kernel where the slice's hi weights and three A stages fit; 1: everything else on the staged
+// conv_wgmma_kernel<true, kN> (w_lo == nullptr). Sets the kernel's ring and stage sizes in `p` and its shared memory.
+constexpr int kHalo1MaxStages = 4;
+
+int f16x1_plan(ConvParams& p, size_t& smem) {
+  if (!conv_shape_ok(p.Cin, p.Cout, p.ksize, 1, kMaxCinH, 2048) || p.B < 1 || p.H < 1 || p.W < 1 ||
+      (double)p.B * p.H * p.W * p.Cout >= 4294967296.0)
+    return 0;
+  if (p.ksize == 3) {
+    ConvParams h = p;
+    h.halo_rows = kTileM + 2 * p.W + 3;
+    h.stage_bytes = p.b_tile_bytes;
+    for (int stages = kHalo1MaxStages; stages >= 3; --stages) {
+      h.halo_stages = stages;
+      smem = 1024 + (size_t)stages * h.stage_bytes + (size_t)h.ncb * h.halo_rows * 128 + (size_t)stages * 2 * 8;
+      if (smem <= (size_t)kSmemLimit) {
+        p = h;
+        return 2;
+      }
+    }
+  } else {
+    smem = pw_smem_bytes<false>(p.ncb, p.nt);
+    if (smem <= (size_t)kSmemLimit) return 3;
+  }
+  smem = 1024 + (size_t)kStages * p.stage_bytes;
+  return 1;
 }
 
 // ================================================= weight gradient =================================================
@@ -1494,6 +1642,36 @@ int conv_tc_h_launch(const float* x, const float* pre_mean, const float* pre_sca
               "conv_tc_h: unsupported shape Cin=%d Cout=%d k=%d H=%d W=%d f16=%d", Cin, Cout, ksize, H, W, f16);
   return conv_launch(x, pre_mean, pre_scale, pre_shift, pre_relu, w_hi, w_lo, f16, bias, residual, relu_mask, y,
                      out_scale, in_scale, B, H, W, Cin, Cout, ksize, num_sms, stream, stat_part, stat_pivot);
+}
+
+int conv_f16x1_kernel(int B, int H, int W, int Cin, int Cout, int ksize) {
+  if (!conv_shape_ok(Cin, Cout, ksize, 1, kMaxCinH, 2048)) return 0;
+  ConvParams p = conv_shape_params(B, H, W, Cin, Cout, ksize, 1, 1);
+  size_t smem = 0;
+  return f16x1_plan(p, smem);
+}
+
+int conv_f16x1_launch(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
+                      int pre_relu, const void* w, const float* bias, const float* residual, const float* relu_mask,
+                      float* y, float out_scale, int B, int H, int W, int Cin, int Cout, int ksize, int num_sms,
+                      cudaStream_t stream) {
+  FPD_REQUIRE(x && w && y, "conv_f16x1: null operand");
+  FPD_REQUIRE((pre_scale == nullptr) == (pre_shift == nullptr), "conv_f16x1: pre_scale/pre_shift come in pairs");
+  FPD_REQUIRE(pre_scale != nullptr || pre_mean == nullptr, "conv_f16x1: pre_mean needs pre_scale/pre_shift");
+  FPD_REQUIRE(conv_shape_ok(Cin, Cout, ksize, 1, kMaxCinH, 2048),
+              "conv_f16x1: unsupported shape Cin=%d Cout=%d k=%d H=%d W=%d", Cin, Cout, ksize, H, W);
+  ConvParams p = conv_shape_params(B, H, W, Cin, Cout, ksize, 1, 1);
+  size_t smem = 0;
+  const int kind = f16x1_plan(p, smem);
+  FPD_REQUIRE(kind > 0, "conv_f16x1: unsupported shape B=%d H=%d W=%d Cin=%d Cout=%d k=%d", B, H, W, Cin, Cout, ksize);
+  p.x = x; p.w_hi = w; p.w_lo = nullptr;
+  p.pre_mean = pre_mean; p.pre_scale = pre_scale; p.pre_shift = pre_shift; p.pre_relu = pre_relu;
+  p.bias = bias; p.residual = residual; p.relu_mask = relu_mask; p.y = y;
+  p.out_scale = out_scale * (1.0f / (float)(1 << kF16WeightScaleLog2));
+  const int grid = p.num_tiles < num_sms ? p.num_tiles : num_sms;
+  if (kind == 2) return launch_halo<false>(p, grid, smem, stream);
+  if (kind == 3) return launch_pw<false>(p, grid, smem, stream);
+  return launch_f<true>(p, grid, smem, stream);
 }
 
 // ---------------------------------------------- weight-gradient entry points ----------------------------------------------

@@ -34,6 +34,33 @@ def precision_passes():
     raise ValueError("FPD_PRECISION must be tf32x3 or tf32, got %r" % mode)
 
 
+INFERENCE_PRECISIONS = ("fp32", "fp16")
+
+
+def set_inference_precision(model, precision):
+    """Operand precision of `model`'s eval-mode forwards that record no tape (net(x) under no_grad, forward_nhwc,
+    FlipTestInference, a frozen FPD teacher): "fp32" (the default: 3xFP16 / 3xTF32, fp32-grade) or "fp16" (single-pass
+    FP16 on ops.conv2d_tc_f16x1 for every convolution it takes: about 2^-11 relative operand rounding, one MMA per
+    product instead of three). Training forwards and forwards that record a backward tape always run at fp32 grade.
+    `model`: an fpd_b200 hourglass / HRNet / ResNet network or an nn.DataParallel around one. Returns the previous
+    setting; a change drops the cached eval operands and bumps the engine generation, so captured graphs capture again."""
+    from .lib.models.hourglass import HourglassNet
+    from .lib.models.pose_hrnet import PoseHighResolutionNet
+    from .lib.models.pose_resnet import PoseResNet
+    if precision not in INFERENCE_PRECISIONS:
+        raise ValueError("inference precision must be one of %s, got %r" % (INFERENCE_PRECISIONS, precision))
+    net = model.module if isinstance(model, torch.nn.DataParallel) else model
+    if not isinstance(net, (HourglassNet, PoseHighResolutionNet, PoseResNet)):
+        raise TypeError("set_inference_precision takes an fpd_b200 hourglass / HRNet / ResNet network (or an "
+                        "nn.DataParallel around one), got %s" % type(net).__name__)
+    eng = net.engine()
+    prev = eng.inference_precision
+    if precision != prev:
+        eng.inference_precision = precision
+        eng.invalidate_eval_cache()
+    return prev
+
+
 class Var:
     """An activation tensor (NHWC) plus its gradient slot and cached batch statistics."""
     __slots__ = ("data", "grad", "owned", "stats", "stat_sums", "grad_sum")
@@ -148,14 +175,20 @@ class BNRef:
         self.mod = mod
 
 
+F16X1 = "f16x1"   # PreparedWeights.fwd's kernel choice for single-pass FP16 weights (ops.conv2d_tc_f16x1)
+
+
 class PreparedWeights:
     """Tensor-core operand forms of the conv weights, prepared on first use within a forward (student: every step,
     inside the captured graph; frozen teacher: once, cached with the eval context):
     [tap][O][I] hi/lo (+ flipped/transposed for dgrad). Forward operands are __half pairs (3xFP16, csrc/conv_wgmma.cu)
-    where ops.conv2d_tc_h takes the shape, fp32 containers holding tf32 values otherwise."""
+    where ops.conv2d_tc_h takes the shape, fp32 containers holding tf32 values otherwise.
+    f16x1 (eval-mode forwards without a tape at inference precision "fp16"): a single __half array of w * 2^8 for every
+    convolution ops.conv2d_tc_f16x1 takes, marked F16X1 in place of use_h."""
 
-    def __init__(self, passes, scale_without_bias=False):
+    def __init__(self, passes, scale_without_bias=False, f16x1=False):
         self.split = passes == 3
+        self.f16x1 = f16x1
         self._fwd = {}
         self._dgrad = {}
         self.derived = {}      # name -> ConvRef with weights derived from another module's (Engine.deconv)
@@ -179,7 +212,9 @@ class PreparedWeights:
             w2 = torch.zeros((c.cout, kpad, 1, 1), dtype=torch.float32, device=w.device)
             w2[:, :c.cin * c.k * c.k, 0, 0] = w.permute(0, 2, 3, 1).reshape(c.cout, -1)
             w, k, cin = w2, 1, kpad
-        if self.split and ops.CONV_F16 and ops.conv2d_tc_h_supported(cin, c.cout, k, H, W, True):
+        if self.f16x1 and ops.conv2d_tc_f16x1_kernel(1, H, W, cin, c.cout, k):
+            e = (ops.weight_prep_f16(w, for_dgrad=False, split=False)[0], None, F16X1)
+        elif self.split and ops.CONV_F16 and ops.conv2d_tc_h_supported(cin, c.cout, k, H, W, True):
             if (also_dgrad and not kpad and ops.CONV_F16_DGRAD and ops.FUSED_REDUCE
                     and (c.bias is not None or self.scale_without_bias) and c.tc_dgrad_at(H, W) and ops.conv2d_tc_h_supported(c.cout, c.cin, c.k, H, W, True)):
                 (hi, lo), (dhi, dlo) = ops.weight_prep_f16_both(w)
@@ -210,6 +245,13 @@ class PreparedWeights:
         return e
 
 
+def _conv_fwd(use_h, x, w_hi, w_lo, k, **kw):
+    """The tensor-core forward convolution PreparedWeights.fwd prepared the weights for."""
+    if use_h == F16X1:
+        return ops.conv2d_tc_f16x1(x, w_hi, k, **kw)
+    return (ops.conv2d_tc_h if use_h else ops.conv2d_tc_fused)(x, w_hi, w_lo, k, **kw)
+
+
 class Engine:
     """Runs one forward (and optionally records a backward tape) of a hourglass-family module tree."""
 
@@ -227,6 +269,7 @@ class Engine:
                 self.deconvs[name] = m
         self._eval_cache = None
         self._eval_cache_key = None
+        self.inference_precision = "fp32"   # set_inference_precision
         # True: the BatchNorm-backward apply pass always also reduces its output (sum + max |dx|): engines whose convolutions
         # have no bias (HRNet) get the 3xFP16 operand scale of dY from it -- without it their data gradients run on 3xTF32
         self.force_apply_sum = False
@@ -262,7 +305,7 @@ class Engine:
         key = self._param_version()
         if self._eval_cache is None or self._eval_cache_key != key:
             passes = precision_passes()
-            w = PreparedWeights(passes)
+            w = PreparedWeights(passes, f16x1=self.inference_precision == "fp16")
             affine = {}
             for name, b in self.bns.items():
                 m = b.mod
@@ -405,8 +448,7 @@ class Engine:
                 if ctx.shared_stem is not None and "cols_key" not in ctx.shared_stem:
                     ctx.shared_stem["cols_key"], ctx.shared_stem["cols"] = key, cols
             w_hi, w_lo, use_h = ctx.weights.fwd(c, cols.shape[1], cols.shape[2])
-            conv_fn = ops.conv2d_tc_h if use_h else ops.conv2d_tc_fused
-            out = Var(conv_fn(cols, w_hi, w_lo, 1, bias=bias, residual=res))
+            out = Var(_conv_fwd(use_h, cols, w_hi, w_lo, 1, bias=bias, residual=res))
             if ctx.tape is not None:
                 def bwd_stem():
                     dy = out.grad
@@ -441,9 +483,8 @@ class Engine:
                                     residual=res, stats_part=stat_sums[0], stats_pivot=stat_sums[2])
             else:
                 # BN-apply + ReLU + operand split happen inside the conv kernel (no separate HBM pass)
-                conv_fn = ops.conv2d_tc_h if use_h else ops.conv2d_tc_fused
-                y = conv_fn(x.data, w_hi, w_lo, c.k, mean=mean, scale=scale, shift=shift, relu=relu, bias=bias,
-                            residual=res)
+                y = _conv_fwd(use_h, x.data, w_hi, w_lo, c.k, mean=mean, scale=scale, shift=shift, relu=relu,
+                              bias=bias, residual=res)
         else:
             a = ops.affine_act(x.data, scale, shift, relu, mean=mean) if bn_name is not None else x.data
             y = ops.conv2d_simt_fwd(a, c.weight.detach(), bias=bias, residual=res, stride=c.stride, pad=c.pad)

@@ -257,6 +257,31 @@ def conv2d_tc_h(x, w_hi, w_lo, ksize, mean=None, scale=None, shift=None, relu=Fa
     return y
 
 
+F16X1_KERNELS = {0: None, 1: "staged", 2: "halo", 3: "1x1"}
+
+
+def conv2d_tc_f16x1_kernel(B, H, W, Cin, Cout, k):
+    """Which kernel conv2d_tc_f16x1 runs this shape on: "halo" (3x3, conv_halo_f16x1_kernel), "1x1"
+    (pw_conv_f16x1_kernel), "staged" (conv_wgmma_kernel) or None (unsupported). Host only."""
+    return F16X1_KERNELS[int(N.lib().fpd_conv2d_tc_f16x1_kernel(B, H, W, Cin, Cout, k))]
+
+
+def conv2d_tc_f16x1(x, w, ksize, mean=None, scale=None, shift=None, relu=False, bias=None, residual=None,
+                    relu_mask=None, out=None, out_scale=1.0):
+    """y = conv(relu?((x-mean)*scale+shift)) with single-pass FP16 operands: fp16_rn of the transformed activation times
+    w = weight_prep_f16(w_oihw, split=False)[0], one MMA per product, fp32 accumulation (about 2^-11 relative operand
+    rounding: for inference, never for gradients)."""
+    B, H, W, Cin = x.shape
+    Cout = w.shape[1]
+    if w.dtype != torch.float16:
+        raise ValueError("conv2d_tc_f16x1 takes the __half weights of weight_prep_f16(split=False), got %s" % w.dtype)
+    y = out if out is not None else torch.empty((B, H, W, Cout), dtype=torch.float32, device=x.device)
+    N.check(N.lib().fpd_conv2d_tc_f16x1(_p(x), _p(mean), _p(scale), _p(shift), int(relu), _p(w), _p(bias), _p(residual),
+                                        _p(relu_mask), _p(y), float(out_scale), B, H, W, Cin, Cout, ksize, _stream()),
+            "conv2d_tc_f16x1")
+    return y
+
+
 def conv2d_simt_fwd(x, w_oihw, bias=None, residual=None, stride=1, pad=0, out=None):
     B, H, W, Cin = x.shape
     Cout, _, k, _ = w_oihw.shape

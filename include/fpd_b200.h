@@ -82,6 +82,18 @@ int fpd_set_conv1x1(int enabled);
  * the staged kernel (enabled = 0), for bit-identity checks between the two. Process-wide; affects launches made after
  * the call; returns the previous setting. */
 int fpd_set_conv_halo(int enabled);
+/* Single-pass FP16 forward convolution for inference: y = conv(relu?((x - mean) * scale + shift)) (+ bias, + residual,
+ * ReLU mask) with ONE fp16 MMA per product: the operand is fp16_rn of the (saturated) transformed activation -- the hi
+ * half of the 3xFP16 split -- and w the single __half array of fpd_weight_prep_f16(w_lo = NULL), w * 2^8; fp32
+ * accumulation. Relative error about 2^-11 per operand instead of fp32 grade: for eval-mode forwards whose output feeds
+ * no gradient. No epilogue statistics, no in_scale. fpd_conv2d_tc_f16x1_kernel says which kernel a shape runs on
+ * (host only, no device needed): 0 unsupported, 1 the staged kernel, 2 the 3x3 halo kernel, 3 the 1x1 weight-resident
+ * kernel. */
+int fpd_conv2d_tc_f16x1_kernel(int B, int H, int W, int Cin, int Cout, int ksize);
+int fpd_conv2d_tc_f16x1(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
+                        int pre_relu, const void* w, const float* bias, const float* residual, const float* relu_mask,
+                        float* y, float out_scale, int B, int H, int W, int Cin, int Cout, int ksize,
+                        fpd_stream_t stream);
 /* Forward ([tap][O][I]) and data-gradient ([taps-1-tap][I][O]) __half hi/lo forms of w * 2^8 from one read of the
  * weights: one launch per convolution and training step instead of two. */
 int fpd_weight_prep_f16_both(const float* w_oihw, void* f_hi, void* f_lo, void* d_hi, void* d_lo, int O, int I, int k,

@@ -6,7 +6,10 @@ than the 50 MB L2), with an L2 flush before every timed window; the two kernels'
 (median and range over the windows), the least HBM bytes of one launch (input, output, and residual where the call has
 one: weights are read from L2) and the achieved share of 3.35 TB/s, with the card's name, power limit and SM clock.
 
-    python tools/bench_conv1x1.py [--windows 7] [--per 8]
+With --single-pass, the forward forms instead run on the 3-pass weight-resident kernel against the single-pass one
+(ops.conv2d_tc_f16x1, pw_conv_f16x1_kernel); the HBM share is then the single-pass kernel's.
+
+    python tools/bench_conv1x1.py [--windows 7] [--per 8] [--single-pass]
 """
 import argparse
 import os
@@ -37,7 +40,7 @@ def card():
     return q
 
 
-def setup(B, H, W, Cin, Cout, form, g):
+def setup(B, H, W, Cin, Cout, form, g, single=False):
     from fpd_b200 import ops
     xs = [torch.randn(B, H, W, Cin, device="cuda", generator=g) for _ in range(2)]
     ys = [torch.empty(B, H, W, Cout, device="cuda") for _ in range(2)]
@@ -55,7 +58,11 @@ def setup(B, H, W, Cin, Cout, form, g):
     nbytes = 4 * B * H * W * (Cin + Cout * (2 if res else 1))
 
     def launch(i):
-        ops.conv2d_tc_h(xs[i % 2], w_hi, w_lo, 1, residual=res[i % 2] if res else None, out=ys[i % 2], **kw)
+        if single:
+            ops.conv2d_tc_f16x1(xs[i % 2], w1, 1, residual=res[i % 2] if res else None, out=ys[i % 2], **kw)
+        else:
+            ops.conv2d_tc_h(xs[i % 2], w_hi, w_lo, 1, residual=res[i % 2] if res else None, out=ys[i % 2], **kw)
+    w1 = ops.weight_prep_f16(w, split=False)[0] if single else None
     return launch, nbytes
 
 
@@ -81,6 +88,7 @@ def main():
     ap.add_argument("--per", type=int, default=8)
     ap.add_argument("--batch", type=int, default=32)
     ap.add_argument("--hw", type=int, default=64)
+    ap.add_argument("--single-pass", action="store_true")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "bench_conv1x1 measures on the GPU"
     import fpd_b200  # noqa: F401
@@ -89,18 +97,25 @@ def main():
     B, H, W = args.batch, args.hw, args.hw
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
     g = torch.Generator(device="cuda").manual_seed(0)
+    names = ("1-pass", "3-pass") if args.single_pass else ("pw", "staged")
     print("%-22s %6s %10s %22s %10s %22s %8s %9s %7s" % (
-        "shape (Cin->Cout form)", "x/step", "pw us", "pw range", "staged us", "staged range", "speedup", "least MB",
-        "HBM %"))
+        "shape (Cin->Cout form)", "x/step", names[0] + " us", names[0] + " range", names[1] + " us",
+        names[1] + " range", "speedup", "least MB", "HBM %"))
     prev = ops.set_conv1x1(True)
     tot_pw = tot_st = 0.0
     try:
         for (Cin, Cout, form, n) in SHAPES:
+            if args.single_pass and form == "dgrad":
+                continue
             launch, nbytes = setup(B, H, W, Cin, Cout, form, g)
             graphs = {}
             for on in (True, False):
                 ops.set_conv1x1(on)
                 graphs[on] = capture(launch, args.per)
+            if args.single_pass:   # True: single pass, False: the 3-pass weight-resident kernel
+                ops.set_conv1x1(True)
+                graphs = {False: graphs[True], True: capture(setup(B, H, W, Cin, Cout, form, g, single=True)[0],
+                                                             args.per)}
             times = {True: [], False: []}
             for _ in range(args.windows):
                 for on in (True, False):
@@ -123,7 +138,8 @@ def main():
             torch.cuda.empty_cache()
     finally:
         ops.set_conv1x1(prev)
-    print("these shapes, one step at %dx%d: pw %.2f ms, staged %.2f ms" % (H, W, tot_pw / 1000.0, tot_st / 1000.0))
+    print("these shapes, one step at %dx%d: %s %.2f ms, %s %.2f ms" % (H, W, names[0], tot_pw / 1000.0, names[1],
+                                                                       tot_st / 1000.0))
     print("device: %s (name, power limit, SM clock, max SM clock)" % card())
 
 

@@ -8,7 +8,10 @@ Prints µs per launch (median and range over the windows), the launch-weighted p
 fp16 tensor-core peak in executed MMAs (3 passes x the algorithmic FLOPs at 989 TFLOP/s, the H100 SXM data sheet's
 dense figure), with the card's name, power limit and SM clock.
 
-    python tools/bench_conv3x3.py [--windows 7] [--per 8]
+With --single-pass, each forward form also runs on ops.conv2d_tc_f16x1 (single-pass FP16, no epilogue statistics),
+the two alternating window by window, and the single-pass share of the fp16 peak counts 1 x the algorithmic FLOPs.
+
+    python tools/bench_conv3x3.py [--windows 7] [--per 8] [--single-pass]
 """
 import argparse
 import collections
@@ -78,7 +81,7 @@ def step_shapes():
     return counts
 
 
-def setup(shape, g):
+def setup(shape, g, single=False):
     from fpd_b200 import ops
     B, H, W, Cin, Cout, form = shape
     xs = [torch.randn(B, H, W, Cin, device="cuda", generator=g) * (1e-3 if form.startswith("dgrad") else 1.0)
@@ -104,7 +107,15 @@ def setup(shape, g):
     def launch(i):
         ops.conv2d_tc_h(xs[i % 2], w_hi, w_lo, 3, residual=res[i % 2] if res else None,
                         relu_mask=mask[i % 2] if mask else None, out=ys[i % 2], **kw)
-    return launch
+    if not single:
+        return launch
+    w1, _ = ops.weight_prep_f16(w, split=False)
+    kw1 = {k: v for k, v in kw.items() if not k.startswith("stats")}
+
+    def launch1(i):
+        ops.conv2d_tc_f16x1(xs[i % 2], w1, 3, residual=res[i % 2] if res else None,
+                            relu_mask=mask[i % 2] if mask else None, out=ys[i % 2], **kw1)
+    return launch, launch1
 
 
 def capture(launch, per):
@@ -127,11 +138,14 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--windows", type=int, default=7)
     ap.add_argument("--per", type=int, default=8)
+    ap.add_argument("--single-pass", action="store_true")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "bench_conv3x3 measures on the GPU"
     import fpd_b200  # noqa: F401
     print("device: %s (name, power limit, SM clock, max SM clock)" % card())
     shapes = step_shapes()
+    if args.single_pass:
+        return single_pass(shapes, args)
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
     g = torch.Generator(device="cuda").manual_seed(0)
     print("%-40s %6s %10s %18s %8s" % ("shape (B,H,W,Cin->Cout form)", "x/step", "us", "range", "%F16"))
@@ -158,6 +172,48 @@ def main():
         del graph, launch
         torch.cuda.empty_cache()
     print("3x3 3xFP16 convolutions of one hg_fpd step: %.2f ms" % (tot / 1000.0))
+    print("device: %s (name, power limit, SM clock, max SM clock)" % card())
+
+
+def window(graph, per, flush):
+    flush.zero_()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    graph.replay()
+    e1.record()
+    torch.cuda.synchronize()
+    return 1000.0 * e0.elapsed_time(e1) / per
+
+
+def single_pass(shapes, args):
+    """The step's forward forms on the 3-pass kernel against the single-pass one, windows alternating."""
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
+    g = torch.Generator(device="cuda").manual_seed(0)
+    print("%-40s %6s %10s %14s %10s %14s %8s %8s" % ("shape (B,H,W,Cin->Cout form)", "x/step", "3-pass us", "range",
+                                                     "1-pass us", "range", "speedup", "%F16 1x"))
+    tot3 = tot1 = 0.0
+    for shape, n in sorted(shapes.items(), key=lambda kv: -kv[0][0] * kv[0][1] * kv[0][2] * kv[0][3] * kv[0][4] * kv[1]):
+        B, H, W, Cin, Cout, form = shape
+        if form.startswith("dgrad"):
+            continue
+        launches = setup(shape, g, single=True)
+        graphs = [capture(fn, args.per) for fn in launches]
+        times = [[], []]
+        for _ in range(args.windows):
+            for i, gr in enumerate(graphs):
+                times[i].append(window(gr, args.per, flush))
+        med = [sorted(t)[len(t) // 2] for t in times]
+        tot3 += n * med[0]
+        tot1 += n * med[1]
+        bound_us = 2.0 * B * H * W * Cin * Cout * 9 / F16_FLOPS * 1e6
+        print("%-40s %6d %10.1f %14s %10.1f %14s %7.2fx %7.1f%%" % (
+            "%d,%d,%d,%d->%d %s" % (B, H, W, Cin, Cout, form), n, med[0], "%.1f-%.1f" % (min(times[0]), max(times[0])),
+            med[1], "%.1f-%.1f" % (min(times[1]), max(times[1])), med[0] / med[1], 100.0 * bound_us / med[1]),
+            flush=True)
+        del graphs, launches
+        torch.cuda.empty_cache()
+    print("3x3 forward convolutions of one hg_fpd step: 3-pass %.2f ms, single-pass %.2f ms" % (tot3 / 1000.0,
+                                                                                              tot1 / 1000.0))
     print("device: %s (name, power limit, SM clock, max SM clock)" % card())
 
 
