@@ -32,6 +32,9 @@ _SIGNATURES = {
     "fpd_conv2d_tc_f16x1_kernel": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int]),
     "fpd_conv2d_tc_f16x1": (c_int, [P, P, P, P, c_int, P, P, P, P, P, c_float, c_int, c_int, c_int, c_int, c_int, c_int,
                                     P]),
+    "fpd_conv2d_tc_f16x1_train_plan": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_int)]),
+    "fpd_conv2d_tc_f16x1_train": (c_int, [P, P, P, P, c_int, P, P, P, P, P, c_float, P, c_int, c_int, c_int, c_int, c_int,
+                                          c_int, P, P, P]),
     "fpd_set_conv1x1": (c_int, [c_int]),
     "fpd_set_conv_halo": (c_int, [c_int]),
     "fpd_set_wgrad_halo": (c_int, [c_int]),

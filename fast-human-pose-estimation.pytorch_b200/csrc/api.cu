@@ -62,15 +62,28 @@ int fpd_conv2d_tc_h(const float* x, const float* pre_mean, const float* pre_scal
 }
 
 int fpd_conv2d_tc_f16x1_kernel(int B, int H, int W, int Cin, int Cout, int ksize) {
-  return conv_f16x1_kernel(B, H, W, Cin, Cout, ksize);
+  return conv_f16x1_kernel(B, H, W, Cin, Cout, ksize, 0, 0, nullptr);
 }
 
 int fpd_conv2d_tc_f16x1(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
                         int pre_relu, const void* w, const float* bias, const float* residual, const float* relu_mask,
                         float* y, float out_scale, int B, int H, int W, int Cin, int Cout, int ksize,
                         fpd_stream_t stream) {
-  return conv_f16x1_launch(x, pre_mean, pre_scale, pre_shift, pre_relu, w, bias, residual, relu_mask, y, out_scale, B,
-                           H, W, Cin, Cout, ksize, device_sm_count(), S(stream));
+  return conv_f16x1_launch(x, pre_mean, pre_scale, pre_shift, pre_relu, w, bias, residual, relu_mask, y, out_scale,
+                           nullptr, B, H, W, Cin, Cout, ksize, device_sm_count(), S(stream), nullptr, nullptr);
+}
+
+int fpd_conv2d_tc_f16x1_train_plan(int B, int H, int W, int Cin, int Cout, int ksize, int stats, int* stat_blocks) {
+  return conv_f16x1_kernel(B, H, W, Cin, Cout, ksize, stats, device_sm_count(), stat_blocks);
+}
+
+int fpd_conv2d_tc_f16x1_train(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
+                              int pre_relu, const void* w, const float* bias, const float* residual,
+                              const float* relu_mask, float* y, float out_scale, const float* in_scale, int B, int H,
+                              int W, int Cin, int Cout, int ksize, double* stat_part, const float* stat_pivot,
+                              fpd_stream_t stream) {
+  return conv_f16x1_launch(x, pre_mean, pre_scale, pre_shift, pre_relu, w, bias, residual, relu_mask, y, out_scale,
+                           in_scale, B, H, W, Cin, Cout, ksize, device_sm_count(), S(stream), stat_part, stat_pivot);
 }
 
 int fpd_set_conv1x1(int enabled) { return set_conv1x1(enabled); }

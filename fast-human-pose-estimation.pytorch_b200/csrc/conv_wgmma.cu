@@ -16,8 +16,9 @@
 //   accumulators merged in a fixed order (deterministic), one [Cout][2] block per CTA for bn_finalize_sums.
 //   3x3 with 3xFP16 operands (conv_halo_kernel, selected by conv_launch where it fits in shared memory): the same GEMM
 //   with the A operand of a tile loaded and transformed once into a halo in shared memory and fed from registers.
-//   Single-pass FP16 for inference (conv_f16x1_launch): the halo and 1x1 weight-resident kernels with kSplit = false
-//   (conv_halo_f16x1_kernel, pw_conv_f16x1_kernel), one MMA per k16 straight into the accumulators.
+//   Single-pass FP16 (conv_f16x1_launch): the halo and 1x1 weight-resident kernels with kSplit = false
+//   (conv_halo_f16x1_kernel, pw_conv_f16x1_kernel), one MMA per k16 straight into the accumulators. Inference calls,
+//   and the training precision "fp16": forward calls with epilogue statistics, data gradients with in_scale.
 //
 // Weight gradient (wgrad_tc_*):
 //   dW[co][ci][tap] = scale * sum_{pixels p} dY[p][co] * A[p (+) tap][ci],  A = relu?((x - mean) * scale + shift)
@@ -762,6 +763,9 @@ __device__ __forceinline__ void pw_epilogue(const ConvParams& p, const float (&a
 // slice fits up to Cin = 640 at 128 columns), one MMA per k16 straight into `acc`. Three A stages and wgmma_wait<1>
 // before each step's barrier keep one step's MMAs in flight across it: stage s % 3 is rewritten by step s after the
 // barrier of step s - 1, which follows every warpgroup's retirement of step s - 3.
+//   Optional epilogue statistics (training calls): the [8 warps][Cout][2] fp64 accumulators follow the resident
+// weights; tiles with statistics take conv_epilogue (same outputs as pw_epilogue, plus the per-warp sums) and the CTA
+// flushes one block at the end, merged in the fixed order of conv_stats_flush. The 3-pass kernel has no statistics.
 constexpr int kPwStages1 = 3;
 
 template <bool kSplit>
@@ -782,6 +786,8 @@ __device__ __forceinline__ void pw_conv_body(const ConvParams& p) {
   const int tid = threadIdx.x, wg = tid >> 7;
   const float in_s = p.in_scale ? __ldg(p.in_scale) : 1.f;
   const float oscale = p.in_scale ? p.out_scale * __ldg(p.in_scale + 1) : p.out_scale;
+  double* s_stat = reinterpret_cast<double*>(smem + (size_t)kNumStages * kAStage + (size_t)p.ncb * w_step);
+  if constexpr (!kSplit) conv_stats_init(p, s_stat);   // visible after the first K step's barrier
 
   // A tile: thread -> 16-byte chunk j (channels 8 j .. 8 j + 7 of the block) of rows r0 + 32 i
   const int j = tid & 7, r0 = tid >> 3;
@@ -869,8 +875,15 @@ __device__ __forceinline__ void pw_conv_body(const ConvParams& p) {
     }
     wgmma_wait<0>();
     if (kSplit) add_part(acc, part);
+    if constexpr (!kSplit) {
+      if (p.stat_part) {
+        conv_epilogue<kN>(p, acc, m0, n0, oscale, s_stat);
+        continue;
+      }
+    }
     pw_epilogue<kN>(p, acc, m0, n0, oscale);
   }
+  if constexpr (!kSplit) conv_stats_flush(p, s_stat);
 }
 
 template <int kN>
@@ -1114,33 +1127,36 @@ int conv_launch(const float* x, const float* pre_mean, const float* pre_scale, c
   return f16 ? launch_f<true>(p, grid, smem, stream) : launch_f<false>(p, grid, smem, stream);
 }
 
-// Single-pass FP16 (conv_f16x1_launch): which kernel takes the shape, from the shape alone. 0: unsupported; 2: 3x3 on
-// conv_halo_f16x1_kernel where the hi-only halo and a ring of four (else three) weight stages fit; 3: 1x1 on
-// pw_conv_f16x1_kernel where the slice's hi weights and three A stages fit; 1: everything else on the staged
-// conv_wgmma_kernel<true, kN> (w_lo == nullptr). Sets the kernel's ring and stage sizes in `p` and its shared memory.
+// Single-pass FP16 (conv_f16x1_launch): which kernel takes the shape, from the shape alone. 0: unsupported (also:
+// statistics with Cout > kMaxStatCout); 2: 3x3 on conv_halo_f16x1_kernel where the hi-only halo, the statistics scratch
+// (`stats`) and a ring of four (else three) weight stages fit; 3: 1x1 on pw_conv_f16x1_kernel where the slice's hi
+// weights, three A stages and the statistics scratch fit; 1: everything else on the staged conv_wgmma_kernel<true, kN>
+// (w_lo == nullptr). Sets the kernel's ring and stage sizes in `p` and its shared memory.
 constexpr int kHalo1MaxStages = 4;
 
-int f16x1_plan(ConvParams& p, size_t& smem) {
+int f16x1_plan(ConvParams& p, size_t& smem, bool stats) {
   if (!conv_shape_ok(p.Cin, p.Cout, p.ksize, 1, kMaxCinH, 2048) || p.B < 1 || p.H < 1 || p.W < 1 ||
-      (double)p.B * p.H * p.W * p.Cout >= 4294967296.0)
+      (double)p.B * p.H * p.W * p.Cout >= 4294967296.0 || (stats && p.Cout > kMaxStatCout))
     return 0;
+  const size_t stat_bytes = stats ? (size_t)8 * p.Cout * 2 * sizeof(double) : 0;
   if (p.ksize == 3) {
     ConvParams h = p;
     h.halo_rows = kTileM + 2 * p.W + 3;
     h.stage_bytes = p.b_tile_bytes;
     for (int stages = kHalo1MaxStages; stages >= 3; --stages) {
       h.halo_stages = stages;
-      smem = 1024 + (size_t)stages * h.stage_bytes + (size_t)h.ncb * h.halo_rows * 128 + (size_t)stages * 2 * 8;
+      smem = 1024 + (size_t)stages * h.stage_bytes + (size_t)h.ncb * h.halo_rows * 128 + stat_bytes +
+             (size_t)stages * 2 * 8;
       if (smem <= (size_t)kSmemLimit) {
         p = h;
         return 2;
       }
     }
   } else {
-    smem = pw_smem_bytes<false>(p.ncb, p.nt);
+    smem = pw_smem_bytes<false>(p.ncb, p.nt) + stat_bytes;
     if (smem <= (size_t)kSmemLimit) return 3;
   }
-  smem = 1024 + (size_t)kStages * p.stage_bytes;
+  smem = 1024 + (size_t)kStages * p.stage_bytes + stat_bytes;
   return 1;
 }
 
@@ -1644,30 +1660,36 @@ int conv_tc_h_launch(const float* x, const float* pre_mean, const float* pre_sca
                      out_scale, in_scale, B, H, W, Cin, Cout, ksize, num_sms, stream, stat_part, stat_pivot);
 }
 
-int conv_f16x1_kernel(int B, int H, int W, int Cin, int Cout, int ksize) {
+int conv_f16x1_kernel(int B, int H, int W, int Cin, int Cout, int ksize, int stats, int num_sms, int* stat_blocks) {
+  if (stat_blocks) *stat_blocks = 0;
   if (!conv_shape_ok(Cin, Cout, ksize, 1, kMaxCinH, 2048)) return 0;
   ConvParams p = conv_shape_params(B, H, W, Cin, Cout, ksize, 1, 1);
   size_t smem = 0;
-  return f16x1_plan(p, smem);
+  const int kind = f16x1_plan(p, smem, stats != 0);
+  if (kind > 0 && stats && stat_blocks) *stat_blocks = p.num_tiles < num_sms ? p.num_tiles : num_sms;
+  return kind;
 }
 
 int conv_f16x1_launch(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
                       int pre_relu, const void* w, const float* bias, const float* residual, const float* relu_mask,
-                      float* y, float out_scale, int B, int H, int W, int Cin, int Cout, int ksize, int num_sms,
-                      cudaStream_t stream) {
+                      float* y, float out_scale, const float* in_scale, int B, int H, int W, int Cin, int Cout,
+                      int ksize, int num_sms, cudaStream_t stream, double* stat_part, const float* stat_pivot) {
   FPD_REQUIRE(x && w && y, "conv_f16x1: null operand");
   FPD_REQUIRE((pre_scale == nullptr) == (pre_shift == nullptr), "conv_f16x1: pre_scale/pre_shift come in pairs");
   FPD_REQUIRE(pre_scale != nullptr || pre_mean == nullptr, "conv_f16x1: pre_mean needs pre_scale/pre_shift");
   FPD_REQUIRE(conv_shape_ok(Cin, Cout, ksize, 1, kMaxCinH, 2048),
               "conv_f16x1: unsupported shape Cin=%d Cout=%d k=%d H=%d W=%d", Cin, Cout, ksize, H, W);
+  FPD_REQUIRE(stat_part == nullptr || Cout <= kMaxStatCout, "conv_f16x1: statistics need Cout <= %d", kMaxStatCout);
   ConvParams p = conv_shape_params(B, H, W, Cin, Cout, ksize, 1, 1);
   size_t smem = 0;
-  const int kind = f16x1_plan(p, smem);
+  const int kind = f16x1_plan(p, smem, stat_part != nullptr);
   FPD_REQUIRE(kind > 0, "conv_f16x1: unsupported shape B=%d H=%d W=%d Cin=%d Cout=%d k=%d", B, H, W, Cin, Cout, ksize);
   p.x = x; p.w_hi = w; p.w_lo = nullptr;
   p.pre_mean = pre_mean; p.pre_scale = pre_scale; p.pre_shift = pre_shift; p.pre_relu = pre_relu;
   p.bias = bias; p.residual = residual; p.relu_mask = relu_mask; p.y = y;
   p.out_scale = out_scale * (1.0f / (float)(1 << kF16WeightScaleLog2));
+  p.in_scale = in_scale;
+  p.stat_part = stat_part; p.stat_pivot = stat_pivot;
   const int grid = p.num_tiles < num_sms ? p.num_tiles : num_sms;
   if (kind == 2) return launch_halo<false>(p, grid, smem, stream);
   if (kind == 3) return launch_pw<false>(p, grid, smem, stream);

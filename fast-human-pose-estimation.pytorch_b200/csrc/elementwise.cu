@@ -946,7 +946,7 @@ __global__ void weight_prep_f16_kernel(const float* __restrict__ w, __half* __re
 }
 
 // Forward AND data-gradient operand forms from one read of the weights (one launch per convolution instead of two):
-// fwd [tap][O][I], dgrad [taps-1-tap][I][O], both as fp16 hi/lo of w * scale.
+// fwd [tap][O][I], dgrad [taps-1-tap][I][O], both as fp16 hi/lo of w * scale (hi only when the lo pointers are null).
 __global__ void weight_prep_f16_both_kernel(const float* __restrict__ w, __half* __restrict__ f_hi,
                                             __half* __restrict__ f_lo, __half* __restrict__ d_hi,
                                             __half* __restrict__ d_lo, int O, int I, int k, float scale) {
@@ -961,11 +961,13 @@ __global__ void weight_prep_f16_both_kernel(const float* __restrict__ w, __half*
     v = fminf(fmaxf(v * scale, -65504.f), 65504.f);
     const __half h = __float2half_rn(v);
     const __half l = __float2half_rn(v - __half2float(h));
-    f_hi[i] = h;
-    f_lo[i] = l;
     const size_t di = ((size_t)(taps - 1 - tap) * I + c) * O + o;
+    f_hi[i] = h;
     d_hi[di] = h;
-    d_lo[di] = l;
+    if (f_lo) {
+      f_lo[i] = l;
+      d_lo[di] = l;
+    }
   }
 }
 
@@ -1464,7 +1466,8 @@ int weight_prep_f16(const float* w_oihw, void* w_hi, void* w_lo, int O, int I, i
 
 int weight_prep_f16_both(const float* w_oihw, void* f_hi, void* f_lo, void* d_hi, void* d_lo, int O, int I, int k,
                          cudaStream_t stream) {
-  FPD_REQUIRE(w_oihw && f_hi && f_lo && d_hi && d_lo, "weight_prep_f16_both: null operand");
+  FPD_REQUIRE(w_oihw && f_hi && d_hi, "weight_prep_f16_both: null operand");
+  FPD_REQUIRE((f_lo == nullptr) == (d_lo == nullptr), "weight_prep_f16_both: f_lo and d_lo are both set or both NULL");
   const int64_t n = (int64_t)O * I * k * k;
   weight_prep_f16_both_kernel<<<grid_for(n, 256), 256, 0, stream>>>(w_oihw, (__half*)f_hi, (__half*)f_lo, (__half*)d_hi,
                                                                     (__half*)d_lo, O, I, k,

@@ -33,13 +33,16 @@ int set_conv1x1(int enabled);
 // 3x3 3xFP16 convolutions: the halo kernel where it fits (1, the default) or the staged kernel (0), process-wide;
 // returns the previous setting
 int set_conv_halo(int enabled);
-// Single-pass FP16 forward (w: __half [tap][Cout][Cin] of w * 2^kF16WeightScaleLog2, no lo half), no statistics.
-// conv_f16x1_kernel: 0 unsupported, 1 staged (conv_wgmma_kernel), 2 3x3 halo, 3 1x1 weight-resident; host only.
-int conv_f16x1_kernel(int B, int H, int W, int Cin, int Cout, int ksize);
+// Single-pass FP16 forward (w: __half [tap][Cout][Cin] of w * 2^kF16WeightScaleLog2, no lo half), optional in_scale
+// and epilogue statistics (as conv_tc_h_launch).
+// conv_f16x1_kernel: 0 unsupported, 1 staged (conv_wgmma_kernel), 2 3x3 halo, 3 1x1 weight-resident, for a launch
+// with (stats != 0) or without statistics; *stat_blocks (nullable) = the partial blocks a statistics launch writes, 0
+// without statistics or when unsupported; host only.
+int conv_f16x1_kernel(int B, int H, int W, int Cin, int Cout, int ksize, int stats, int num_sms, int* stat_blocks);
 int conv_f16x1_launch(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
                       int pre_relu, const void* w, const float* bias, const float* residual, const float* relu_mask,
-                      float* y, float out_scale, int B, int H, int W, int Cin, int Cout, int ksize, int num_sms,
-                      cudaStream_t stream);
+                      float* y, float out_scale, const float* in_scale, int B, int H, int W, int Cin, int Cout,
+                      int ksize, int num_sms, cudaStream_t stream, double* stat_part, const float* stat_pivot);
 
 // ---- conv_wgmma.cu : warpgroup-MMA weight-gradient GEMM (K = pixels) reading RAW x and dY; BN-apply + ReLU + tf32 split
 //      fused into the operand staging ----

@@ -35,30 +35,48 @@ def precision_passes():
 
 
 INFERENCE_PRECISIONS = ("fp32", "fp16")
+TRAINING_PRECISIONS = ("fp32", "fp16")
+
+
+def _set_precision(model, attr, precision, choices, what):
+    from .lib.models.hourglass import HourglassNet
+    from .lib.models.pose_hrnet import PoseHighResolutionNet
+    from .lib.models.pose_resnet import PoseResNet
+    if precision not in choices:
+        raise ValueError("%s precision must be one of %s, got %r" % (what, choices, precision))
+    net = model.module if isinstance(model, torch.nn.DataParallel) else model
+    if not isinstance(net, (HourglassNet, PoseHighResolutionNet, PoseResNet)):
+        raise TypeError("set_%s_precision takes an fpd_b200 hourglass / HRNet / ResNet network (or an "
+                        "nn.DataParallel around one), got %s" % (what, type(net).__name__))
+    eng = net.engine()
+    prev = getattr(eng, attr)
+    if precision != prev:
+        setattr(eng, attr, precision)
+        eng.invalidate_eval_cache()
+    return prev
 
 
 def set_inference_precision(model, precision):
     """Operand precision of `model`'s eval-mode forwards that record no tape (net(x) under no_grad, forward_nhwc,
     FlipTestInference, a frozen FPD teacher): "fp32" (the default: 3xFP16 / 3xTF32, fp32-grade) or "fp16" (single-pass
     FP16 on ops.conv2d_tc_f16x1 for every convolution it takes: about 2^-11 relative operand rounding, one MMA per
-    product instead of three). Training forwards and forwards that record a backward tape always run at fp32 grade.
+    product instead of three). Training forwards and forwards that record a backward tape follow
+    set_training_precision instead.
     `model`: an fpd_b200 hourglass / HRNet / ResNet network or an nn.DataParallel around one. Returns the previous
     setting; a change drops the cached eval operands and bumps the engine generation, so captured graphs capture again."""
-    from .lib.models.hourglass import HourglassNet
-    from .lib.models.pose_hrnet import PoseHighResolutionNet
-    from .lib.models.pose_resnet import PoseResNet
-    if precision not in INFERENCE_PRECISIONS:
-        raise ValueError("inference precision must be one of %s, got %r" % (INFERENCE_PRECISIONS, precision))
-    net = model.module if isinstance(model, torch.nn.DataParallel) else model
-    if not isinstance(net, (HourglassNet, PoseHighResolutionNet, PoseResNet)):
-        raise TypeError("set_inference_precision takes an fpd_b200 hourglass / HRNet / ResNet network (or an "
-                        "nn.DataParallel around one), got %s" % type(net).__name__)
-    eng = net.engine()
-    prev = eng.inference_precision
-    if precision != prev:
-        eng.inference_precision = precision
-        eng.invalidate_eval_cache()
-    return prev
+    return _set_precision(model, "inference_precision", precision, INFERENCE_PRECISIONS, "inference")
+
+
+def set_training_precision(model, precision):
+    """Operand precision of `model`'s forwards that run in train mode or record a backward tape, and of their backward:
+    "fp32" (the default: 3xFP16 / 3xTF32 convolutions, fp32-grade) or "fp16": single-pass FP16 forward convolutions
+    (ops.conv2d_tc_f16x1, BatchNorm statistics from the epilogue in fp64 as before), single-pass FP16 data gradients of
+    dY * S where the BatchNorm-backward pass or the bias gradient gives dY's power-of-two operand scale S (fp32-grade
+    elsewhere), and single-pass TF32 weight gradients. BatchNorm, losses and the optimizer stay fp32. Convolutions the
+    single-pass kernels do not take keep their fp32-grade kernel (and FPD_PRECISION).
+    `model`: an fpd_b200 hourglass / HRNet / ResNet network or an nn.DataParallel around one. Returns the previous
+    setting; a change bumps the engine generation, and FPDTrainStep captures its graph again."""
+    return _set_precision(model, "training_precision", precision, TRAINING_PRECISIONS, "training")
 
 
 class Var:
@@ -183,8 +201,9 @@ class PreparedWeights:
     inside the captured graph; frozen teacher: once, cached with the eval context):
     [tap][O][I] hi/lo (+ flipped/transposed for dgrad). Forward operands are __half pairs (3xFP16, csrc/conv_wgmma.cu)
     where ops.conv2d_tc_h takes the shape, fp32 containers holding tf32 values otherwise.
-    f16x1 (eval-mode forwards without a tape at inference precision "fp16"): a single __half array of w * 2^8 for every
-    convolution ops.conv2d_tc_f16x1 takes, marked F16X1 in place of use_h."""
+    f16x1 (eval-mode forwards without a tape at inference precision "fp16", training-mode and tape-recording forwards
+    at training precision "fp16"): a single __half array of w * 2^8 for every convolution ops.conv2d_tc_f16x1 takes,
+    marked F16X1 in place of use_h, in the forward and (given dY's operand scale) the data-gradient layout."""
 
     def __init__(self, passes, scale_without_bias=False, f16x1=False):
         self.split = passes == 3
@@ -213,7 +232,13 @@ class PreparedWeights:
             w2[:, :c.cin * c.k * c.k, 0, 0] = w.permute(0, 2, 3, 1).reshape(c.cout, -1)
             w, k, cin = w2, 1, kpad
         if self.f16x1 and ops.conv2d_tc_f16x1_kernel(1, H, W, cin, c.cout, k):
-            e = (ops.weight_prep_f16(w, for_dgrad=False, split=False)[0], None, F16X1)
+            if (also_dgrad and not kpad and ops.FUSED_REDUCE and (c.bias is not None or self.scale_without_bias)
+                    and c.tc_dgrad_at(H, W) and ops.conv2d_tc_f16x1_kernel(1, H, W, c.cout, c.cin, c.k)):
+                (hi, _), (dhi, _) = ops.weight_prep_f16_both(w, split=False)
+                self._dgrad[c.name] = (dhi, None, F16X1)
+            else:
+                hi = ops.weight_prep_f16(w, for_dgrad=False, split=False)[0]
+            e = (hi, None, F16X1)
         elif self.split and ops.CONV_F16 and ops.conv2d_tc_h_supported(cin, c.cout, k, H, W, True):
             if (also_dgrad and not kpad and ops.CONV_F16_DGRAD and ops.FUSED_REDUCE
                     and (c.bias is not None or self.scale_without_bias) and c.tc_dgrad_at(H, W) and ops.conv2d_tc_h_supported(c.cout, c.cin, c.k, H, W, True)):
@@ -234,7 +259,9 @@ class PreparedWeights:
         if e is not None and e[0].dtype == torch.float16 and not f16_ok:
             e = None   # prepared together with the forward form, but no operand scale for dY: use the 3xTF32 form
         if e is None:
-            if (f16_ok and self.split and ops.CONV_F16_DGRAD
+            if f16_ok and self.f16x1 and ops.conv2d_tc_f16x1_kernel(1, H, W, c.cout, c.cin, c.k):
+                e = (ops.weight_prep_f16(c.weight.detach(), for_dgrad=True, split=False)[0], None, F16X1)
+            elif (f16_ok and self.split and ops.CONV_F16_DGRAD
                     and ops.conv2d_tc_h_supported(c.cout, c.cin, c.k, H, W, True)):
                 hi, lo = ops.weight_prep_f16(c.weight.detach(), for_dgrad=True, split=True)
                 e = (hi, lo, True)
@@ -270,6 +297,7 @@ class Engine:
         self._eval_cache = None
         self._eval_cache_key = None
         self.inference_precision = "fp32"   # set_inference_precision
+        self.training_precision = "fp32"    # set_training_precision
         # True: the BatchNorm-backward apply pass always also reduces its output (sum + max |dx|): engines whose convolutions
         # have no bias (HRNet) get the 3xFP16 operand scale of dY from it -- without it their data gradients run on 3xTF32
         self.force_apply_sum = False
@@ -458,7 +486,7 @@ class Engine:
                         residual.add_grad(dy, owned=False)
                     if c.bias is not None:
                         ctx.pgrads[c.bias] = ops.channel_sum(dy)
-                    dw = ops.conv2d_wgrad_tc_fused(cols, dy, 1, passes=ctx.passes)      # [Cout, kpad, 1, 1]
+                    dw = ops.conv2d_wgrad_tc_fused(cols, dy, 1, passes=ctx.wgrad_passes)      # [Cout, kpad, 1, 1]
                     K = c.cin * c.k * c.k
                     ctx.pgrads[c.weight] = dw[:, :K, 0, 0].reshape(c.cout, c.k, c.k, c.cin).permute(0, 3, 1, 2).contiguous()
                     if need_dx:
@@ -472,15 +500,18 @@ class Engine:
             stat_sums = None
             if use_h and out_bn and ctx.training and ctx.sync is None:
                 Bn, Hn, Wn = x.data.shape[0], x.data.shape[1], x.data.shape[2]
-                nblk = ops.conv2d_tc_h_stats_blocks(Bn, Hn, Wn, c.cin, c.cout, c.k, w_hi.dtype == torch.float16)
+                if use_h == F16X1:
+                    nblk = ops.conv2d_tc_f16x1_stats_blocks(Bn, Hn, Wn, c.cin, c.cout, c.k)
+                else:
+                    nblk = ops.conv2d_tc_h_stats_blocks(Bn, Hn, Wn, c.cin, c.cout, c.k, w_hi.dtype == torch.float16)
                 if nblk > 0:
                     pivot = None
                     if out_bn is not True and self.bns[out_bn].mod.running_mean is not None:
                         pivot = self.bns[out_bn].mod.running_mean
                     stat_sums = (torch.empty((nblk, c.cout, 2), dtype=torch.float64, device=x.data.device), nblk, pivot)
             if stat_sums is not None:
-                y = ops.conv2d_tc_h(x.data, w_hi, w_lo, c.k, mean=mean, scale=scale, shift=shift, relu=relu, bias=bias,
-                                    residual=res, stats_part=stat_sums[0], stats_pivot=stat_sums[2])
+                y = _conv_fwd(use_h, x.data, w_hi, w_lo, c.k, mean=mean, scale=scale, shift=shift, relu=relu, bias=bias,
+                              residual=res, stats_part=stat_sums[0], stats_pivot=stat_sums[2])
             else:
                 # BN-apply + ReLU + operand split happen inside the conv kernel (no separate HBM pass)
                 y = _conv_fwd(use_h, x.data, w_hi, w_lo, c.k, mean=mean, scale=scale, shift=shift, relu=relu,
@@ -526,14 +557,15 @@ class Engine:
                     with torch.cuda.stream(ctx.wgrad_stream):
                         ctx.wgrad_stream.wait_event(ev)
                         ctx.pgrads[c.weight] = ops.conv2d_wgrad_tc_fused(x.data, dy, c.k, mean=mean, scale=scale,
-                                                                         shift=shift, relu=relu, passes=ctx.passes)
+                                                                         shift=shift, relu=relu,
+                                                                         passes=ctx.wgrad_passes)
                     ctx.keepalive.append(dy)     # dy must outlive the side-stream kernel (released after the join)
                 elif tc_wgrad:
                     ctx.pgrads[c.weight] = ops.conv2d_wgrad_tc_fused(x.data, dy, c.k, mean=mean, scale=scale, shift=shift,
-                                                                     relu=relu, passes=ctx.passes)
+                                                                     relu=relu, passes=ctx.wgrad_passes)
                 elif wgrad_chunks is not None:
                     ctx.pgrads[c.weight] = ops.conv2d_wgrad_tc_chunked(x.data, dy, c.k, wgrad_chunks, mean=mean, scale=scale,
-                                                                       shift=shift, relu=relu, passes=ctx.passes)
+                                                                       shift=shift, relu=relu, passes=ctx.wgrad_passes)
                 else:
                     a_full = (ops.affine_act(x.data, scale, shift, relu, mean=mean) if bn_name is not None
                               else x.data)
@@ -547,7 +579,9 @@ class Engine:
                 # ---- data gradient w.r.t. the conv input a = act(bn(x))
                 if tc_dgrad:
                     wd_hi, wd_lo, use_h = ctx.weights.dgrad(c, dy.shape[1], dy.shape[2], f16_ok=dy_scale is not None)
-                    if use_h:
+                    if use_h == F16X1:
+                        da = ops.conv2d_tc_f16x1(dy, wd_hi, c.k, in_scale=dy_scale)
+                    elif use_h:
                         da = ops.conv2d_tc_h(dy, wd_hi, wd_lo, c.k,
                                              in_scale=dy_scale if wd_hi.dtype == torch.float16 else None)
                     else:
@@ -771,14 +805,17 @@ class Engine:
         ctx.sync = self._sync_spec() if training else None
         ctx.passes = precision_passes()
         ctx.tape = [] if record_tape else None
+        # set_training_precision("fp16"): single-pass FP16 convolutions and single-pass TF32 weight gradients
+        f16_train = (training or record_tape) and self.training_precision == "fp16"
+        ctx.wgrad_passes = 1 if f16_train else ctx.passes
         if training:
-            ctx.weights = PreparedWeights(ctx.passes, self.force_apply_sum)
+            ctx.weights = PreparedWeights(ctx.passes, self.force_apply_sum, f16x1=f16_train)
             ctx.affine = None
             self.invalidate_eval_cache()      # this forward rewrites the running statistics on the device
         else:
             w, affine = self._eval_prepared()
             if record_tape:
-                w = PreparedWeights(ctx.passes, self.force_apply_sum)
+                w = PreparedWeights(ctx.passes, self.force_apply_sum, f16x1=f16_train)
             ctx.weights, ctx.affine = w, affine
         img = img_nchw if (img_nchw.is_contiguous() and img_nchw.dtype == torch.float32) else img_nchw.contiguous().float()
         outs = self.run_network(ctx, img)
@@ -822,6 +859,7 @@ class _Ctx:
         self._in_s1 = False
         self.sync = None
         self.passes = 3
+        self.wgrad_passes = 3
         self.tape = None
         self.weights = None
         self.affine = None

@@ -196,14 +196,15 @@ def weight_prep_f16(w_oihw, for_dgrad=False, split=True):
     return hi, lo
 
 
-def weight_prep_f16_both(w_oihw):
-    """-> ((fwd_hi, fwd_lo), (dgrad_hi, dgrad_lo)) in one launch."""
+def weight_prep_f16_both(w_oihw, split=True):
+    """-> ((fwd_hi, fwd_lo), (dgrad_hi, dgrad_lo)) in one launch; split=False: the lo halves are None (the single-pass
+    FP16 operands of conv2d_tc_f16x1)."""
     _chk(w_oihw, "w")
     O, I, k, _ = w_oihw.shape
     f_hi = torch.empty((k * k, O, I), dtype=torch.float16, device=w_oihw.device)
-    f_lo = torch.empty_like(f_hi)
+    f_lo = torch.empty_like(f_hi) if split else None
     d_hi = torch.empty((k * k, I, O), dtype=torch.float16, device=w_oihw.device)
-    d_lo = torch.empty_like(d_hi)
+    d_lo = torch.empty_like(d_hi) if split else None
     N.check(N.lib().fpd_weight_prep_f16_both(_p(w_oihw), _p(f_hi), _p(f_lo), _p(d_hi), _p(d_lo), O, I, k, _stream()),
             "weight_prep_f16_both")
     return (f_hi, f_lo), (d_hi, d_lo)
@@ -266,19 +267,46 @@ def conv2d_tc_f16x1_kernel(B, H, W, Cin, Cout, k):
     return F16X1_KERNELS[int(N.lib().fpd_conv2d_tc_f16x1_kernel(B, H, W, Cin, Cout, k))]
 
 
+def conv2d_tc_f16x1_train_plan(B, H, W, Cin, Cout, k, stats=False):
+    """-> (kernel, stat_blocks): the kernel conv2d_tc_f16x1 runs this shape on with (stats=True) or without epilogue
+    statistics, named as conv2d_tc_f16x1_kernel, and the number of partial blocks a statistics call writes (0 without
+    statistics or when the shape cannot carry them). Host only."""
+    nblk = ctypes.c_int(0)
+    kind = int(N.lib().fpd_conv2d_tc_f16x1_train_plan(B, H, W, Cin, Cout, k, int(bool(stats)), ctypes.byref(nblk)))
+    return F16X1_KERNELS[kind], int(nblk.value)
+
+
+def conv2d_tc_f16x1_stats_blocks(B, H, W, Cin, Cout, k):
+    """conv2d_tc_h_stats_blocks for conv2d_tc_f16x1(stats_part=...): 0 if the call should carry no statistics."""
+    if CONV_STATS == "0" or (CONV_STATS == "3x3" and k != 3):
+        return 0
+    return conv2d_tc_f16x1_train_plan(B, H, W, Cin, Cout, k, stats=True)[1]
+
+
 def conv2d_tc_f16x1(x, w, ksize, mean=None, scale=None, shift=None, relu=False, bias=None, residual=None,
-                    relu_mask=None, out=None, out_scale=1.0):
+                    relu_mask=None, out=None, out_scale=1.0, in_scale=None, stats_part=None, stats_pivot=None):
     """y = conv(relu?((x-mean)*scale+shift)) with single-pass FP16 operands: fp16_rn of the transformed activation times
     w = weight_prep_f16(w_oihw, split=False)[0], one MMA per product, fp32 accumulation (about 2^-11 relative operand
-    rounding: for inference, never for gradients)."""
+    rounding).
+    Training calls (set_training_precision "fp16"): in_scale, the device float[2] {S, 1/S} of channel_sum(want_amax=True),
+    makes the operand fp16_rn(x * S) and divides the output by S (data gradients: x = dY, S puts max |dY| into
+    [2^14, 2^15)); stats_part [conv2d_tc_f16x1_stats_blocks(...)][Cout][2] fp64 receives the output's per-channel sums
+    as conv2d_tc_h(stats_part=...) does."""
     B, H, W, Cin = x.shape
     Cout = w.shape[1]
     if w.dtype != torch.float16:
         raise ValueError("conv2d_tc_f16x1 takes the __half weights of weight_prep_f16(split=False), got %s" % w.dtype)
     y = out if out is not None else torch.empty((B, H, W, Cout), dtype=torch.float32, device=x.device)
-    N.check(N.lib().fpd_conv2d_tc_f16x1(_p(x), _p(mean), _p(scale), _p(shift), int(relu), _p(w), _p(bias), _p(residual),
-                                        _p(relu_mask), _p(y), float(out_scale), B, H, W, Cin, Cout, ksize, _stream()),
-            "conv2d_tc_f16x1")
+    if in_scale is None and stats_part is None:
+        N.check(N.lib().fpd_conv2d_tc_f16x1(_p(x), _p(mean), _p(scale), _p(shift), int(relu), _p(w), _p(bias),
+                                            _p(residual), _p(relu_mask), _p(y), float(out_scale), B, H, W, Cin, Cout,
+                                            ksize, _stream()), "conv2d_tc_f16x1")
+        return y
+    assert stats_part is None or stats_part.dtype == torch.float64
+    N.check(N.lib().fpd_conv2d_tc_f16x1_train(_p(x), _p(mean), _p(scale), _p(shift), int(relu), _p(w), _p(bias),
+                                              _p(residual), _p(relu_mask), _p(y), float(out_scale), _p(in_scale), B, H,
+                                              W, Cin, Cout, ksize, _p(stats_part), _p(stats_pivot), _stream()),
+            "conv2d_tc_f16x1_train")
     return y
 
 

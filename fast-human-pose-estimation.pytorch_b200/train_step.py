@@ -110,6 +110,7 @@ class FPDTrainStep:
         self._have_next = False
         self._static_shapes = None
         self._static_ptrs = None
+        self._student_prec = None
         self._teacher_gen = 0
         self._stage_x = self._copy_stream = self._stage_ev = self._stage_free = None   # next batch's images, prefetched
         self._staged_for = None
@@ -261,19 +262,22 @@ class FPDTrainStep:
         if self.use_graph:
             shapes = (tuple(x.shape), tuple(target.shape), tuple(tw.shape))
             t_gen = self.teacher.engine().generation if self.teacher is not None else 0
+            s_prec = self.student.engine().training_precision
             # fused-Adam mode owns the parameters' storage (FlatParams); otherwise the caller may give them new storage
             ptrs = None if self.fused_adam else self._student_ptrs()
             if self.graph is not None and (shapes != self._static_shapes or t_gen != self._teacher_gen
-                                           or ptrs != self._static_ptrs):
+                                           or ptrs != self._static_ptrs or s_prec != self._student_prec):
                 # a short last batch / a different resolution, teacher weights reloaded after capture (the graph holds
-                # pointers to the teacher's prepared weights), or a student parameter / buffer given new storage (the
-                # graph holds its old address): capture again instead of broadcasting or using stale data
+                # pointers to the teacher's prepared weights), a student parameter / buffer given new storage (the
+                # graph holds its old address), or another student training precision (the graph holds its kernels):
+                # capture again instead of broadcasting or using stale data
                 self.graph = None
             if self.graph is None:
                 xd, td, wd = (t.cuda(non_blocking=True).float().contiguous() for t in (x, target, tw))
                 self._capture(xd, td, wd)
                 self._static_shapes = shapes
                 self._static_ptrs = ptrs
+                self._student_prec = s_prec
                 self._teacher_gen = self.teacher.engine().generation if self.teacher is not None else 0
                 self._have_next = False
             if self.pipeline:

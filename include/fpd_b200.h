@@ -94,8 +94,21 @@ int fpd_conv2d_tc_f16x1(const float* x, const float* pre_mean, const float* pre_
                         int pre_relu, const void* w, const float* bias, const float* residual, const float* relu_mask,
                         float* y, float out_scale, int B, int H, int W, int Cin, int Cout, int ksize,
                         fpd_stream_t stream);
+/* The same single-pass FP16 convolution for training calls: in_scale (device float[2] {S, 1/S} or NULL) makes the
+ * operand fp16_rn(x * S) and the epilogue scale out_scale * 2^-8 / S (data gradients: x = dY, S its power-of-two
+ * operand scale); stat_part (device double[stat_blocks][Cout][2] or NULL) and stat_pivot as fpd_conv2d_tc_h_stats.
+ * fpd_conv2d_tc_f16x1_train_plan (host only, no device needed) returns the kernel a launch with (stats != 0) or
+ * without statistics runs on, coded as fpd_conv2d_tc_f16x1_kernel (0: unsupported, including statistics with
+ * Cout > 256), and writes to *stat_blocks (nullable) the number of partial blocks a statistics launch writes. */
+int fpd_conv2d_tc_f16x1_train_plan(int B, int H, int W, int Cin, int Cout, int ksize, int stats, int* stat_blocks);
+int fpd_conv2d_tc_f16x1_train(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
+                              int pre_relu, const void* w, const float* bias, const float* residual,
+                              const float* relu_mask, float* y, float out_scale, const float* in_scale, int B, int H,
+                              int W, int Cin, int Cout, int ksize, double* stat_part, const float* stat_pivot,
+                              fpd_stream_t stream);
 /* Forward ([tap][O][I]) and data-gradient ([taps-1-tap][I][O]) __half hi/lo forms of w * 2^8 from one read of the
- * weights: one launch per convolution and training step instead of two. */
+ * weights: one launch per convolution and training step instead of two. f_lo and d_lo may both be NULL (the
+ * single-pass FP16 forms). */
 int fpd_weight_prep_f16_both(const float* w_oihw, void* f_hi, void* f_lo, void* d_hi, void* d_lo, int O, int I, int k,
                              fpd_stream_t stream);
 /* OIHW fp32 -> __half hi/lo of w * 2^8 in the layouts of fpd_weight_prep (w_lo may be NULL); the 2^-8 is applied by

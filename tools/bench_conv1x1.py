@@ -7,9 +7,10 @@ than the 50 MB L2), with an L2 flush before every timed window; the two kernels'
 one: weights are read from L2) and the achieved share of 3.35 TB/s, with the card's name, power limit and SM clock.
 
 With --single-pass, the forward forms instead run on the 3-pass weight-resident kernel against the single-pass one
-(ops.conv2d_tc_f16x1, pw_conv_f16x1_kernel); the HBM share is then the single-pass kernel's.
+(ops.conv2d_tc_f16x1, pw_conv_f16x1_kernel); the HBM share is then the single-pass kernel's. --train adds the data
+gradients, single-pass with their power-of-two input scale as the training precision "fp16" runs them.
 
-    python tools/bench_conv1x1.py [--windows 7] [--per 8] [--single-pass]
+    python tools/bench_conv1x1.py [--windows 7] [--per 8] [--single-pass [--train]]
 """
 import argparse
 import os
@@ -89,6 +90,7 @@ def main():
     ap.add_argument("--batch", type=int, default=32)
     ap.add_argument("--hw", type=int, default=64)
     ap.add_argument("--single-pass", action="store_true")
+    ap.add_argument("--train", action="store_true")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "bench_conv1x1 measures on the GPU"
     import fpd_b200  # noqa: F401
@@ -105,7 +107,7 @@ def main():
     tot_pw = tot_st = 0.0
     try:
         for (Cin, Cout, form, n) in SHAPES:
-            if args.single_pass and form == "dgrad":
+            if args.single_pass and form == "dgrad" and not args.train:
                 continue
             launch, nbytes = setup(B, H, W, Cin, Cout, form, g)
             graphs = {}

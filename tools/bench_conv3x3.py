@@ -10,8 +10,10 @@ dense figure), with the card's name, power limit and SM clock.
 
 With --single-pass, each forward form also runs on ops.conv2d_tc_f16x1 (single-pass FP16, no epilogue statistics),
 the two alternating window by window, and the single-pass share of the fp16 peak counts 1 x the algorithmic FLOPs.
+With --train, the single-pass calls are the training precision "fp16" ones: the statistics forms keep their epilogue
+statistics and the data gradients run too, with their power-of-two input scale.
 
-    python tools/bench_conv3x3.py [--windows 7] [--per 8] [--single-pass]
+    python tools/bench_conv3x3.py [--windows 7] [--per 8] [--single-pass [--train]]
 """
 import argparse
 import collections
@@ -81,7 +83,7 @@ def step_shapes():
     return counts
 
 
-def setup(shape, g, single=False):
+def setup(shape, g, single=False, train=False):
     from fpd_b200 import ops
     B, H, W, Cin, Cout, form = shape
     xs = [torch.randn(B, H, W, Cin, device="cuda", generator=g) * (1e-3 if form.startswith("dgrad") else 1.0)
@@ -111,6 +113,10 @@ def setup(shape, g, single=False):
         return launch
     w1, _ = ops.weight_prep_f16(w, split=False)
     kw1 = {k: v for k, v in kw.items() if not k.startswith("stats")}
+    if train and "stats" in form:
+        nblk = ops.conv2d_tc_f16x1_train_plan(B, H, W, Cin, Cout, 3, stats=True)[1]
+        kw1["stats_part"] = torch.empty((nblk, Cout, 2), dtype=torch.float64, device="cuda")
+        kw1["stats_pivot"] = kw["stats_pivot"]
 
     def launch1(i):
         ops.conv2d_tc_f16x1(xs[i % 2], w1, 3, residual=res[i % 2] if res else None,
@@ -139,6 +145,7 @@ def main():
     ap.add_argument("--windows", type=int, default=7)
     ap.add_argument("--per", type=int, default=8)
     ap.add_argument("--single-pass", action="store_true")
+    ap.add_argument("--train", action="store_true")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "bench_conv3x3 measures on the GPU"
     import fpd_b200  # noqa: F401
@@ -194,9 +201,9 @@ def single_pass(shapes, args):
     tot3 = tot1 = 0.0
     for shape, n in sorted(shapes.items(), key=lambda kv: -kv[0][0] * kv[0][1] * kv[0][2] * kv[0][3] * kv[0][4] * kv[1]):
         B, H, W, Cin, Cout, form = shape
-        if form.startswith("dgrad"):
+        if form.startswith("dgrad") and not args.train:
             continue
-        launches = setup(shape, g, single=True)
+        launches = setup(shape, g, single=True, train=args.train)
         graphs = [capture(fn, args.per) for fn in launches]
         times = [[], []]
         for _ in range(args.windows):
@@ -212,8 +219,8 @@ def single_pass(shapes, args):
             flush=True)
         del graphs, launches
         torch.cuda.empty_cache()
-    print("3x3 forward convolutions of one hg_fpd step: 3-pass %.2f ms, single-pass %.2f ms" % (tot3 / 1000.0,
-                                                                                              tot1 / 1000.0))
+    print("3x3 %s convolutions of one hg_fpd step: 3-pass %.2f ms, single-pass %.2f ms" % (
+        "forward and data-gradient" if args.train else "forward", tot3 / 1000.0, tot1 / 1000.0))
     print("device: %s (name, power limit, SM clock, max SM clock)" % card())
 
 

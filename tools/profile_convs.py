@@ -8,8 +8,14 @@ aggregated per (kernel, shape). Each weight gradient is followed by one wgrad_re
 The side streams (teacher overlap, hourglass branch fork, weight-gradient stream) are switched off so that each family
 runs on one stream in call order; the kernels and their shapes are the same as in the overlapped step.
 
-    python tools/profile_convs.py      # writes profile_out/profile_convs.txt
+    python tools/profile_convs.py [--training-precision fp16]      # writes profile_out/profile_convs[_fp16].txt
+
+--training-precision fp16 profiles the student at engine.set_training_precision("fp16"): its forward and data-gradient
+convolutions then run on ops.conv2d_tc_f16x1 (conv_halo_f16x1_kernel, pw_conv_f16x1_kernel, or conv_wgmma_kernel
+single-pass) and its weight gradients single-pass; the "wgrad" share of the step decides whether a faster weight
+gradient is worth having.
 """
+import argparse
 import collections
 import os
 import re
@@ -20,7 +26,8 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-FAMILIES = {"conv": ("conv_wgmma_kernel", "conv_halo_kernel"), "wgrad": ("wgrad_halo_kernel", "wgrad_wgmma_kernel")}
+FAMILIES = {"conv": ("conv_wgmma_kernel", "conv_halo_kernel", "conv_halo_f16x1_kernel", "pw_conv_f16x1_kernel"),
+            "wgrad": ("wgrad_halo_kernel", "wgrad_wgmma_kernel")}
 
 
 def kernel_label(name):
@@ -30,6 +37,9 @@ def kernel_label(name):
 
 
 def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--training-precision", default="fp32", choices=("fp32", "fp16"))
+    args = ap.parse_args()
     for k in ("FPD_OVERLAP_TEACHER", "FPD_FORK_UP1", "FPD_WGRAD_STREAM"):
         os.environ[k] = "0"
     import fpd_b200  # noqa: F401
@@ -39,6 +49,7 @@ def main():
     from bench import cfg, synthetic_batch
     calls = collections.defaultdict(list)
     orig_h, orig_fused, orig_wgrad = ops.conv2d_tc_h, ops.conv2d_tc_fused, ops.conv2d_wgrad_tc_fused
+    orig_f16x1 = ops.conv2d_tc_f16x1
 
     def conv_h(x, w_hi, w_lo, k, **kw):
         tag = "dgrad" if kw.get("in_scale") is not None or kw.get("relu_mask") is not None else "fwd"
@@ -49,13 +60,21 @@ def main():
         calls["conv"].append((tuple(x.shape), w_hi.shape[1], k, "tf32", "fused"))
         return orig_fused(x, w_hi, w_lo, k, **kw)
 
+    def conv_f16x1(x, w, k, **kw):
+        tag = "dgrad" if kw.get("in_scale") is not None else "fwd"
+        calls["conv"].append((tuple(x.shape), w.shape[1], k, "f16x1", tag))
+        return orig_f16x1(x, w, k, **kw)
+
     def wgrad(x, dy, k, **kw):
-        calls["wgrad"].append((tuple(x.shape), dy.shape[-1], k, "tf32", "wgrad"))
+        calls["wgrad"].append((tuple(x.shape), dy.shape[-1], k, "tf32x%d" % kw.get("passes", 3), "wgrad"))
         return orig_wgrad(x, dy, k, **kw)
     ops.conv2d_tc_h, ops.conv2d_tc_fused, ops.conv2d_wgrad_tc_fused = conv_h, conv_fused, wgrad
+    ops.conv2d_tc_f16x1 = conv_f16x1
+    from fpd_b200.engine import set_training_precision
     torch.manual_seed(0)
     student = H.get_pose_net(cfg(128, 4), True).cuda()
     teacher = H.get_pose_net(cfg(256, 8), False).cuda()
+    set_training_precision(student, args.training_precision)
     step = FPDTrainStep(student, teacher, use_graph=False)
     x, t, w = (v.cuda() for v in synthetic_batch(32, 0))
     for _ in range(2):
@@ -69,8 +88,8 @@ def main():
     evs = sorted([e for e in prof.events() if e.device_type is not None and "cuda" in str(e.device_type).lower()],
                  key=lambda e: e.time_range.start)
     step_us = sum(e.time_range.end - e.time_range.start for e in evs)
-    out = ["one eager FPD step (side streams off), device %s: kernel time %.2f ms" % (
-        torch.cuda.get_device_name(0), step_us / 1000.0)]
+    out = ["one eager FPD step (side streams off), student training precision %s, device %s: kernel time %.2f ms" % (
+        args.training_precision, torch.cuda.get_device_name(0), step_us / 1000.0)]
     for fam, shapes in calls.items():
         ks = [e for e in evs if any(n in e.name for n in FAMILIES[fam])]
         assert len(ks) == len(shapes), (fam, len(ks), len(shapes))
@@ -99,7 +118,8 @@ def main():
                            v[1], 100 * v[1] / tot, v[0], v[1] / v[0], kname, tag, prec, B, Hh, Ww, Cin, Cout, k, gf,
                            gf / (v[1] / v[0]) * 1e3))
     text = "\n".join(out)
-    path = os.path.join(ROOT, "profile_out", "profile_convs.txt")
+    path = os.path.join(ROOT, "profile_out", "profile_convs%s.txt" % (
+        "" if args.training_precision == "fp32" else "_" + args.training_precision))
     os.makedirs(os.path.dirname(path), exist_ok=True)
     open(path, "w").write(text + "\n")
     print(text)
