@@ -14,9 +14,9 @@
 //   Split operands: acc += A_lo * B_hi + A_hi * B_lo + A_hi * B_hi (the lo * lo term is below fp32 rounding).
 //   Optional epilogue statistics: per output channel {sum (y - pivot), sum (y - pivot)^2} in fp64, per-warp shared
 //   accumulators merged in a fixed order (deterministic), one [Cout][2] block per CTA for bn_finalize_sums.
-//   3x3 with 3xFP16 operands (conv_halo_kernel, selected by conv_launch where it fits in shared memory): the same GEMM
+//   3x3 with 3xFP16 operands (conv_halo_kernel, where conv_plan finds it fits in shared memory): the same GEMM
 //   with the A operand of a tile loaded and transformed once into a halo in shared memory and fed from registers.
-//   Single-pass FP16 (conv_f16x1_launch): the halo and 1x1 weight-resident kernels with kSplit = false
+//   Single-pass FP16 (conv_f16x1_*): the halo and 1x1 weight-resident kernels with kSplit = false
 //   (conv_halo_f16x1_kernel, pw_conv_f16x1_kernel), one MMA per k16 straight into the accumulators. Inference calls,
 //   and the training precision "fp16": forward calls with epilogue statistics, data gradients with in_scale.
 //
@@ -768,10 +768,9 @@ __device__ __forceinline__ void pw_epilogue(const ConvParams& p, const float (&a
 // flushes one block at the end, merged in the fixed order of conv_stats_flush. The 3-pass kernel has no statistics.
 constexpr int kPwStages1 = 3;
 
-template <bool kSplit>
-size_t pw_smem_bytes(int ncb, int nt) {
-  return 1024 + (size_t)(kSplit ? kPwStages : kPwStages1) * (kSplit ? 2 : 1) * kATileBytes +
-         (size_t)ncb * (kSplit ? 2 : 1) * nt * 128;
+size_t pw_smem_bytes(bool split, int ncb, int nt) {
+  return 1024 + (size_t)(split ? kPwStages : kPwStages1) * (split ? 2 : 1) * kATileBytes +
+         (size_t)ncb * (split ? 2 : 1) * nt * 128;
 }
 
 template <int kN, bool kSplit>
@@ -920,11 +919,12 @@ int allow_smem(Kernel kernel, std::atomic<uint64_t>& done) {
   return FPD_OK;
 }
 
-template <bool kF16, int kN>
-int launch_n(const ConvParams& p, int grid, size_t smem, cudaStream_t stream) {
+// Launches kKernel, with its dynamic shared-memory limit raised first (once per device).
+template <auto kKernel, typename... Args>
+int launch(int grid, int threads, size_t smem, cudaStream_t stream, const Args&... args) {
   static std::atomic<uint64_t> done{0};
-  if (int rc = allow_smem(conv_wgmma_kernel<kF16, kN>, done)) return rc;
-  conv_wgmma_kernel<kF16, kN><<<grid, kThreads, smem, stream>>>(p);
+  if (int rc = allow_smem(kKernel, done)) return rc;
+  kKernel<<<grid, threads, smem, stream>>>(args...);
   FPD_LAUNCH_CHECK();
   return FPD_OK;
 }
@@ -984,92 +984,25 @@ int halo_weight_map(CUtensorMap* map, const void* w, const ConvParams& p) {
   return FPD_OK;
 }
 
-template <int kN, bool kSplit>
-int launch_halo_n(const ConvParams& p, const CUtensorMap& hi, const CUtensorMap& lo, int grid, size_t smem,
-                  cudaStream_t stream) {
-  static std::atomic<uint64_t> done{0};
-  if constexpr (kSplit) {
-    if (int rc = allow_smem(conv_halo_kernel<kN>, done)) return rc;
-    conv_halo_kernel<kN><<<grid, kThreads, smem, stream>>>(p, hi, lo);
-  } else {
-    if (int rc = allow_smem(conv_halo_f16x1_kernel<kN>, done)) return rc;
-    conv_halo_f16x1_kernel<kN><<<grid, kThreads, smem, stream>>>(p, hi);
+// f(std::integral_constant<int, kN>{}) for an output slice of nt columns: the kN of every forward-convolution kernel.
+template <typename F>
+int with_slice(int nt, F&& f) {
+  switch (nt) {
+    case 16: return f(std::integral_constant<int, 16>{});
+    case 32: return f(std::integral_constant<int, 32>{});
+    case 48: return f(std::integral_constant<int, 48>{});
+    case 64: return f(std::integral_constant<int, 64>{});
+    case 80: return f(std::integral_constant<int, 80>{});
+    case 96: return f(std::integral_constant<int, 96>{});
+    case 112: return f(std::integral_constant<int, 112>{});
+    case 128: return f(std::integral_constant<int, 128>{});
   }
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
-}
-
-template <bool kSplit>
-int launch_halo(const ConvParams& p, int grid, size_t smem, cudaStream_t stream) {
-  CUtensorMap hi, lo;
-  if (int rc = halo_weight_map(&hi, p.w_hi, p)) return rc;
-  if (kSplit) {
-    if (int rc = halo_weight_map(&lo, p.w_lo, p)) return rc;
-  } else {
-    lo = hi;
-  }
-  switch (p.nt) {
-    case 16: return launch_halo_n<16, kSplit>(p, hi, lo, grid, smem, stream);
-    case 32: return launch_halo_n<32, kSplit>(p, hi, lo, grid, smem, stream);
-    case 48: return launch_halo_n<48, kSplit>(p, hi, lo, grid, smem, stream);
-    case 64: return launch_halo_n<64, kSplit>(p, hi, lo, grid, smem, stream);
-    case 80: return launch_halo_n<80, kSplit>(p, hi, lo, grid, smem, stream);
-    case 96: return launch_halo_n<96, kSplit>(p, hi, lo, grid, smem, stream);
-    case 112: return launch_halo_n<112, kSplit>(p, hi, lo, grid, smem, stream);
-    case 128: return launch_halo_n<128, kSplit>(p, hi, lo, grid, smem, stream);
-  }
-  set_last_error("conv_halo: no kernel for a %d-column slice", p.nt);
-  return FPD_ERR_UNSUPPORTED;
-}
-
-template <int kN, bool kSplit>
-int launch_pw_n(const ConvParams& p, int grid, size_t smem, cudaStream_t stream) {
-  static std::atomic<uint64_t> done{0};
-  if constexpr (kSplit) {
-    if (int rc = allow_smem(pw_conv_wgmma_kernel<kN>, done)) return rc;
-    pw_conv_wgmma_kernel<kN><<<grid, kThreads, smem, stream>>>(p);
-  } else {
-    if (int rc = allow_smem(pw_conv_f16x1_kernel<kN>, done)) return rc;
-    pw_conv_f16x1_kernel<kN><<<grid, kThreads, smem, stream>>>(p);
-  }
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
-}
-
-template <bool kSplit>
-int launch_pw(const ConvParams& p, int grid, size_t smem, cudaStream_t stream) {
-  switch (p.nt) {
-    case 16: return launch_pw_n<16, kSplit>(p, grid, smem, stream);
-    case 32: return launch_pw_n<32, kSplit>(p, grid, smem, stream);
-    case 48: return launch_pw_n<48, kSplit>(p, grid, smem, stream);
-    case 64: return launch_pw_n<64, kSplit>(p, grid, smem, stream);
-    case 80: return launch_pw_n<80, kSplit>(p, grid, smem, stream);
-    case 96: return launch_pw_n<96, kSplit>(p, grid, smem, stream);
-    case 112: return launch_pw_n<112, kSplit>(p, grid, smem, stream);
-    case 128: return launch_pw_n<128, kSplit>(p, grid, smem, stream);
-  }
-  set_last_error("conv_pw: no kernel for a %d-column slice", p.nt);
+  set_last_error("conv_wgmma: no kernel for a %d-column slice", nt);
   return FPD_ERR_UNSUPPORTED;
 }
 
 std::atomic<int> g_conv1x1{1};
 std::atomic<int> g_conv_halo{1};
-
-template <bool kF16>
-int launch_f(const ConvParams& p, int grid, size_t smem, cudaStream_t stream) {
-  switch (p.nt) {
-    case 16: return launch_n<kF16, 16>(p, grid, smem, stream);
-    case 32: return launch_n<kF16, 32>(p, grid, smem, stream);
-    case 48: return launch_n<kF16, 48>(p, grid, smem, stream);
-    case 64: return launch_n<kF16, 64>(p, grid, smem, stream);
-    case 80: return launch_n<kF16, 80>(p, grid, smem, stream);
-    case 96: return launch_n<kF16, 96>(p, grid, smem, stream);
-    case 112: return launch_n<kF16, 112>(p, grid, smem, stream);
-    case 128: return launch_n<kF16, 128>(p, grid, smem, stream);
-  }
-  set_last_error("conv_wgmma: no kernel for a %d-column slice", p.nt);
-  return FPD_ERR_UNSUPPORTED;
-}
 
 // The shape part of a launch's parameters, staged-kernel layout (passes 3: hi and lo tiles per stage).
 ConvParams conv_shape_params(int B, int H, int W, int Cin, int Cout, int ksize, int f16, int passes) {
@@ -1086,78 +1019,106 @@ ConvParams conv_shape_params(int B, int H, int W, int Cin, int Cout, int ksize, 
   return p;
 }
 
+// The forward-convolution kernels, numbered as conv_f16x1_kernel reports them.
+enum ConvKernel { kConvNone = 0, kConvStaged = 1, kConvHalo = 2, kConvPw = 3 };
+
+struct ConvPlan {
+  int kernel;    // ConvKernel
+  int grid;      // persistent CTAs; a launch with statistics writes one partial block per CTA
+  size_t smem;
+};
+
+// Which kernel runs a forward convolution. p: conv_shape_params of the call (passes 3: hi and lo operands); the halo
+// kernel's ring goes into p. kConvNone only where the staged kernel's shared memory does not fit.
+//   3x3: the halo kernel (conv_halo_kernel, conv_halo_f16x1_kernel) wherever the halo (one copy per operand half), the
+//   statistics scratch and a ring of weight stages with two mbarriers each fit: 3, else 2 stages with hi and lo
+//   operands; 4, else 3 single-pass.
+//   1x1: the weight-resident kernel (pw_conv_wgmma_kernel, pw_conv_f16x1_kernel) wherever the slice's weights, the A
+//   stages and the statistics scratch fit; only the single-pass kernel carries statistics.
+//   Everything else: the staged conv_wgmma_kernel.
+// The halo and 1x1 kernels take the 3xFP16 calls (f16 with w_lo), under the set_conv_halo / set_conv1x1 toggles, and
+// the single-pass calls (conv_f16x1_*), regardless of the toggles. TF32 calls and conv_tc_h's fp16 calls without w_lo
+// stay on the staged kernel.
+ConvPlan conv_plan(ConvParams& p, bool f16, bool single_pass, bool stats, int num_sms) {
+  const bool split = p.passes == 3;
+  const bool fast = single_pass || (f16 && split);
+  const int copies = split ? 2 : 1;
+  const size_t stat_bytes = stats ? (size_t)8 * p.Cout * 2 * sizeof(double) : 0;
+  ConvPlan pl{kConvStaged, p.num_tiles < num_sms ? p.num_tiles : num_sms, 0};
+  if (fast && p.ksize == 3 && (single_pass || g_conv_halo.load(std::memory_order_relaxed))) {
+    const int max_stages = split ? 3 : 4;
+    ConvParams h = p;
+    h.halo_rows = kTileM + 2 * p.W + 3;
+    h.stage_bytes = copies * p.b_tile_bytes;
+    for (int stages = max_stages; stages >= max_stages - 1; --stages) {
+      h.halo_stages = stages;
+      pl.smem = 1024 + (size_t)stages * h.stage_bytes + (size_t)copies * h.ncb * h.halo_rows * 128 + stat_bytes +
+                (size_t)stages * 2 * 8;
+      if (pl.smem <= (size_t)kSmemLimit) {
+        p = h;
+        pl.kernel = kConvHalo;
+        return pl;
+      }
+    }
+  }
+  if (fast && p.ksize == 1 && (single_pass || (!stats && g_conv1x1.load(std::memory_order_relaxed)))) {
+    pl.smem = pw_smem_bytes(split, p.ncb, p.nt) + stat_bytes;
+    if (pl.smem <= (size_t)kSmemLimit) {
+      pl.kernel = kConvPw;
+      return pl;
+    }
+  }
+  pl.smem = 1024 + (size_t)kStages * p.stage_bytes + stat_bytes;
+  if (pl.smem > (size_t)kSmemLimit) pl.kernel = kConvNone;
+  return pl;
+}
+
+// Every forward convolution: checks the call, plans it and launches the planned kernel. w_lo == nullptr: hi operands
+// only; single_pass: a conv_f16x1_* call.
 int conv_launch(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift, int pre_relu,
-                const void* w_hi, const void* w_lo, int f16, const float* bias, const float* residual,
-                const float* relu_mask, float* y, float out_scale, const float* in_scale, int B, int H, int W, int Cin,
-                int Cout, int ksize, int num_sms, cudaStream_t stream, double* stat_part, const float* stat_pivot) {
+                const void* w_hi, const void* w_lo, int f16, bool single_pass, const float* bias,
+                const float* residual, const float* relu_mask, float* y, float out_scale, const float* in_scale, int B,
+                int H, int W, int Cin, int Cout, int ksize, int num_sms, cudaStream_t stream, double* stat_part,
+                const float* stat_pivot) {
   FPD_REQUIRE(x && w_hi && y, "conv_wgmma: null operand");
   FPD_REQUIRE((double)B * H * W * Cout < 4294967296.0, "conv_wgmma: output has 2^32 or more elements");
   FPD_REQUIRE((pre_scale == nullptr) == (pre_shift == nullptr), "conv_wgmma: pre_scale/pre_shift come in pairs");
   FPD_REQUIRE(pre_scale != nullptr || pre_mean == nullptr, "conv_wgmma: pre_mean needs pre_scale/pre_shift");
   FPD_REQUIRE(stat_part == nullptr || Cout <= kMaxStatCout, "conv_wgmma: statistics need Cout <= %d", kMaxStatCout);
   ConvParams p = conv_shape_params(B, H, W, Cin, Cout, ksize, f16, w_lo ? 3 : 1);
+  const ConvPlan pl = conv_plan(p, f16, single_pass, stat_part != nullptr, num_sms);
+  FPD_REQUIRE(pl.kernel != kConvNone, "conv_wgmma: shared memory plan %zu B too large", pl.smem);
   p.x = x; p.w_hi = w_hi; p.w_lo = w_lo;
   p.pre_mean = pre_mean; p.pre_scale = pre_scale; p.pre_shift = pre_shift; p.pre_relu = pre_relu;
   p.bias = bias; p.residual = residual; p.relu_mask = relu_mask; p.y = y;
   p.out_scale = f16 ? out_scale * (1.0f / (float)(1 << kF16WeightScaleLog2)) : out_scale;
   p.in_scale = in_scale;
   p.stat_part = stat_part; p.stat_pivot = stat_pivot;
-  const size_t stat_bytes = stat_part ? (size_t)8 * Cout * 2 * sizeof(double) : 0;
-  const int grid = p.num_tiles < num_sms ? p.num_tiles : num_sms;
-  if (f16 && p.passes == 3 && ksize == 3 && g_conv_halo.load(std::memory_order_relaxed)) {
-    // 3x3 3xFP16: the halo-resident kernel wherever the halo, the statistics scratch and a ring of three (else two)
-    // weight stages with their two mbarriers each fit
-    ConvParams h = p;
-    h.halo_rows = kTileM + 2 * W + 3;
-    h.stage_bytes = 2 * p.b_tile_bytes;
-    for (int stages = 3; stages >= 2; --stages) {
-      h.halo_stages = stages;
-      const size_t smem = 1024 + (size_t)stages * h.stage_bytes + 2 * (size_t)h.ncb * h.halo_rows * 128 + stat_bytes +
-                          (size_t)stages * 2 * 8;
-      if (smem <= (size_t)kSmemLimit) return launch_halo<true>(h, grid, smem, stream);
+  const bool split = p.passes == 3;
+  CUtensorMap hi, lo;
+  if (pl.kernel == kConvHalo) {
+    if (int rc = halo_weight_map(&hi, w_hi, p)) return rc;
+    if (split) {
+      if (int rc = halo_weight_map(&lo, w_lo, p)) return rc;
     }
   }
-  if (f16 && p.passes == 3 && ksize == 1 && stat_part == nullptr && g_conv1x1.load(std::memory_order_relaxed)) {
-    // 1x1 3xFP16: the weight-resident kernel wherever the slice's weights and two A stages fit
-    const size_t smem = pw_smem_bytes<true>(p.ncb, p.nt);
-    if (smem <= (size_t)kSmemLimit) return launch_pw<true>(p, grid, smem, stream);
-  }
-  const size_t smem = 1024 + (size_t)kStages * p.stage_bytes + stat_bytes;
-  FPD_REQUIRE(smem <= (size_t)kSmemLimit, "conv_wgmma: shared memory plan %zu B too large", smem);
-  return f16 ? launch_f<true>(p, grid, smem, stream) : launch_f<false>(p, grid, smem, stream);
+  return with_slice(p.nt, [&](auto n) {
+    constexpr int kN = decltype(n)::value;
+    if (pl.kernel == kConvHalo)
+      return split ? launch<conv_halo_kernel<kN>>(pl.grid, kThreads, pl.smem, stream, p, hi, lo)
+                   : launch<conv_halo_f16x1_kernel<kN>>(pl.grid, kThreads, pl.smem, stream, p, hi);
+    if (pl.kernel == kConvPw)
+      return split ? launch<pw_conv_wgmma_kernel<kN>>(pl.grid, kThreads, pl.smem, stream, p)
+                   : launch<pw_conv_f16x1_kernel<kN>>(pl.grid, kThreads, pl.smem, stream, p);
+    return f16 ? launch<conv_wgmma_kernel<true, kN>>(pl.grid, kThreads, pl.smem, stream, p)
+               : launch<conv_wgmma_kernel<false, kN>>(pl.grid, kThreads, pl.smem, stream, p);
+  });
 }
 
-// Single-pass FP16 (conv_f16x1_launch): which kernel takes the shape, from the shape alone. 0: unsupported (also:
-// statistics with Cout > kMaxStatCout); 2: 3x3 on conv_halo_f16x1_kernel where the hi-only halo, the statistics scratch
-// (`stats`) and a ring of four (else three) weight stages fit; 3: 1x1 on pw_conv_f16x1_kernel where the slice's hi
-// weights, three A stages and the statistics scratch fit; 1: everything else on the staged conv_wgmma_kernel<true, kN>
-// (w_lo == nullptr). Sets the kernel's ring and stage sizes in `p` and its shared memory.
-constexpr int kHalo1MaxStages = 4;
-
-int f16x1_plan(ConvParams& p, size_t& smem, bool stats) {
-  if (!conv_shape_ok(p.Cin, p.Cout, p.ksize, 1, kMaxCinH, 2048) || p.B < 1 || p.H < 1 || p.W < 1 ||
-      (double)p.B * p.H * p.W * p.Cout >= 4294967296.0 || (stats && p.Cout > kMaxStatCout))
-    return 0;
-  const size_t stat_bytes = stats ? (size_t)8 * p.Cout * 2 * sizeof(double) : 0;
-  if (p.ksize == 3) {
-    ConvParams h = p;
-    h.halo_rows = kTileM + 2 * p.W + 3;
-    h.stage_bytes = p.b_tile_bytes;
-    for (int stages = kHalo1MaxStages; stages >= 3; --stages) {
-      h.halo_stages = stages;
-      smem = 1024 + (size_t)stages * h.stage_bytes + (size_t)h.ncb * h.halo_rows * 128 + stat_bytes +
-             (size_t)stages * 2 * 8;
-      if (smem <= (size_t)kSmemLimit) {
-        p = h;
-        return 2;
-      }
-    }
-  } else {
-    smem = pw_smem_bytes<false>(p.ncb, p.nt) + stat_bytes;
-    if (smem <= (size_t)kSmemLimit) return 3;
-  }
-  smem = 1024 + (size_t)kStages * p.stage_bytes + stat_bytes;
-  return 1;
+// The single-pass FP16 calls' shapes (also: statistics need Cout <= kMaxStatCout).
+bool conv_f16x1_supported(int B, int H, int W, int Cin, int Cout, int ksize, bool stats) {
+  return conv_shape_ok(Cin, Cout, ksize, 1, kMaxCinH, 2048) && B >= 1 && H >= 1 && W >= 1 &&
+         (double)B * H * W * Cout < 4294967296.0 && (!stats || Cout <= kMaxStatCout);
 }
 
 // ================================================= weight gradient =================================================
@@ -1554,15 +1515,6 @@ WgradPlan wgrad_plan(int B, int H, int W, int Cin, int Cout, int ksize, int num_
   return pl;
 }
 
-template <int kN>
-int wgrad_launch_n(const WgradParams& p, int grid, size_t smem, cudaStream_t stream) {
-  static std::atomic<uint64_t> done{0};
-  if (int rc = allow_smem(wgrad_wgmma_kernel<kN>, done)) return rc;
-  wgrad_wgmma_kernel<kN><<<grid, kThreads, smem, stream>>>(p);
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
-}
-
 std::atomic<int> g_wgrad_halo{1};
 
 // wgrad_halo_kernel takes every 3x3 shape of wgrad_tc_supported, and the 1x1 shapes whose input channels fill whole
@@ -1573,15 +1525,6 @@ bool wgrad_halo_ok(int Cin, int Cout, int ksize) {
   if (!g_wgrad_halo.load(std::memory_order_relaxed)) return false;
   if (ksize == 3) return true;
   return Cin % 64 == 0 && (Cout == 32 || Cout == 64);
-}
-
-template <int kN, bool kSplit>
-int wgrad_halo_launch_n(const WgradParams& p, int grid, int threads, size_t smem, cudaStream_t stream) {
-  static std::atomic<uint64_t> done{0};
-  if (int rc = allow_smem(wgrad_halo_kernel<kN, kSplit>, done)) return rc;
-  wgrad_halo_kernel<kN, kSplit><<<grid, threads, smem, stream>>>(p);
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
 }
 
 // The tap-row kernel for a plan of wgrad_plan (the splits are the plan's; only the CTA decomposition differs).
@@ -1604,10 +1547,10 @@ int wgrad_halo_launch(WgradParams p, const WgradPlan& pl, cudaStream_t stream) {
   const size_t smem = 1024 + 2 * (size_t)p.h_stage_bytes;
   const int grid = pl.splits * p.h_rows * p.h_ci_tiles * p.h_co_tiles;
   if (p.passes == 3)
-    return n == 64 ? wgrad_halo_launch_n<64, true>(p, grid, threads, smem, stream)
-                   : wgrad_halo_launch_n<32, true>(p, grid, threads, smem, stream);
-  return n == 64 ? wgrad_halo_launch_n<64, false>(p, grid, threads, smem, stream)
-                 : wgrad_halo_launch_n<32, false>(p, grid, threads, smem, stream);
+    return n == 64 ? launch<wgrad_halo_kernel<64, true>>(grid, threads, smem, stream, p)
+                   : launch<wgrad_halo_kernel<32, true>>(grid, threads, smem, stream, p);
+  return n == 64 ? launch<wgrad_halo_kernel<64, false>>(grid, threads, smem, stream, p)
+                 : launch<wgrad_halo_kernel<32, false>>(grid, threads, smem, stream, p);
 }
 
 }  // namespace
@@ -1631,7 +1574,7 @@ int conv_tc_ts_launch(const float* x, const float* pre_mean, const float* pre_sc
                       int ksize, int num_sms, cudaStream_t stream) {
   FPD_REQUIRE(conv_tc_ts_supported(Cin, Cout, ksize), "conv_tc_ts: unsupported shape Cin=%d Cout=%d k=%d", Cin, Cout,
               ksize);
-  return conv_launch(x, pre_mean, pre_scale, pre_shift, pre_relu, w_hi, w_lo, 0, bias, residual, relu_mask, y,
+  return conv_launch(x, pre_mean, pre_scale, pre_shift, pre_relu, w_hi, w_lo, 0, false, bias, residual, relu_mask, y,
                      out_scale, nullptr, B, H, W, Cin, Cout, ksize, num_sms, stream, nullptr, nullptr);
 }
 
@@ -1645,8 +1588,9 @@ bool conv_tc_h_supported(int Cin, int Cout, int ksize, int H, int W, int f16) {
 
 int conv_tc_h_stats_grid(int B, int H, int W, int Cin, int Cout, int ksize, int f16, int num_sms) {
   if (!conv_tc_h_supported(Cin, Cout, ksize, H, W, f16) || Cout > kMaxStatCout) return 0;
-  const int tiles = conv_num_tiles(B, H, W, Cout);
-  return tiles < num_sms ? tiles : num_sms;
+  ConvParams p = conv_shape_params(B, H, W, Cin, Cout, ksize, f16, 3);   // the grid is the same with hi operands only
+  const ConvPlan pl = conv_plan(p, f16, false, true, num_sms);
+  return pl.kernel != kConvNone ? pl.grid : 0;
 }
 
 int conv_tc_h_launch(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
@@ -1656,44 +1600,28 @@ int conv_tc_h_launch(const float* x, const float* pre_mean, const float* pre_sca
                      double* stat_part, const float* stat_pivot) {
   FPD_REQUIRE(conv_tc_h_supported(Cin, Cout, ksize, H, W, f16),
               "conv_tc_h: unsupported shape Cin=%d Cout=%d k=%d H=%d W=%d f16=%d", Cin, Cout, ksize, H, W, f16);
-  return conv_launch(x, pre_mean, pre_scale, pre_shift, pre_relu, w_hi, w_lo, f16, bias, residual, relu_mask, y,
-                     out_scale, in_scale, B, H, W, Cin, Cout, ksize, num_sms, stream, stat_part, stat_pivot);
+  return conv_launch(x, pre_mean, pre_scale, pre_shift, pre_relu, w_hi, w_lo, f16, false, bias, residual, relu_mask,
+                     y, out_scale, in_scale, B, H, W, Cin, Cout, ksize, num_sms, stream, stat_part, stat_pivot);
 }
 
 int conv_f16x1_kernel(int B, int H, int W, int Cin, int Cout, int ksize, int stats, int num_sms, int* stat_blocks) {
   if (stat_blocks) *stat_blocks = 0;
-  if (!conv_shape_ok(Cin, Cout, ksize, 1, kMaxCinH, 2048)) return 0;
+  if (!conv_f16x1_supported(B, H, W, Cin, Cout, ksize, stats != 0)) return 0;
   ConvParams p = conv_shape_params(B, H, W, Cin, Cout, ksize, 1, 1);
-  size_t smem = 0;
-  const int kind = f16x1_plan(p, smem, stats != 0);
-  if (kind > 0 && stats && stat_blocks) *stat_blocks = p.num_tiles < num_sms ? p.num_tiles : num_sms;
-  return kind;
+  const ConvPlan pl = conv_plan(p, true, true, stats != 0, num_sms);
+  if (pl.kernel != kConvNone && stats && stat_blocks) *stat_blocks = pl.grid;
+  return pl.kernel;
 }
 
 int conv_f16x1_launch(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
                       int pre_relu, const void* w, const float* bias, const float* residual, const float* relu_mask,
                       float* y, float out_scale, const float* in_scale, int B, int H, int W, int Cin, int Cout,
                       int ksize, int num_sms, cudaStream_t stream, double* stat_part, const float* stat_pivot) {
-  FPD_REQUIRE(x && w && y, "conv_f16x1: null operand");
-  FPD_REQUIRE((pre_scale == nullptr) == (pre_shift == nullptr), "conv_f16x1: pre_scale/pre_shift come in pairs");
-  FPD_REQUIRE(pre_scale != nullptr || pre_mean == nullptr, "conv_f16x1: pre_mean needs pre_scale/pre_shift");
-  FPD_REQUIRE(conv_shape_ok(Cin, Cout, ksize, 1, kMaxCinH, 2048),
-              "conv_f16x1: unsupported shape Cin=%d Cout=%d k=%d H=%d W=%d", Cin, Cout, ksize, H, W);
-  FPD_REQUIRE(stat_part == nullptr || Cout <= kMaxStatCout, "conv_f16x1: statistics need Cout <= %d", kMaxStatCout);
-  ConvParams p = conv_shape_params(B, H, W, Cin, Cout, ksize, 1, 1);
-  size_t smem = 0;
-  const int kind = f16x1_plan(p, smem, stat_part != nullptr);
-  FPD_REQUIRE(kind > 0, "conv_f16x1: unsupported shape B=%d H=%d W=%d Cin=%d Cout=%d k=%d", B, H, W, Cin, Cout, ksize);
-  p.x = x; p.w_hi = w; p.w_lo = nullptr;
-  p.pre_mean = pre_mean; p.pre_scale = pre_scale; p.pre_shift = pre_shift; p.pre_relu = pre_relu;
-  p.bias = bias; p.residual = residual; p.relu_mask = relu_mask; p.y = y;
-  p.out_scale = out_scale * (1.0f / (float)(1 << kF16WeightScaleLog2));
-  p.in_scale = in_scale;
-  p.stat_part = stat_part; p.stat_pivot = stat_pivot;
-  const int grid = p.num_tiles < num_sms ? p.num_tiles : num_sms;
-  if (kind == 2) return launch_halo<false>(p, grid, smem, stream);
-  if (kind == 3) return launch_pw<false>(p, grid, smem, stream);
-  return launch_f<true>(p, grid, smem, stream);
+  FPD_REQUIRE(conv_f16x1_supported(B, H, W, Cin, Cout, ksize, stat_part != nullptr),
+              "conv_f16x1: unsupported shape B=%d H=%d W=%d Cin=%d Cout=%d k=%d (statistics: %d, Cout <= %d)", B, H,
+              W, Cin, Cout, ksize, stat_part != nullptr, kMaxStatCout);
+  return conv_launch(x, pre_mean, pre_scale, pre_shift, pre_relu, w, nullptr, 1, true, bias, residual, relu_mask, y,
+                     out_scale, in_scale, B, H, W, Cin, Cout, ksize, num_sms, stream, stat_part, stat_pivot);
 }
 
 // ---------------------------------------------- weight-gradient entry points ----------------------------------------------
@@ -1742,9 +1670,9 @@ int wgrad_tc_fused_launch(const float* x, const float* pre_mean, const float* pr
   const size_t smem = 1024 + (size_t)kStages * p.stage_bytes;
   const int grid = pl.splits * pl.taps * pl.co_tiles * pl.ci_tiles;
   int rc = wgrad_halo_ok(Cin, Cout, ksize) ? wgrad_halo_launch(p, pl, stream)
-         : pl.n == 32 ? wgrad_launch_n<32>(p, grid, smem, stream)
-         : pl.n == 64 ? wgrad_launch_n<64>(p, grid, smem, stream)
-                      : wgrad_launch_n<128>(p, grid, smem, stream);
+         : pl.n == 32 ? launch<wgrad_wgmma_kernel<32>>(grid, kThreads, smem, stream, p)
+         : pl.n == 64 ? launch<wgrad_wgmma_kernel<64>>(grid, kThreads, smem, stream, p)
+                      : launch<wgrad_wgmma_kernel<128>>(grid, kThreads, smem, stream, p);
   if (rc) return rc;
   const int64_t total = (int64_t)pl.taps * Cin * Cout;
   wgrad_reduce_kernel<<<(int)((total + 31) / 32), 256, 0, stream>>>(p.partial, dw_oihw, scale, Cin, Cout, pl.taps,

@@ -8,6 +8,7 @@ and the backward pass is an explicit tape of kernel launches instead of a per-op
 Python here only sequences launches and owns tensors (torch = device memory + streams); there is no
 torch math on the hot path and no CPU fallback.
 """
+import collections
 import os
 
 import torch
@@ -173,14 +174,6 @@ class ConvRef:
                 and ops.conv2d_tc_h_supported(self.cout, self.cin, self.k, H, W, False)))
 
     @property
-    def tc_fwd(self):
-        return self.s1 and self.pad == self.k // 2 and ops.conv2d_tc_supported(self.cin, self.cout, self.k)
-
-    @property
-    def tc_dgrad(self):
-        return self.s1 and self.pad == self.k // 2 and ops.conv2d_tc_supported(self.cout, self.cin, self.k)
-
-    @property
     def tc_wgrad(self):
         return self.s1 and self.pad == self.k // 2 and ops.conv2d_wgrad_tc_supported(self.cin, self.cout, self.k)
 
@@ -193,17 +186,33 @@ class BNRef:
         self.mod = mod
 
 
-F16X1 = "f16x1"   # PreparedWeights.fwd's kernel choice for single-pass FP16 weights (ops.conv2d_tc_f16x1)
+# the tensor-core convolution a PreparedWeights entry is prepared for: ops.conv2d_tc_f16x1 (single-pass FP16),
+# ops.conv2d_tc_h (3xFP16, or 3xTF32 / single-pass TF32 with fp32 containers) or ops.conv2d_tc_fused (TF32)
+TC_F16X1, TC_H, TC_TS = "f16x1", "h", "ts"
+TCWeights = collections.namedtuple("TCWeights", ("kernel", "hi", "lo"))
+
+
+def tc_operand_form(cin, cout, k, H, W, f16x1, split, dgrad=False, scaled=False):
+    """-> (kernel, fp16 weights, hi/lo split) of a tensor-core convolution from cin to cout channels at H x W (the data
+    gradient's: the convolution from Cout to Cin). Single-pass FP16 where f16x1 and ops.conv2d_tc_f16x1 takes the shape,
+    else 3xFP16 (ops.CONV_F16, for the data gradient ops.CONV_F16_DGRAD) where split and ops.conv2d_tc_h takes it, else
+    fp32 containers (split: 3xTF32). A data gradient takes the fp16 forms only when dY has an operand scale (scaled)."""
+    f16_ok = scaled or not dgrad
+    if f16_ok and f16x1 and ops.conv2d_tc_f16x1_kernel(1, H, W, cin, cout, k):
+        return TC_F16X1, True, False
+    if (f16_ok and split and (ops.CONV_F16_DGRAD if dgrad else ops.CONV_F16)
+            and ops.conv2d_tc_h_supported(cin, cout, k, H, W, True)):
+        return TC_H, True, True
+    return (TC_H if ops.conv2d_tc_h_supported(cin, cout, k, H, W, False) else TC_TS), False, split
 
 
 class PreparedWeights:
     """Tensor-core operand forms of the conv weights, prepared on first use within a forward (student: every step,
-    inside the captured graph; frozen teacher: once, cached with the eval context):
-    [tap][O][I] hi/lo (+ flipped/transposed for dgrad). Forward operands are __half pairs (3xFP16, csrc/conv_wgmma.cu)
-    where ops.conv2d_tc_h takes the shape, fp32 containers holding tf32 values otherwise.
-    f16x1 (eval-mode forwards without a tape at inference precision "fp16", training-mode and tape-recording forwards
-    at training precision "fp16"): a single __half array of w * 2^8 for every convolution ops.conv2d_tc_f16x1 takes,
-    marked F16X1 in place of use_h, in the forward and (given dY's operand scale) the data-gradient layout."""
+    inside the captured graph; frozen teacher: once, cached with the eval context): TCWeights(kernel, hi, lo) entries,
+    [tap][O][I] (flipped / transposed for the data gradient) in the form tc_operand_form picks. f16x1 (eval-mode
+    forwards without a tape at inference precision "fp16", training-mode and tape-recording forwards at training
+    precision "fp16"): single __half arrays of w * 2^8 for every convolution ops.conv2d_tc_f16x1 takes, in the forward
+    and (given dY's operand scale) the data-gradient layout."""
 
     def __init__(self, passes, scale_without_bias=False, f16x1=False):
         self.split = passes == 3
@@ -212,14 +221,13 @@ class PreparedWeights:
         self._dgrad = {}
         self.derived = {}      # name -> ConvRef with weights derived from another module's (Engine.deconv)
         # bias-free convolutions get the operand scale of dY from the BatchNorm-backward pass (Engine.force_apply_sum):
-        # their 3xFP16 data-gradient weights can then come out of the same launch as the forward ones
+        # their fp16 data-gradient weights can then come out of the same launch as the forward ones
         self.scale_without_bias = scale_without_bias
 
     def fwd(self, c, H, W, also_dgrad=False):
-        """-> (w_hi, w_lo, use_h): use_h selects ops.conv2d_tc_h (Cin up to 2048, 3xFP16) over ops.conv2d_tc_fused
-        (3xTF32, Cin up to 512).
-        also_dgrad: a backward pass will want the data-gradient form too -- when both are 3xFP16 they come out of one
-        launch (one read of the weights)."""
+        """-> the forward TCWeights of c at H x W.
+        also_dgrad: a backward pass will want the data-gradient form too -- when the backward will have dY's operand
+        scale and both forms are fp16 with the same split, they come out of one launch (one read of the weights)."""
         e = self._fwd.get(c.name)
         if e is not None:
             return e
@@ -231,52 +239,42 @@ class PreparedWeights:
             w2 = torch.zeros((c.cout, kpad, 1, 1), dtype=torch.float32, device=w.device)
             w2[:, :c.cin * c.k * c.k, 0, 0] = w.permute(0, 2, 3, 1).reshape(c.cout, -1)
             w, k, cin = w2, 1, kpad
-        if self.f16x1 and ops.conv2d_tc_f16x1_kernel(1, H, W, cin, c.cout, k):
-            if (also_dgrad and not kpad and ops.FUSED_REDUCE and (c.bias is not None or self.scale_without_bias)
-                    and c.tc_dgrad_at(H, W) and ops.conv2d_tc_f16x1_kernel(1, H, W, c.cout, c.cin, c.k)):
-                (hi, _), (dhi, _) = ops.weight_prep_f16_both(w, split=False)
-                self._dgrad[c.name] = (dhi, None, F16X1)
-            else:
-                hi = ops.weight_prep_f16(w, for_dgrad=False, split=False)[0]
-            e = (hi, None, F16X1)
-        elif self.split and ops.CONV_F16 and ops.conv2d_tc_h_supported(cin, c.cout, k, H, W, True):
-            if (also_dgrad and not kpad and ops.CONV_F16_DGRAD and ops.FUSED_REDUCE
-                    and (c.bias is not None or self.scale_without_bias) and c.tc_dgrad_at(H, W) and ops.conv2d_tc_h_supported(c.cout, c.cin, c.k, H, W, True)):
-                (hi, lo), (dhi, dlo) = ops.weight_prep_f16_both(w)
-                self._dgrad[c.name] = (dhi, dlo, True)
-            else:
-                hi, lo = ops.weight_prep_f16(w, for_dgrad=False, split=True)
-            e = (hi, lo, True)
+        kernel, f16, split = tc_operand_form(cin, c.cout, k, H, W, self.f16x1, self.split)
+        dform = None
+        # the backward has dY's operand scale where the bias gradient's pass or the BatchNorm-backward pass yields it
+        if (f16 and also_dgrad and not kpad and ops.FUSED_REDUCE and (c.bias is not None or self.scale_without_bias)
+                and c.tc_dgrad_at(H, W)):
+            dform = tc_operand_form(c.cout, c.cin, c.k, H, W, self.f16x1, self.split, dgrad=True, scaled=True)
+        if dform is not None and dform[1:] == (True, split):
+            (hi, lo), (dhi, dlo) = ops.weight_prep_f16_both(w, split=split)
+            self._dgrad[c.name] = TCWeights(dform[0], dhi, dlo)
         else:
-            hi, lo = ops.weight_prep(w, for_dgrad=False, split=self.split)
-            e = (hi, lo, ops.conv2d_tc_h_supported(cin, c.cout, k, H, W, False))
-        self._fwd[c.name] = e
+            hi, lo = (ops.weight_prep_f16 if f16 else ops.weight_prep)(w, for_dgrad=False, split=split)
+        e = self._fwd[c.name] = TCWeights(kernel, hi, lo)
         return e
 
-    def dgrad(self, c, H, W, f16_ok=False):
-        """f16_ok: the caller has the power-of-two operand scale of dY (ops.channel_sum(..., want_amax=True))."""
+    def dgrad(self, c, H, W, scaled=False):
+        """-> the data-gradient TCWeights of c at H x W. scaled: the caller has the power-of-two operand scale of dY
+        (ops.channel_sum(..., want_amax=True))."""
         e = self._dgrad.get(c.name)
-        if e is not None and e[0].dtype == torch.float16 and not f16_ok:
-            e = None   # prepared together with the forward form, but no operand scale for dY: use the 3xTF32 form
+        if e is not None and e.hi.dtype == torch.float16 and not scaled:
+            e = None   # prepared together with the forward form, but no operand scale for dY: use an fp32 form
         if e is None:
-            if f16_ok and self.f16x1 and ops.conv2d_tc_f16x1_kernel(1, H, W, c.cout, c.cin, c.k):
-                e = (ops.weight_prep_f16(c.weight.detach(), for_dgrad=True, split=False)[0], None, F16X1)
-            elif (f16_ok and self.split and ops.CONV_F16_DGRAD
-                    and ops.conv2d_tc_h_supported(c.cout, c.cin, c.k, H, W, True)):
-                hi, lo = ops.weight_prep_f16(c.weight.detach(), for_dgrad=True, split=True)
-                e = (hi, lo, True)
-            else:
-                hi, lo = ops.weight_prep(c.weight.detach(), for_dgrad=True, split=self.split)
-                e = (hi, lo, ops.conv2d_tc_h_supported(c.cout, c.cin, c.k, H, W, False))
-            self._dgrad[c.name] = e
+            kernel, f16, split = tc_operand_form(c.cout, c.cin, c.k, H, W, self.f16x1, self.split, dgrad=True,
+                                                 scaled=scaled)
+            hi, lo = (ops.weight_prep_f16 if f16 else ops.weight_prep)(c.weight.detach(), for_dgrad=True, split=split)
+            e = self._dgrad[c.name] = TCWeights(kernel, hi, lo)
         return e
 
 
-def _conv_fwd(use_h, x, w_hi, w_lo, k, **kw):
-    """The tensor-core forward convolution PreparedWeights.fwd prepared the weights for."""
-    if use_h == F16X1:
-        return ops.conv2d_tc_f16x1(x, w_hi, k, **kw)
-    return (ops.conv2d_tc_h if use_h else ops.conv2d_tc_fused)(x, w_hi, w_lo, k, **kw)
+def _tc_conv(e, x, k, in_scale=None, **kw):
+    """The tensor-core convolution of x with the prepared weights e. in_scale (dY's operand scale) goes to the kernels
+    that take it: single-pass FP16, and ops.conv2d_tc_h with fp16 weights."""
+    if e.kernel == TC_F16X1:
+        return ops.conv2d_tc_f16x1(x, e.hi, k, in_scale=in_scale, **kw)
+    if e.kernel == TC_H:
+        return ops.conv2d_tc_h(x, e.hi, e.lo, k, in_scale=in_scale if e.hi.dtype == torch.float16 else None, **kw)
+    return ops.conv2d_tc_fused(x, e.hi, e.lo, k, **kw)
 
 
 class Engine:
@@ -433,32 +431,23 @@ class Engine:
         out_bn: name of a train-mode BatchNorm that will consume y (True: some BatchNorm, name unknown) -- the conv then
         also emits y's per-channel sums from its epilogue (Var.stat_sums), pivoted on that module's running mean."""
         c = conv_name if isinstance(conv_name, ConvRef) else self.convs[conv_name]
-        if c.pick_first and not getattr(ctx, "_in_s1", False):
-            H_, W_ = x.data.shape[1], x.data.shape[2]
-            if (H_ % 2 == 0 and W_ % 2 == 0 and bn_name is None and residual is None and x.data.shape[-1] % 4 == 0
-                    and c.tc_fwd_at(H_ // 2, W_ // 2)):
-                xs = self.subsample2(ctx, x)
-                ctx._in_s1 = True
-                try:
-                    return self.conv(ctx, xs, c, None, relu, None, need_dx, out_bn=out_bn)
-                finally:
-                    ctx._in_s1 = False
-        if c.as_s1 and not getattr(ctx, "_in_s1", False):
-            H_, W_ = x.data.shape[1], x.data.shape[2]
-            if (H_ % 2 == 0 and W_ % 2 == 0 and c.cout % 4 == 0 and c.tc_fwd_at(H_, W_) and residual is None
-                    and not (bn_name is None and c.im2col_kpad)):
-                # stride 2 = stride-1 convolution on the tensor cores + even-position pick (recorded as two tape entries:
-                # the pick's backward scatters dY into a zero tensor, the stride-1 conv's backward is the ordinary one)
-                ctx._in_s1 = True
-                try:
-                    full = self.conv(ctx, x, c, bn_name, relu, residual, need_dx, out_bn=None)
-                finally:
-                    ctx._in_s1 = False
-                return self.subsample2(ctx, full)
-        wrapped = getattr(ctx, "_in_s1", False)        # called by one of the two stride-2 wrappers above
-        s1_ok = c.stride == 1 or wrapped
+        H, W = x.data.shape[1], x.data.shape[2]
+        if (c.pick_first and H % 2 == 0 and W % 2 == 0 and bn_name is None and residual is None
+                and x.data.shape[-1] % 4 == 0 and c.tc_fwd_at(H // 2, W // 2)):
+            return self._conv_at(ctx, self.subsample2(ctx, x), c, None, relu, None, need_dx, out_bn, stride=1)
+        if (c.as_s1 and H % 2 == 0 and W % 2 == 0 and c.cout % 4 == 0 and c.tc_fwd_at(H, W) and residual is None
+                and not (bn_name is None and c.im2col_kpad)):
+            # stride 2 = stride-1 convolution on the tensor cores + even-position pick (recorded as two tape entries:
+            # the pick's backward scatters dY into a zero tensor, the stride-1 conv's backward is the ordinary one)
+            full = self._conv_at(ctx, x, c, bn_name, relu, None, need_dx, None, stride=1, as_s1=True)
+            return self.subsample2(ctx, full)
+        return self._conv_at(ctx, x, c, bn_name, relu, residual, need_dx, out_bn, stride=c.stride)
+
+    def _conv_at(self, ctx, x, c, bn_name, relu, residual, need_dx, out_bn, stride, as_s1=False):
+        """Engine.conv at `stride`: 1 for the stride-2 convolutions that conv routes to the stride-1 kernels (pick_first:
+        x is already the picked tensor; as_s1: a stride-2 3x3 run at stride 1, its dY arrives zero-upsampled)."""
         Hx, Wx = x.data.shape[1], x.data.shape[2]
-        tc_fwd = c.tc_fwd_at(Hx, Wx) and s1_ok
+        tc_fwd = c.tc_fwd_at(Hx, Wx) and stride == 1
         scale = shift = mean = None
         aff = None
         if bn_name is not None:
@@ -475,8 +464,7 @@ class Engine:
                 cols = ops.im2col(x.data, c.k, c.stride, c.pad, kpad)
                 if ctx.shared_stem is not None and "cols_key" not in ctx.shared_stem:
                     ctx.shared_stem["cols_key"], ctx.shared_stem["cols"] = key, cols
-            w_hi, w_lo, use_h = ctx.weights.fwd(c, cols.shape[1], cols.shape[2])
-            out = Var(_conv_fwd(use_h, cols, w_hi, w_lo, 1, bias=bias, residual=res))
+            out = Var(_tc_conv(ctx.weights.fwd(c, cols.shape[1], cols.shape[2]), cols, 1, bias=bias, residual=res))
             if ctx.tape is not None:
                 def bwd_stem():
                     dy = out.grad
@@ -495,39 +483,30 @@ class Engine:
                 ctx.tape.append(bwd_stem)
             return out
         if tc_fwd:
-            w_hi, w_lo, use_h = ctx.weights.fwd(c, x.data.shape[1], x.data.shape[2],
-                                                also_dgrad=ctx.tape is not None and need_dx)
+            e = ctx.weights.fwd(c, Hx, Wx, also_dgrad=ctx.tape is not None and need_dx)
             stat_sums = None
-            if use_h and out_bn and ctx.training and ctx.sync is None:
-                Bn, Hn, Wn = x.data.shape[0], x.data.shape[1], x.data.shape[2]
-                if use_h == F16X1:
-                    nblk = ops.conv2d_tc_f16x1_stats_blocks(Bn, Hn, Wn, c.cin, c.cout, c.k)
-                else:
-                    nblk = ops.conv2d_tc_h_stats_blocks(Bn, Hn, Wn, c.cin, c.cout, c.k, w_hi.dtype == torch.float16)
+            if e.kernel != TC_TS and out_bn and ctx.training and ctx.sync is None:
+                nblk = ops.conv2d_tc_stats_blocks(x.data.shape[0], Hx, Wx, c.cin, c.cout, c.k,
+                                                  e.hi.dtype == torch.float16, single_pass=e.kernel == TC_F16X1)
                 if nblk > 0:
                     pivot = None
                     if out_bn is not True and self.bns[out_bn].mod.running_mean is not None:
                         pivot = self.bns[out_bn].mod.running_mean
                     stat_sums = (torch.empty((nblk, c.cout, 2), dtype=torch.float64, device=x.data.device), nblk, pivot)
-            if stat_sums is not None:
-                y = _conv_fwd(use_h, x.data, w_hi, w_lo, c.k, mean=mean, scale=scale, shift=shift, relu=relu, bias=bias,
-                              residual=res, stats_part=stat_sums[0], stats_pivot=stat_sums[2])
-            else:
-                # BN-apply + ReLU + operand split happen inside the conv kernel (no separate HBM pass)
-                y = _conv_fwd(use_h, x.data, w_hi, w_lo, c.k, mean=mean, scale=scale, shift=shift, relu=relu,
-                              bias=bias, residual=res)
+            stats = {} if stat_sums is None else dict(stats_part=stat_sums[0], stats_pivot=stat_sums[2])
+            # BN-apply + ReLU + operand split happen inside the conv kernel (no separate HBM pass)
+            y = _tc_conv(e, x.data, c.k, mean=mean, scale=scale, shift=shift, relu=relu, bias=bias, residual=res,
+                         **stats)
         else:
             a = ops.affine_act(x.data, scale, shift, relu, mean=mean) if bn_name is not None else x.data
             y = ops.conv2d_simt_fwd(a, c.weight.detach(), bias=bias, residual=res, stride=c.stride, pad=c.pad)
         out = Var(y)
         if tc_fwd:
             out.stat_sums = stat_sums
-        tc_wgrad = c.tc_wgrad and s1_ok
-        tc_dgrad = c.tc_dgrad_at(Hx, Wx) and s1_ok
-        in_s1 = c.as_s1 and wrapped          # stride-2 3x3 running as stride 1 + pick: dY arrives zero-upsampled
-        stride_eff = 1 if wrapped else c.stride   # (pick-first 1x1: x is already the picked tensor, a true stride-1 conv)
+        tc_wgrad = c.tc_wgrad and stride == 1
+        tc_dgrad = c.tc_dgrad_at(Hx, Wx) and stride == 1
         wgrad_chunks = None                  # too wide for one tensor-core wgrad launch: one launch per channel chunk
-        if (ctx.tape is not None and not tc_wgrad and s1_ok and c.pad == c.k // 2
+        if (ctx.tape is not None and not tc_wgrad and stride == 1 and c.pad == c.k // 2
                 and (bn_name is not None or not c.im2col_kpad)):
             wgrad_chunks = ops.wgrad_channel_chunks(c.cin, c.cout, c.k)
         if ctx.tape is not None:
@@ -571,23 +550,17 @@ class Engine:
                               else x.data)
                     # CUDA-core fallback; for a stride-2 conv in stride-1 mode go back to the compact dY (the even
                     # positions of the zero-upsampled one) and the true stride: a quarter of the work
-                    dy_w = ops.subsample2(dy) if in_s1 else dy
-                    ctx.pgrads[c.weight] = ops.conv2d_simt_wgrad(a_full, dy_w, c.k, stride=c.stride if (in_s1 or not wrapped) else 1,
+                    dy_w = ops.subsample2(dy) if as_s1 else dy
+                    ctx.pgrads[c.weight] = ops.conv2d_simt_wgrad(a_full, dy_w, c.k, stride=c.stride if as_s1 else stride,
                                                                  pad=c.pad)
                 if not need_dx:
                     return
                 # ---- data gradient w.r.t. the conv input a = act(bn(x))
                 if tc_dgrad:
-                    wd_hi, wd_lo, use_h = ctx.weights.dgrad(c, dy.shape[1], dy.shape[2], f16_ok=dy_scale is not None)
-                    if use_h == F16X1:
-                        da = ops.conv2d_tc_f16x1(dy, wd_hi, c.k, in_scale=dy_scale)
-                    elif use_h:
-                        da = ops.conv2d_tc_h(dy, wd_hi, wd_lo, c.k,
-                                             in_scale=dy_scale if wd_hi.dtype == torch.float16 else None)
-                    else:
-                        da = ops.conv2d_tc_fused(dy, wd_hi, wd_lo, c.k)
+                    wd = ctx.weights.dgrad(c, dy.shape[1], dy.shape[2], scaled=dy_scale is not None)
+                    da = _tc_conv(wd, dy, c.k, in_scale=dy_scale)
                 else:
-                    da = ops.conv2d_simt_dgrad(dy, c.weight.detach(), x.data.shape[1:3], stride=stride_eff, pad=c.pad)
+                    da = ops.conv2d_simt_dgrad(dy, c.weight.detach(), x.data.shape[1:3], stride=stride, pad=c.pad)
                 if bn_name is not None:
                     self._bn_backward(ctx, x, bn_name, relu, da, aff)
                 else:
@@ -856,7 +829,6 @@ class Engine:
 class _Ctx:
     def __init__(self):
         self.training = False
-        self._in_s1 = False
         self.sync = None
         self.passes = 3
         self.wgrad_passes = 3

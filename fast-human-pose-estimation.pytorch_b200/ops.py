@@ -63,7 +63,7 @@ def _counter(device):
 FUSED_REDUCE = os.environ.get("FPD_FUSED_REDUCE", "1") != "0"   # single-launch reductions (A/B switch)
 
 
-def conv2d_tc_supported(cin, cout, k, fused=True):
+def conv2d_tc_supported(cin, cout, k):
     """Does a tensor-core convolution kernel take these channel counts (the TS kernel takes Cout > 256 in slices)?"""
     return bool(N.lib().fpd_conv2d_tc_ts_supported(cin, cout, k))
 
@@ -217,11 +217,19 @@ def weight_prep_f16_both(w_oihw, split=True):
 CONV_STATS = os.environ.get("FPD_CONV_STATS", "3x3").lower()
 
 
-def conv2d_tc_h_stats_blocks(B, H, W, Cin, Cout, k, f16):
-    """Number of per-CTA partial blocks conv2d_tc_h(..., stats_part=) writes; 0 if the shape cannot carry statistics."""
+def conv2d_tc_stats_blocks(B, H, W, Cin, Cout, k, f16, single_pass=False):
+    """Number of per-CTA partial blocks the statistics call (stats_part=) of conv2d_tc_h (f16: fp16 weights) or, with
+    single_pass, conv2d_tc_f16x1 writes; 0 if the call should carry no statistics (CONV_STATS) or the shape cannot."""
     if CONV_STATS == "0" or (CONV_STATS == "3x3" and k != 3):
         return 0
+    if single_pass:
+        return conv2d_tc_f16x1_train_plan(B, H, W, Cin, Cout, k, stats=True)[1]
     return int(N.lib().fpd_conv2d_tc_h_stats_blocks(B, H, W, Cin, Cout, k, int(f16)))
+
+
+def conv2d_tc_h_stats_blocks(B, H, W, Cin, Cout, k, f16):
+    """Number of per-CTA partial blocks conv2d_tc_h(..., stats_part=) writes; 0 if the shape cannot carry statistics."""
+    return conv2d_tc_stats_blocks(B, H, W, Cin, Cout, k, f16)
 
 
 def bn_finalize_sums(part, nblocks, pivot, P, gamma, beta, eps, running_mean=None, running_var=None, momentum=0.1):
@@ -278,9 +286,7 @@ def conv2d_tc_f16x1_train_plan(B, H, W, Cin, Cout, k, stats=False):
 
 def conv2d_tc_f16x1_stats_blocks(B, H, W, Cin, Cout, k):
     """conv2d_tc_h_stats_blocks for conv2d_tc_f16x1(stats_part=...): 0 if the call should carry no statistics."""
-    if CONV_STATS == "0" or (CONV_STATS == "3x3" and k != 3):
-        return 0
-    return conv2d_tc_f16x1_train_plan(B, H, W, Cin, Cout, k, stats=True)[1]
+    return conv2d_tc_stats_blocks(B, H, W, Cin, Cout, k, True, single_pass=True)
 
 
 def conv2d_tc_f16x1(x, w, ksize, mean=None, scale=None, shift=None, relu=False, bias=None, residual=None,
