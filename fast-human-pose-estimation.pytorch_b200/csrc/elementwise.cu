@@ -312,12 +312,14 @@ bn_sums_finalize_kernel(const double* __restrict__ part, int nblocks, const floa
 // -------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void write_amax_scale(float m, float* amax_scale) {
   // power-of-two scale that puts max|v| into [2^14, 2^15): fp16 hi/lo operands of v * S then keep every element to within
-  // 2^-39 of the largest one (csrc/conv_wgmma.cu in_scale). Zero / non-finite maxima -> no scaling.
+  // 2^-39 of the largest one (csrc/conv_wgmma.cu in_scale). Zero, non-finite and >= 3e38 maxima -> no scaling. S is at most 2^126,
+  // so that S and 1/S are both normal floats: maxima below 2^-112 (which would need S >= 2^127, and below 2^-113 an
+  // infinite S) get S = 2^126 and land below 2^14, still exact powers of two apart from v.
   float S = 1.f;
   if (m > 0.f && m < 3.0e38f) {
     int e;
-    frexpf(m, &e);            // m = f * 2^e, f in [0.5, 1)
-    S = ldexpf(1.f, 15 - e);  // m * S in [2^14, 2^15)
+    frexpf(m, &e);                              // m = f * 2^e, f in [0.5, 1)
+    S = ldexpf(1.f, min(15 - e, 126));          // m * S in [2^14, 2^15) for m >= 2^-112
   }
   amax_scale[0] = S;
   amax_scale[1] = 1.f / S;

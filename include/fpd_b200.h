@@ -134,7 +134,8 @@ int fpd_bn_finalize_sums(const double* part, int nblocks, const float* pivot, in
 /* Leaner forms of fpd_channel_sum / fpd_bn_bwd_reduce / (fpd_bn_stats + fpd_bn_finalize): the BatchNorm statistics'
  * second stage and the module's finalize (affine + running statistics) run as one kernel (division-free fp64 merge), and
  * the channel sum can also return the operand scale of the 3xFP16 gradient convolutions: amax_scale (nullable float[2])
- * receives {S, 1/S} with S the power of two that puts max|dy| into [2^14, 2^15). `counter` is reserved (a single-launch
+ * receives {S, 1/S} with S the power of two that puts max|dy| into [2^14, 2^15), at most 2^126 (maxima below 2^-112 stay
+ * below 2^14; zero, non-finite and >= 3e38 maxima give S = 1; NaN elements are ignored). `counter` is reserved (a single-launch
  * "last block finishes" variant measured slower and is disabled); pass a zeroed unsigned int or NULL.
  * Workspace sizes: fpd_channel_reduce_workspace_bytes / fpd_bn_stats_workspace_bytes.
  * Replace the per-channel sums of Conv2d bias backward, BatchNorm2d backward and BatchNorm2d train-mode forward
