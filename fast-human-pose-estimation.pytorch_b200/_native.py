@@ -35,6 +35,8 @@ _SIGNATURES = {
     "fpd_conv2d_tc_f16x1_train_plan": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_int)]),
     "fpd_conv2d_tc_f16x1_train": (c_int, [P, P, P, P, c_int, P, P, P, P, P, c_float, P, c_int, c_int, c_int, c_int, c_int,
                                           c_int, P, P, P]),
+    "fpd_conv2d_tc_f16x1_io": (c_int, [P, c_int, P, P, P, c_int, P, P, P, P, c_int, c_float, c_int, c_int, c_int, c_int,
+                                       c_int, c_int, P]),
     "fpd_set_conv1x1": (c_int, [c_int]),
     "fpd_set_conv_halo": (c_int, [c_int]),
     "fpd_set_wgrad_halo": (c_int, [c_int]),
@@ -83,6 +85,13 @@ _SIGNATURES = {
     "fpd_deconv_weight_map": (c_int, [P, P, c_int, c_int, c_int, c_int, c_int, P]),
     "fpd_subsample2": (c_int, [P, P, c_int, c_int, c_int, c_int, P]),
     "fpd_upsample_zero2": (c_int, [P, P, c_int, c_int, c_int, c_int, P]),
+    "fpd_affine_act_f16": (c_int, [P, P, P, P, c_int, P, c_int64, c_int, P]),
+    "fpd_affine_add_act_f16": (c_int, [P, P, P, P, P, c_int, P, c_int64, c_int, P]),
+    "fpd_fuse_sum_f16": (c_int, [POINTER(c_void_p), POINTER(c_int), c_int, c_int, P, c_int, c_int, c_int, c_int, P]),
+    "fpd_maxpool2x2_fwd_f16": (c_int, [P, P, c_int, c_int, c_int, c_int, P]),
+    "fpd_upsample2x_add_f16": (c_int, [P, P, P, c_int, c_int, c_int, c_int, P]),
+    "fpd_subsample2_f16": (c_int, [P, P, c_int, c_int, c_int, c_int, P]),
+    "fpd_half_to_float": (c_int, [P, P, c_int64, P]),
     "fpd_nchw_to_nhwc": (c_int, [P, P, c_int, c_int, c_int, c_int, P]),
     "fpd_nchw_to_nhwc_flipw": (c_int, [P, P, c_int, c_int, c_int, c_int, P]),
     "fpd_nhwc_to_nchw": (c_int, [P, P, c_int, c_int, c_int, c_int, P]),

@@ -73,6 +73,14 @@ int fpd_conv2d_tc_f16x1(const float* x, const float* pre_mean, const float* pre_
                            nullptr, B, H, W, Cin, Cout, ksize, device_sm_count(), S(stream), nullptr, nullptr);
 }
 
+int fpd_conv2d_tc_f16x1_io(const void* x, int x_f16, const float* pre_mean, const float* pre_scale,
+                           const float* pre_shift, int pre_relu, const void* w, const float* bias, const void* residual,
+                           void* y, int y_f16, float out_scale, int B, int H, int W, int Cin, int Cout, int ksize,
+                           fpd_stream_t stream) {
+  return conv_f16x1_io_launch(x, x_f16, pre_mean, pre_scale, pre_shift, pre_relu, w, bias, residual, y, y_f16,
+                              out_scale, B, H, W, Cin, Cout, ksize, device_sm_count(), S(stream));
+}
+
 int fpd_conv2d_tc_f16x1_train_plan(int B, int H, int W, int Cin, int Cout, int ksize, int stats, int* stat_blocks) {
   return conv_f16x1_kernel(B, H, W, Cin, Cout, ksize, stats, device_sm_count(), stat_blocks);
 }
@@ -269,6 +277,33 @@ int fpd_subsample2(const float* x, float* y, int B, int H, int W, int C, fpd_str
 }
 int fpd_upsample_zero2(const float* dy, float* dx, int B, int Ho, int Wo, int C, fpd_stream_t stream) {
   return upsample_zero2(dy, dx, B, Ho, Wo, C, S(stream));
+}
+int fpd_affine_act_f16(const void* x, const float* mean, const float* scale, const float* shift, int relu, void* y,
+                       int64_t P, int C, fpd_stream_t stream) {
+  return affine_act_f16(x, mean, scale, shift, nullptr, relu, y, P, C, S(stream));
+}
+int fpd_affine_add_act_f16(const void* x, const float* mean, const float* scale, const float* shift,
+                           const void* residual, int relu, void* y, int64_t P, int C, fpd_stream_t stream) {
+  FPD_REQUIRE(residual, "fpd_affine_add_act_f16: NULL residual");
+  return affine_act_f16(x, mean, scale, shift, residual, relu, y, P, C, S(stream));
+}
+int fpd_fuse_sum_f16(const void* const* terms_host, const int* shifts_host, int n, int relu, void* out, int B, int H,
+                     int W, int C, fpd_stream_t stream) {
+  FPD_REQUIRE(terms_host && shifts_host, "fpd_fuse_sum_f16: NULL term table");
+  return fuse_sum_f16(terms_host, shifts_host, n, relu, out, B, H, W, C, S(stream));
+}
+int fpd_maxpool2x2_fwd_f16(const void* x, void* y, int B, int H, int W, int C, fpd_stream_t stream) {
+  return maxpool2x2_fwd_f16(x, y, B, H, W, C, S(stream));
+}
+int fpd_upsample2x_add_f16(const void* up1, const void* low, void* out, int B, int H, int W, int C,
+                           fpd_stream_t stream) {
+  return upsample2x_add_f16(up1, low, out, B, H, W, C, S(stream));
+}
+int fpd_subsample2_f16(const void* x, void* y, int B, int H, int W, int C, fpd_stream_t stream) {
+  return subsample2_f16(x, y, B, H, W, C, S(stream));
+}
+int fpd_half_to_float(const void* x, float* y, int64_t n, fpd_stream_t stream) {
+  return half_to_float(x, y, n, S(stream));
 }
 int fpd_nchw_to_nhwc(const float* x, float* y, int B, int C, int H, int W, fpd_stream_t stream) {
   return nchw_to_nhwc(x, y, B, C, H, W, S(stream));

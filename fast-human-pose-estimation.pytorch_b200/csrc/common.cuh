@@ -1,9 +1,11 @@
 // common.cuh -- error plumbing and small device helpers shared by every kernel in libfpd_b200 (built for sm_90a:
 //   -gencode arch=compute_90a,code=sm_90a)
 #pragma once
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <cstdio>
+#include <type_traits>
 
 namespace fpd {
 
@@ -70,6 +72,54 @@ __device__ __forceinline__ void split_tf32_fast(float x, float& hi, float& lo) {
   hi = __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
   const float r = x - hi;
   lo = __uint_as_float((__float_as_uint(r) + 0x1000u) & 0xFFFFE000u);
+}
+
+// ---- fp16 activation storage (inference precision "fp16_act"): kernels compute in fp32 from float(x) and store
+// fp16_rn of the result saturated to +-65504, so NaN stays NaN and no finite value becomes infinite.
+__device__ __forceinline__ float sat_f16(float v) { return fabsf(v) > 65504.f ? copysignf(65504.f, v) : v; }
+__device__ __forceinline__ uint32_t f16x2_sat_bits(float a, float b) {
+  const __half2 h = __floats2half2_rn(sat_f16(a), sat_f16(b));
+  return *reinterpret_cast<const uint32_t*>(&h);
+}
+__device__ __forceinline__ float2 f16x2_bits_to_float2(uint32_t u) {
+  return __half22float2(*reinterpret_cast<const __half2*>(&u));
+}
+
+// Four consecutive activations (element offset 4 i) of an fp32 or fp16 tensor, as fp32 / stored from fp32.
+template <typename T>
+__device__ __forceinline__ float4 ld_act4(const T* p, int64_t i) {
+  if constexpr (std::is_same<T, float>::value) {
+    return __ldg(reinterpret_cast<const float4*>(p) + i);
+  } else {
+    const uint2 u = __ldg(reinterpret_cast<const uint2*>(p) + i);
+    const float2 a = f16x2_bits_to_float2(u.x), b = f16x2_bits_to_float2(u.y);
+    return make_float4(a.x, a.y, b.x, b.y);
+  }
+}
+template <typename T>
+__device__ __forceinline__ void st_act4(T* p, int64_t i, float4 v) {
+  if constexpr (std::is_same<T, float>::value) {
+    reinterpret_cast<float4*>(p)[i] = v;
+  } else {
+    reinterpret_cast<uint2*>(p)[i] = make_uint2(f16x2_sat_bits(v.x, v.y), f16x2_sat_bits(v.z, v.w));
+  }
+}
+// Two consecutive activations at element offset `off` (even).
+template <typename T>
+__device__ __forceinline__ float2 ld_act2(const T* p, size_t off) {
+  if constexpr (std::is_same<T, float>::value) {
+    return __ldg(reinterpret_cast<const float2*>(p + off));
+  } else {
+    return f16x2_bits_to_float2(__ldg(reinterpret_cast<const unsigned int*>(p + off)));
+  }
+}
+template <typename T>
+__device__ __forceinline__ void st_act2(T* p, size_t off, float2 v) {
+  if constexpr (std::is_same<T, float>::value) {
+    *reinterpret_cast<float2*>(p + off) = v;
+  } else {
+    *reinterpret_cast<uint32_t*>(p + off) = f16x2_sat_bits(v.x, v.y);
+  }
 }
 
 __device__ __forceinline__ float warp_sum(float v) {

@@ -18,7 +18,9 @@
 //   with the A operand of a tile loaded and transformed once into a halo in shared memory and fed from registers.
 //   Single-pass FP16 (conv_f16x1_*): the halo and 1x1 weight-resident kernels with kSplit = false
 //   (conv_halo_f16x1_kernel, pw_conv_f16x1_kernel), one MMA per k16 straight into the accumulators. Inference calls,
-//   and the training precision "fp16": forward calls with epilogue statistics, data gradients with in_scale.
+//   and the training precision "fp16": forward calls with epilogue statistics, data gradients with in_scale. Their
+//   TIn / TOut template parameters (float or __half) are the activation types of x and of y with the residual: the
+//   inference precision "fp16_act" (conv_f16x1_io_launch) stores activations in fp16.
 //
 // Weight gradient (wgrad_tc_*):
 //   dW[co][ci][tap] = scale * sum_{pixels p} dY[p][co] * A[p (+) tap][ci],  A = relu?((x - mean) * scale + shift)
@@ -88,6 +90,32 @@ __device__ __forceinline__ float4 affine_relu4(float4 v, const float* mean, cons
     v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
   }
   return v;
+}
+
+// Raw load of the 8 activations at element offset `off` of x (fp32 or fp16 NHWC): fp32 into v[0], v[1]; fp16 as its
+// 16 bytes in v[0], kept as bits until cvt_raw8 widens them (so the load stays in flight like the fp32 one).
+template <typename TIn>
+__device__ __forceinline__ void ld_raw8(const float* x, size_t off, float4 (&v)[2]) {
+  if constexpr (std::is_same<TIn, float>::value) {
+    const float4* src = reinterpret_cast<const float4*>(x + off);
+    v[0] = __ldg(src);
+    v[1] = __ldg(src + 1);
+  } else {
+    const uint4 h = __ldg(reinterpret_cast<const uint4*>(reinterpret_cast<const __half*>(x) + off));
+    v[0] = make_float4(__uint_as_float(h.x), __uint_as_float(h.y), __uint_as_float(h.z), __uint_as_float(h.w));
+  }
+}
+template <typename TIn>
+__device__ __forceinline__ void cvt_raw8(const float4 (&v)[2], float4& a0, float4& a1) {
+  if constexpr (std::is_same<TIn, float>::value) {
+    a0 = v[0];
+    a1 = v[1];
+  } else {
+    const float2 p0 = f16x2_bits_to_float2(__float_as_uint(v[0].x)), p1 = f16x2_bits_to_float2(__float_as_uint(v[0].y));
+    const float2 p2 = f16x2_bits_to_float2(__float_as_uint(v[0].z)), p3 = f16x2_bits_to_float2(__float_as_uint(v[0].w));
+    a0 = make_float4(p0.x, p0.y, p1.x, p1.y);
+    a1 = make_float4(p2.x, p2.y, p3.x, p3.y);
+  }
 }
 
 __device__ __forceinline__ void split_tf32x4(float4 v, float4& h, float4& l) {
@@ -160,7 +188,7 @@ struct ConvParams {
   const float* pre_shift;
   int pre_relu;
   const float* bias;
-  const float* residual;
+  const float* residual;       // x, residual and y point to __half where the kernel's TIn / TOut is __half
   const float* relu_mask;
   float* y;
   float out_scale;
@@ -201,8 +229,9 @@ __device__ __forceinline__ void conv_stats_init(const ConvParams& p, double* s_s
 }
 
 // Epilogue of one 128 x kN tile: y = acc * oscale (+ bias) (+ residual) (ReLU mask), and the per-warp fp64 statistics.
-// Fragment row g (+8), columns 8 i + 2 t (+1) of this warp's 16 rows.
-template <int kN>
+// Fragment row g (+8), columns 8 i + 2 t (+1) of this warp's 16 rows. TOut: the type of y and the residual (__half:
+// the same fp32 expression from float(residual), stored as a saturated fp16_rn).
+template <int kN, typename TOut = float>
 __device__ __forceinline__ void conv_epilogue(const ConvParams& p, const float (&acc)[kN / 2], int m0, int n0,
                                               float oscale, double* s_stat) {
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
@@ -224,14 +253,14 @@ __device__ __forceinline__ void conv_epilogue(const ConvParams& p, const float (
       const size_t off = (size_t)m * p.Cout + col;
       float2 o = make_float2(acc[4 * i + 2 * rr] * oscale + b2.x, acc[4 * i + 2 * rr + 1] * oscale + b2.y);
       if (p.residual) {
-        const float2 r2 = __ldg(reinterpret_cast<const float2*>(p.residual + off));
+        const float2 r2 = ld_act2(reinterpret_cast<const TOut*>(p.residual), off);
         o.x += r2.x; o.y += r2.y;
       }
       if (p.relu_mask) {
         const float2 k = __ldg(reinterpret_cast<const float2*>(p.relu_mask + off));
         o.x = k.x > 0.f ? o.x : 0.f; o.y = k.y > 0.f ? o.y : 0.f;
       }
-      *reinterpret_cast<float2*>(p.y + off) = o;
+      st_act2(reinterpret_cast<TOut*>(p.y), off, o);
       if (stats) {
         const double d0 = (double)(o.x - pv.x), d1 = (double)(o.y - pv.y);
         s1a += d0; s2a += d0 * d0; s1b += d1; s2b += d1 * d1;
@@ -466,9 +495,13 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
 // ends with wgmma_wait<1>, so step s + 1 issues while step s is still in the tensor core; that wait retires step s - 1,
 // whose stage the warp releases then. The producer therefore fills step s + S - 2 into the stage of step s - 2 (both
 // warpgroups released it during step s - 1, before warpgroup 0's turn for step s), and the ring has S >= 3 stages.
-template <int kN, bool kSplit>
+//   Half-precision activations (TIn / TOut = __half, single-pass only): the halo fill reads 16 bytes per 8 channels
+// instead of 32 and applies the same fp32 transform to float(x); the epilogue is conv_epilogue<kN, TOut>.
+template <int kN, bool kSplit, typename TIn = float, typename TOut = float>
 __device__ __forceinline__ void conv_halo_body(const ConvParams& p, const CUtensorMap& w_hi_map,
                                                const CUtensorMap& w_lo_map) {
+  static_assert(!kSplit || (std::is_same<TIn, float>::value && std::is_same<TOut, float>::value),
+                "half-precision activations only on the single-pass kernel");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int R = p.halo_rows;
@@ -534,11 +567,7 @@ __device__ __forceinline__ void conv_halo_body(const ConvParams& p, const CUtens
         const int r = rc / p.ncb, cb = rc - r * p.ncb;
         const int q = hs + r, c = cb * 64 + jj * 8;
         v[u][0] = v[u][1] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (idx < items && q >= 0 && q < p.P && c < p.Cin) {
-          const float4* src = reinterpret_cast<const float4*>(p.x + (size_t)q * p.Cin + c);
-          v[u][0] = __ldg(src);
-          v[u][1] = __ldg(src + 1);
-        }
+        if (idx < items && q >= 0 && q < p.P && c < p.Cin) ld_raw8<TIn>(p.x, (size_t)q * p.Cin + c, v[u]);
       }
 #pragma unroll
       for (int u = 0; u < kHaloBatch; ++u) {
@@ -549,8 +578,10 @@ __device__ __forceinline__ void conv_halo_body(const ConvParams& p, const CUtens
         const int q = hs + r, c = cb * 64 + jj * 8;
         uint4 oh = make_uint4(0u, 0u, 0u, 0u), ol = make_uint4(0u, 0u, 0u, 0u);
         if (q >= 0 && q < p.P && c < p.Cin) {
-          float4 a0 = affine_relu4(v[u][0], p.pre_mean, p.pre_scale, p.pre_shift, c, p.pre_relu);
-          float4 a1 = affine_relu4(v[u][1], p.pre_mean, p.pre_scale, p.pre_shift, c + 4, p.pre_relu);
+          float4 a0, a1;
+          cvt_raw8<TIn>(v[u], a0, a1);
+          a0 = affine_relu4(a0, p.pre_mean, p.pre_scale, p.pre_shift, c, p.pre_relu);
+          a1 = affine_relu4(a1, p.pre_mean, p.pre_scale, p.pre_shift, c + 4, p.pre_relu);
           a0.x *= in_s; a0.y *= in_s; a0.z *= in_s; a0.w *= in_s;
           a1.x *= in_s; a1.y *= in_s; a1.z *= in_s; a1.w *= in_s;
           split_f16x2(a0.x, a0.y, oh.x, ol.x);
@@ -617,7 +648,7 @@ __device__ __forceinline__ void conv_halo_body(const ConvParams& p, const CUtens
       wgmma_wait<0>();
       if (lane == 0) mbar_arrive(empty + 8u * ((s - 1u) % S));
       __syncthreads();   // every warpgroup is done with the halo: the next tile may refill it
-      conv_epilogue<kN>(p, acc, m0, n0, oscale, s_stat);
+      conv_epilogue<kN, TOut>(p, acc, m0, n0, oscale, s_stat);
       continue;
     }
     float part[kN / 2];
@@ -685,10 +716,10 @@ __global__ void __launch_bounds__(kThreads, 1)
   conv_halo_body<kN, true>(p, w_hi_map, w_lo_map);
 }
 
-template <int kN>
+template <int kN, typename TIn = float, typename TOut = float>
 __global__ void __launch_bounds__(kThreads, 1)
     conv_halo_f16x1_kernel(const __grid_constant__ ConvParams p, const __grid_constant__ CUtensorMap w_map) {
-  conv_halo_body<kN, false>(p, w_map, w_map);
+  conv_halo_body<kN, false, TIn, TOut>(p, w_map, w_map);
 }
 
 // ============================================ forward, 1x1 resident weights ============================================
@@ -714,7 +745,7 @@ __device__ __forceinline__ void prefetch_l2(const void* src, uint32_t bytes) {
   asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"(bytes) : "memory");
 }
 
-template <int kN>
+template <int kN, typename TOut = float>
 __device__ __forceinline__ void pw_epilogue(const ConvParams& p, const float (&acc)[kN / 2], int m0, int n0,
                                             float oscale) {
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
@@ -731,7 +762,7 @@ __device__ __forceinline__ void pw_epilogue(const ConvParams& p, const float (&a
         r2[u][rr] = k2[u][rr] = make_float2(0.f, 0.f);
         if (i0 + u >= kN / 8 || m >= p.P) continue;
         const size_t off = (size_t)m * p.Cout + n0 + (i0 + u) * 8 + 2 * t;
-        if (p.residual) r2[u][rr] = __ldg(reinterpret_cast<const float2*>(p.residual + off));
+        if (p.residual) r2[u][rr] = ld_act2(reinterpret_cast<const TOut*>(p.residual), off);
         if (p.relu_mask) k2[u][rr] = __ldg(reinterpret_cast<const float2*>(p.relu_mask + off));
       }
     }
@@ -753,7 +784,7 @@ __device__ __forceinline__ void pw_epilogue(const ConvParams& p, const float (&a
         if (p.relu_mask) {
           o.x = k2[u][rr].x > 0.f ? o.x : 0.f; o.y = k2[u][rr].y > 0.f ? o.y : 0.f;
         }
-        *reinterpret_cast<float2*>(p.y + (size_t)m * p.Cout + col) = o;
+        st_act2(reinterpret_cast<TOut*>(p.y), (size_t)m * p.Cout + col, o);
       }
     }
   }
@@ -766,6 +797,8 @@ __device__ __forceinline__ void pw_epilogue(const ConvParams& p, const float (&a
 //   Optional epilogue statistics (training calls): the [8 warps][Cout][2] fp64 accumulators follow the resident
 // weights; tiles with statistics take conv_epilogue (same outputs as pw_epilogue, plus the per-warp sums) and the CTA
 // flushes one block at the end, merged in the fixed order of conv_stats_flush. The 3-pass kernel has no statistics.
+//   Half-precision activations (TIn / TOut = __half, single-pass only): the A staging loads 16 bytes per row and K step
+// instead of 32 and transforms float(x) as before; the epilogue is pw_epilogue<kN, TOut>.
 constexpr int kPwStages1 = 3;
 
 size_t pw_smem_bytes(bool split, int ncb, int nt) {
@@ -773,8 +806,10 @@ size_t pw_smem_bytes(bool split, int ncb, int nt) {
          (size_t)ncb * (split ? 2 : 1) * nt * 128;
 }
 
-template <int kN, bool kSplit>
+template <int kN, bool kSplit, typename TIn = float, typename TOut = float>
 __device__ __forceinline__ void pw_conv_body(const ConvParams& p) {
+  static_assert(!kSplit || (std::is_same<TIn, float>::value && std::is_same<TOut, float>::value),
+                "half-precision activations only on the single-pass kernel");
   constexpr uint32_t kAStage = (kSplit ? 2u : 1u) * kATileBytes;   // A hi, then A lo
   constexpr uint32_t kNumStages = kSplit ? kPwStages : kPwStages1;
   extern __shared__ uint8_t smem_raw[];
@@ -801,9 +836,7 @@ __device__ __forceinline__ void pw_conv_body(const ConvParams& p) {
       ra[i][0] = ra[i][1] = make_float4(0.f, 0.f, 0.f, 0.f);
       if (m < p.P && c < p.Cin) {
         okm |= 1u << i;
-        const float4* src = reinterpret_cast<const float4*>(p.x + (size_t)m * p.Cin + c);
-        ra[i][0] = __ldg(src);
-        ra[i][1] = __ldg(src + 1);
+        ld_raw8<TIn>(p.x, (size_t)m * p.Cin + c, ra[i]);
       }
     }
   };
@@ -816,9 +849,10 @@ __device__ __forceinline__ void pw_conv_body(const ConvParams& p) {
       uint4 oh = make_uint4(0u, 0u, 0u, 0u), ol = make_uint4(0u, 0u, 0u, 0u);
       if (okm & (1u << i)) {
         float4 v[2];
+        cvt_raw8<TIn>(ra[i], v[0], v[1]);
 #pragma unroll
         for (int u = 0; u < 2; ++u) {
-          v[u] = affine_relu4(ra[i][u], p.pre_mean, p.pre_scale, p.pre_shift, c + 4 * u, p.pre_relu);
+          v[u] = affine_relu4(v[u], p.pre_mean, p.pre_scale, p.pre_shift, c + 4 * u, p.pre_relu);
           v[u].x *= in_s; v[u].y *= in_s; v[u].z *= in_s; v[u].w *= in_s;
         }
         split_f16x2(v[0].x, v[0].y, oh.x, ol.x);
@@ -845,7 +879,8 @@ __device__ __forceinline__ void pw_conv_body(const ConvParams& p) {
     if (tid < kTileM) {   // the epilogue inputs of this tile: row m0 + tid, columns [n0, n0 + nt)
       const int m = m0 + tid;
       const size_t off = (size_t)m * p.Cout + n0;
-      if (m < p.P && p.residual) prefetch_l2(p.residual + off, (uint32_t)p.nt * 4u);
+      if (m < p.P && p.residual)
+        prefetch_l2(reinterpret_cast<const TOut*>(p.residual) + off, (uint32_t)p.nt * (uint32_t)sizeof(TOut));
       if (m < p.P && p.relu_mask) prefetch_l2(p.relu_mask + off, (uint32_t)p.nt * 4u);
     }
     float acc[kN / 2], part[kN / 2];
@@ -876,11 +911,11 @@ __device__ __forceinline__ void pw_conv_body(const ConvParams& p) {
     if (kSplit) add_part(acc, part);
     if constexpr (!kSplit) {
       if (p.stat_part) {
-        conv_epilogue<kN>(p, acc, m0, n0, oscale, s_stat);
+        conv_epilogue<kN, TOut>(p, acc, m0, n0, oscale, s_stat);
         continue;
       }
     }
-    pw_epilogue<kN>(p, acc, m0, n0, oscale);
+    pw_epilogue<kN, TOut>(p, acc, m0, n0, oscale);
   }
   if constexpr (!kSplit) conv_stats_flush(p, s_stat);
 }
@@ -890,9 +925,9 @@ __global__ void __launch_bounds__(kThreads, 1) pw_conv_wgmma_kernel(const __grid
   pw_conv_body<kN, true>(p);
 }
 
-template <int kN>
+template <int kN, typename TIn = float, typename TOut = float>
 __global__ void __launch_bounds__(kThreads, 1) pw_conv_f16x1_kernel(const __grid_constant__ ConvParams p) {
-  pw_conv_body<kN, false>(p);
+  pw_conv_body<kN, false, TIn, TOut>(p);
 }
 
 bool conv_shape_ok(int Cin, int Cout, int ksize, int f16, int max_cin, int max_cout) {
@@ -1073,13 +1108,26 @@ ConvPlan conv_plan(ConvParams& p, bool f16, bool single_pass, bool stats, int nu
   return pl;
 }
 
+template <typename T>
+struct TypeTag {
+  using type = T;
+};
+
+// f(TypeTag<TIn>{}, TypeTag<TOut>{}) for the activation types of a single-pass call (__half where the flag is set).
+template <typename F>
+int with_act_types(bool x_f16, bool y_f16, F&& f) {
+  if (x_f16) return y_f16 ? f(TypeTag<__half>{}, TypeTag<__half>{}) : f(TypeTag<__half>{}, TypeTag<float>{});
+  return y_f16 ? f(TypeTag<float>{}, TypeTag<__half>{}) : f(TypeTag<float>{}, TypeTag<float>{});
+}
+
 // Every forward convolution: checks the call, plans it and launches the planned kernel. w_lo == nullptr: hi operands
-// only; single_pass: a conv_f16x1_* call.
+// only; single_pass: a conv_f16x1_* call. x_f16 / y_f16: x, or y and the residual, are __half (single-pass calls on the
+// halo and 1x1 kernels without statistics only).
 int conv_launch(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift, int pre_relu,
                 const void* w_hi, const void* w_lo, int f16, bool single_pass, const float* bias,
                 const float* residual, const float* relu_mask, float* y, float out_scale, const float* in_scale, int B,
                 int H, int W, int Cin, int Cout, int ksize, int num_sms, cudaStream_t stream, double* stat_part,
-                const float* stat_pivot) {
+                const float* stat_pivot, bool x_f16 = false, bool y_f16 = false) {
   FPD_REQUIRE(x && w_hi && y, "conv_wgmma: null operand");
   FPD_REQUIRE((double)B * H * W * Cout < 4294967296.0, "conv_wgmma: output has 2^32 or more elements");
   FPD_REQUIRE((pre_scale == nullptr) == (pre_shift == nullptr), "conv_wgmma: pre_scale/pre_shift come in pairs");
@@ -1088,6 +1136,8 @@ int conv_launch(const float* x, const float* pre_mean, const float* pre_scale, c
   ConvParams p = conv_shape_params(B, H, W, Cin, Cout, ksize, f16, w_lo ? 3 : 1);
   const ConvPlan pl = conv_plan(p, f16, single_pass, stat_part != nullptr, num_sms);
   FPD_REQUIRE(pl.kernel != kConvNone, "conv_wgmma: shared memory plan %zu B too large", pl.smem);
+  FPD_REQUIRE(!(x_f16 || y_f16) || (single_pass && !w_lo && !stat_part && (pl.kernel == kConvHalo || pl.kernel == kConvPw)),
+              "conv_wgmma: half-precision activations need a single-pass halo or 1x1 launch without statistics");
   p.x = x; p.w_hi = w_hi; p.w_lo = w_lo;
   p.pre_mean = pre_mean; p.pre_scale = pre_scale; p.pre_shift = pre_shift; p.pre_relu = pre_relu;
   p.bias = bias; p.residual = residual; p.relu_mask = relu_mask; p.y = y;
@@ -1104,12 +1154,16 @@ int conv_launch(const float* x, const float* pre_mean, const float* pre_scale, c
   }
   return with_slice(p.nt, [&](auto n) {
     constexpr int kN = decltype(n)::value;
-    if (pl.kernel == kConvHalo)
-      return split ? launch<conv_halo_kernel<kN>>(pl.grid, kThreads, pl.smem, stream, p, hi, lo)
-                   : launch<conv_halo_f16x1_kernel<kN>>(pl.grid, kThreads, pl.smem, stream, p, hi);
-    if (pl.kernel == kConvPw)
-      return split ? launch<pw_conv_wgmma_kernel<kN>>(pl.grid, kThreads, pl.smem, stream, p)
-                   : launch<pw_conv_f16x1_kernel<kN>>(pl.grid, kThreads, pl.smem, stream, p);
+    if (pl.kernel == kConvHalo && split) return launch<conv_halo_kernel<kN>>(pl.grid, kThreads, pl.smem, stream, p, hi, lo);
+    if (pl.kernel == kConvPw && split) return launch<pw_conv_wgmma_kernel<kN>>(pl.grid, kThreads, pl.smem, stream, p);
+    if (pl.kernel == kConvHalo || pl.kernel == kConvPw)
+      return with_act_types(x_f16, y_f16, [&](auto ti, auto to) {
+        using TIn = typename decltype(ti)::type;
+        using TOut = typename decltype(to)::type;
+        return pl.kernel == kConvHalo
+                   ? launch<conv_halo_f16x1_kernel<kN, TIn, TOut>>(pl.grid, kThreads, pl.smem, stream, p, hi)
+                   : launch<pw_conv_f16x1_kernel<kN, TIn, TOut>>(pl.grid, kThreads, pl.smem, stream, p);
+      });
     return f16 ? launch<conv_wgmma_kernel<true, kN>>(pl.grid, kThreads, pl.smem, stream, p)
                : launch<conv_wgmma_kernel<false, kN>>(pl.grid, kThreads, pl.smem, stream, p);
   });
@@ -1622,6 +1676,23 @@ int conv_f16x1_launch(const float* x, const float* pre_mean, const float* pre_sc
               W, Cin, Cout, ksize, stat_part != nullptr, kMaxStatCout);
   return conv_launch(x, pre_mean, pre_scale, pre_shift, pre_relu, w, nullptr, 1, true, bias, residual, relu_mask, y,
                      out_scale, in_scale, B, H, W, Cin, Cout, ksize, num_sms, stream, stat_part, stat_pivot);
+}
+
+int conv_f16x1_io_launch(const void* x, int x_f16, const float* pre_mean, const float* pre_scale,
+                         const float* pre_shift, int pre_relu, const void* w, const float* bias, const void* residual,
+                         void* y, int y_f16, float out_scale, int B, int H, int W, int Cin, int Cout, int ksize,
+                         int num_sms, cudaStream_t stream) {
+  FPD_REQUIRE(conv_f16x1_supported(B, H, W, Cin, Cout, ksize, false),
+              "conv_f16x1_io: unsupported shape B=%d H=%d W=%d Cin=%d Cout=%d k=%d", B, H, W, Cin, Cout, ksize);
+  const int kind = conv_f16x1_kernel(B, H, W, Cin, Cout, ksize, 0, num_sms, nullptr);
+  if (kind != kConvHalo && kind != kConvPw) {
+    set_last_error("conv_f16x1_io: B=%d H=%d W=%d Cin=%d Cout=%d k=%d runs on the staged kernel, which has no "
+                   "half-precision activation form", B, H, W, Cin, Cout, ksize);
+    return FPD_ERR_UNSUPPORTED;
+  }
+  return conv_launch(static_cast<const float*>(x), pre_mean, pre_scale, pre_shift, pre_relu, w, nullptr, 1, true, bias,
+                     static_cast<const float*>(residual), nullptr, static_cast<float*>(y), out_scale, nullptr, B, H, W,
+                     Cin, Cout, ksize, num_sms, stream, nullptr, nullptr, x_f16 != 0, y_f16 != 0);
 }
 
 // ---------------------------------------------- weight-gradient entry points ----------------------------------------------

@@ -611,8 +611,10 @@ __global__ void affine_act_bwd_kernel(const float4* __restrict__ da, const float
   }
 }
 
-__global__ void maxpool2x2_fwd_kernel(const float4* __restrict__ x, float4* __restrict__ y, int B, int Ho, int Wo,
-                                      int L) {
+// T: the activation type (float, or __half for the fp16 activation storage of inference precision "fp16_act": loads
+// widen to fp32, stores are one saturating fp16_rn, ld_act4 / st_act4 of common.cuh). Vectors of 4 channels.
+template <typename T>
+__global__ void maxpool2x2_fwd_kernel(const T* __restrict__ x, T* __restrict__ y, int B, int Ho, int Wo, int L) {
   const int64_t n = (int64_t)B * Ho * Wo * L;
   const int W = Wo * 2;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
@@ -622,15 +624,48 @@ __global__ void maxpool2x2_fwd_kernel(const float4* __restrict__ x, float4* __re
     const int ho = (int)(t % Ho);
     const int b = (int)(t / Ho);
     const int64_t base = (((int64_t)b * Ho * 2 + ho * 2) * W + wo * 2) * L + cx;
-    const float4 a = __ldg(x + base), bb = __ldg(x + base + L), c = __ldg(x + base + (int64_t)W * L),
-                 d = __ldg(x + base + (int64_t)W * L + L);
+    const float4 a = ld_act4(x, base), bb = ld_act4(x, base + L), c = ld_act4(x, base + (int64_t)W * L),
+                 d = ld_act4(x, base + (int64_t)W * L + L);
     float4 r;
     r.x = fmaxf(fmaxf(a.x, bb.x), fmaxf(c.x, d.x));
     r.y = fmaxf(fmaxf(a.y, bb.y), fmaxf(c.y, d.y));
     r.z = fmaxf(fmaxf(a.z, bb.z), fmaxf(c.z, d.z));
     r.w = fmaxf(fmaxf(a.w, bb.w), fmaxf(c.w, d.w));
-    y[i] = r;
+    st_act4(y, i, r);
   }
+}
+
+// y = relu?((x - mean) * scale + shift (+ residual)) with fp16 x, residual and y: the expression of
+// affine_act_split_kernel's unrounded form, in fp32 from float(x), float(residual).
+__global__ void affine_act_f16_kernel(const __half* __restrict__ x, const float* __restrict__ mean,
+                                      const float* __restrict__ scale, const float* __restrict__ shift, int relu,
+                                      const __half* __restrict__ residual, __half* __restrict__ y, int64_t n4, int L) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
+    float4 v = ld_act4(x, i);
+    if (scale) {
+      const int cx = (int)(i % L);
+      const float4 sc = __ldg(reinterpret_cast<const float4*>(scale) + cx);
+      const float4 sh = __ldg(reinterpret_cast<const float4*>(shift) + cx);
+      const float4 mu = mean ? __ldg(reinterpret_cast<const float4*>(mean) + cx) : make_float4(0.f, 0.f, 0.f, 0.f);
+      v.x = fmaf(v.x - mu.x, sc.x, sh.x); v.y = fmaf(v.y - mu.y, sc.y, sh.y);
+      v.z = fmaf(v.z - mu.z, sc.z, sh.z); v.w = fmaf(v.w - mu.w, sc.w, sh.w);
+    }
+    if (residual) {
+      const float4 r = ld_act4(residual, i);
+      v.x += r.x; v.y += r.y; v.z += r.z; v.w += r.w;
+    }
+    if (relu) {
+      v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
+    }
+    st_act4(y, i, v);
+  }
+}
+
+// The explicit widening of fp16 activations for the calls that have no half-precision form (CUDA-core convolutions,
+// the staged tensor-core kernel): y = float(x), n4 vectors of 4.
+__global__ void half_to_float_kernel(const __half* __restrict__ x, float* __restrict__ y, int64_t n4) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x)
+    st_act4(y, i, ld_act4(x, i));
 }
 
 // gradient goes to the first maximum in window scan order (row-major), like ATen's max_pool2d backward
@@ -674,8 +709,9 @@ __global__ void maxpool2x2_bwd_kernel(const float4* __restrict__ x, const float4
   }
 }
 
-__global__ void upsample2x_add_kernel(const float4* __restrict__ up1, const float4* __restrict__ low,
-                                      float4* __restrict__ out, int B, int H, int W, int L) {
+template <typename T>
+__global__ void upsample2x_add_kernel(const T* __restrict__ up1, const T* __restrict__ low, T* __restrict__ out, int B,
+                                      int H, int W, int L) {
   const int64_t n = (int64_t)B * H * W * L;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const int cx = (int)(i % L);
@@ -683,9 +719,9 @@ __global__ void upsample2x_add_kernel(const float4* __restrict__ up1, const floa
     const int w = (int)(t % W); t /= W;
     const int h = (int)(t % H);
     const int b = (int)(t / H);
-    const float4 a = __ldg(up1 + i);
-    const float4 l = __ldg(low + (((int64_t)b * (H / 2) + h / 2) * (W / 2) + w / 2) * L + cx);
-    out[i] = make_float4(a.x + l.x, a.y + l.y, a.z + l.z, a.w + l.w);
+    const float4 a = ld_act4(up1, i);
+    const float4 l = ld_act4(low, (((int64_t)b * (H / 2) + h / 2) * (W / 2) + w / 2) * L + cx);
+    st_act4(out, i, make_float4(a.x + l.x, a.y + l.y, a.z + l.z, a.w + l.w));
   }
 }
 
@@ -710,7 +746,8 @@ __global__ void upsample2x_bwd_kernel(const float4* __restrict__ dout, float4* _
 // Stride-2 convolutions on the stride-1 tensor-core kernels: y_s2[ho, wo] = y_s1[2 ho, 2 wo] (k = 3, pad = 1), so the
 // forward is the stride-1 convolution followed by this even-position pick, and the backward feeds the stride-1 data /
 // weight gradient kernels with dY scattered back to the even positions of a zero tensor.
-__global__ void subsample2_kernel(const float4* __restrict__ x, float4* __restrict__ y, int B, int Ho, int Wo, int L) {
+template <typename T>
+__global__ void subsample2_kernel(const T* __restrict__ x, T* __restrict__ y, int B, int Ho, int Wo, int L) {
   const int64_t n = (int64_t)B * Ho * Wo * L;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const int cx = (int)(i % L);
@@ -718,7 +755,7 @@ __global__ void subsample2_kernel(const float4* __restrict__ x, float4* __restri
     const int wo = (int)(t % Wo); t /= Wo;
     const int ho = (int)(t % Ho);
     const int64_t b = t / Ho;
-    y[i] = __ldg(x + ((b * (2 * Ho) + 2 * ho) * (2 * Wo) + 2 * wo) * L + cx);
+    st_act4(y, i, ld_act4(x, ((b * (2 * Ho) + 2 * ho) * (2 * Wo) + 2 * wo) * L + cx));
   }
 }
 __global__ void upsample_zero2_kernel(const float4* __restrict__ dy, float4* __restrict__ dx, int B, int Ho, int Wo, int L) {
@@ -975,14 +1012,15 @@ __global__ void weight_prep_f16_both_kernel(const float* __restrict__ w, __half*
 
 // ---- HRNet glue (reference lib/models/pose_hrnet.py:256-263 fuse, :41-57 BasicBlock tail) -------------------
 struct FuseTerms {
-  const float4* t[4];
+  const void* t[4];   // float or __half, as the kernel's T
   int shift[4];  // log2 of the nearest-neighbour upsampling factor of each term
   int n;
 };
 
 // out[b,h,w,:] = relu?( sum_j t_j[b, h >> s_j, w >> s_j, :] ), summed in term order like the reference's
-// `y = y + fuse_layers[i][j](x[j])` loop
-__global__ void fuse_sum_kernel(FuseTerms ft, int relu, float4* __restrict__ out, int B, int H, int W, int L) {
+// `y = y + fuse_layers[i][j](x[j])` loop (in fp32 for both activation types T)
+template <typename T>
+__global__ void fuse_sum_kernel(FuseTerms ft, int relu, T* __restrict__ out, int B, int H, int W, int L) {
   const int64_t n = (int64_t)B * H * W * L;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const int cx = (int)(i % L);
@@ -994,12 +1032,12 @@ __global__ void fuse_sum_kernel(FuseTerms ft, int relu, float4* __restrict__ out
     for (int j = 0; j < ft.n; ++j) {
       const int s = ft.shift[j];
       const int hs = H >> s, wsz = W >> s;
-      const float4 v = __ldg(ft.t[j] + (((int64_t)b * hs + (h >> s)) * wsz + (w >> s)) * L + cx);
+      const float4 v = ld_act4(static_cast<const T*>(ft.t[j]), (((int64_t)b * hs + (h >> s)) * wsz + (w >> s)) * L + cx);
       if (j == 0) acc = v;
       else { acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w; }
     }
     if (relu) { acc.x = fmaxf(acc.x, 0.f); acc.y = fmaxf(acc.y, 0.f); acc.z = fmaxf(acc.z, 0.f); acc.w = fmaxf(acc.w, 0.f); }
-    out[i] = acc;
+    st_act4(out, i, acc);
   }
 }
 
@@ -1138,10 +1176,36 @@ int affine_act(const float* x, const float* mean, const float* scale, const floa
   return FPD_OK;
 }
 
+int affine_act_f16(const void* x, const float* mean, const float* scale, const float* shift, const void* residual,
+                   int relu, void* y, int64_t P, int C, cudaStream_t stream) {
+  FPD_REQUIRE(C % 4 == 0, "affine_act_f16: C=%d must be a multiple of 4", C);
+  FPD_REQUIRE((scale == nullptr) == (shift == nullptr), "affine_act_f16: scale/shift must come in pairs");
+  const int64_t n4 = P * C / 4;
+  affine_act_f16_kernel<<<grid_for(n4, 256), 256, 0, stream>>>((const __half*)x, mean, scale, shift, relu,
+                                                               (const __half*)residual, (__half*)y, n4, C / 4);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int half_to_float(const void* x, float* y, int64_t n, cudaStream_t stream) {
+  FPD_REQUIRE(n % 4 == 0, "half_to_float: n=%lld must be a multiple of 4", (long long)n);
+  half_to_float_kernel<<<grid_for(n / 4, 256), 256, 0, stream>>>((const __half*)x, y, n / 4);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
 int maxpool2x2_fwd(const float* x, float* y, int B, int H, int W, int C, cudaStream_t stream) {
   FPD_REQUIRE(C % 4 == 0 && H % 2 == 0 && W % 2 == 0, "maxpool2x2: bad shape H=%d W=%d C=%d", H, W, C);
   const int64_t n = (int64_t)B * (H / 2) * (W / 2) * (C / 4);
-  maxpool2x2_fwd_kernel<<<grid_for(n, 256), 256, 0, stream>>>((const float4*)x, (float4*)y, B, H / 2, W / 2, C / 4);
+  maxpool2x2_fwd_kernel<<<grid_for(n, 256), 256, 0, stream>>>(x, y, B, H / 2, W / 2, C / 4);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int maxpool2x2_fwd_f16(const void* x, void* y, int B, int H, int W, int C, cudaStream_t stream) {
+  FPD_REQUIRE(C % 4 == 0 && H % 2 == 0 && W % 2 == 0, "maxpool2x2_f16: bad shape H=%d W=%d C=%d", H, W, C);
+  const int64_t n = (int64_t)B * (H / 2) * (W / 2) * (C / 4);
+  maxpool2x2_fwd_kernel<<<grid_for(n, 256), 256, 0, stream>>>((const __half*)x, (__half*)y, B, H / 2, W / 2, C / 4);
   FPD_LAUNCH_CHECK();
   return FPD_OK;
 }
@@ -1159,8 +1223,16 @@ int maxpool2x2_bwd(const float* x, const float* dy, float* dx, int accumulate, i
 int upsample2x_add(const float* up1, const float* low, float* out, int B, int H, int W, int C, cudaStream_t stream) {
   FPD_REQUIRE(C % 4 == 0 && H % 2 == 0 && W % 2 == 0, "upsample2x_add: bad shape H=%d W=%d C=%d", H, W, C);
   const int64_t n = (int64_t)B * H * W * (C / 4);
-  upsample2x_add_kernel<<<grid_for(n, 256), 256, 0, stream>>>((const float4*)up1, (const float4*)low, (float4*)out,
-                                                              B, H, W, C / 4);
+  upsample2x_add_kernel<<<grid_for(n, 256), 256, 0, stream>>>(up1, low, out, B, H, W, C / 4);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int upsample2x_add_f16(const void* up1, const void* low, void* out, int B, int H, int W, int C, cudaStream_t stream) {
+  FPD_REQUIRE(C % 4 == 0 && H % 2 == 0 && W % 2 == 0, "upsample2x_add_f16: bad shape H=%d W=%d C=%d", H, W, C);
+  const int64_t n = (int64_t)B * H * W * (C / 4);
+  upsample2x_add_kernel<<<grid_for(n, 256), 256, 0, stream>>>((const __half*)up1, (const __half*)low, (__half*)out, B,
+                                                              H, W, C / 4);
   FPD_LAUNCH_CHECK();
   return FPD_OK;
 }
@@ -1177,7 +1249,16 @@ int upsample2x_bwd(const float* dout, float* dlow, int B, int H, int W, int C, c
 int subsample2(const float* x, float* y, int B, int H, int W, int C, cudaStream_t stream) {
   FPD_REQUIRE(C % 4 == 0 && H % 2 == 0 && W % 2 == 0, "subsample2: need C %% 4 == 0 and even H, W (C=%d H=%d W=%d)", C, H, W);
   const int64_t n = (int64_t)B * (H / 2) * (W / 2) * (C / 4);
-  subsample2_kernel<<<grid_for(n, 256), 256, 0, stream>>>((const float4*)x, (float4*)y, B, H / 2, W / 2, C / 4);
+  subsample2_kernel<<<grid_for(n, 256), 256, 0, stream>>>(x, y, B, H / 2, W / 2, C / 4);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int subsample2_f16(const void* x, void* y, int B, int H, int W, int C, cudaStream_t stream) {
+  FPD_REQUIRE(C % 4 == 0 && H % 2 == 0 && W % 2 == 0, "subsample2_f16: need C %% 4 == 0 and even H, W (C=%d H=%d W=%d)",
+              C, H, W);
+  const int64_t n = (int64_t)B * (H / 2) * (W / 2) * (C / 4);
+  subsample2_kernel<<<grid_for(n, 256), 256, 0, stream>>>((const __half*)x, (__half*)y, B, H / 2, W / 2, C / 4);
   FPD_LAUNCH_CHECK();
   return FPD_OK;
 }
@@ -1490,8 +1571,9 @@ int affine_add_act(const float* x, const float* mean, const float* scale, const 
   return FPD_OK;
 }
 
-int fuse_sum(const float* const* terms, const int* shifts, int n, int relu, float* out, int B, int H, int W, int C,
-             cudaStream_t stream) {
+template <typename T>
+static int fuse_sum_t(const void* const* terms, const int* shifts, int n, int relu, T* out, int B, int H, int W, int C,
+                      cudaStream_t stream) {
   FPD_REQUIRE(n >= 1 && n <= 4, "fuse_sum: 1..4 terms, got %d", n);
   FPD_REQUIRE(C % 4 == 0, "fuse_sum: C=%d must be a multiple of 4", C);
   FuseTerms ft{};
@@ -1499,13 +1581,23 @@ int fuse_sum(const float* const* terms, const int* shifts, int n, int relu, floa
   for (int j = 0; j < n; ++j) {
     FPD_REQUIRE(shifts[j] >= 0 && (H % (1 << shifts[j])) == 0 && (W % (1 << shifts[j])) == 0,
                 "fuse_sum: term %d upsampling factor does not divide the output size", j);
-    ft.t[j] = (const float4*)terms[j];
+    ft.t[j] = terms[j];
     ft.shift[j] = shifts[j];
   }
   const int64_t n4 = (int64_t)B * H * W * (C / 4);
-  fuse_sum_kernel<<<grid_for(n4, 256), 256, 0, stream>>>(ft, relu, (float4*)out, B, H, W, C / 4);
+  fuse_sum_kernel<<<grid_for(n4, 256), 256, 0, stream>>>(ft, relu, out, B, H, W, C / 4);
   FPD_LAUNCH_CHECK();
   return FPD_OK;
+}
+
+int fuse_sum(const float* const* terms, const int* shifts, int n, int relu, float* out, int B, int H, int W, int C,
+             cudaStream_t stream) {
+  return fuse_sum_t(reinterpret_cast<const void* const*>(terms), shifts, n, relu, out, B, H, W, C, stream);
+}
+
+int fuse_sum_f16(const void* const* terms, const int* shifts, int n, int relu, void* out, int B, int H, int W, int C,
+                 cudaStream_t stream) {
+  return fuse_sum_t(terms, shifts, n, relu, (__half*)out, B, H, W, C, stream);
 }
 
 int upsample_bwd(const float* dout, float* dlow, int shift, int B, int H, int W, int C, cudaStream_t stream) {

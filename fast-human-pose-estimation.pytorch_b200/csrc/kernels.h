@@ -43,6 +43,12 @@ int conv_f16x1_launch(const float* x, const float* pre_mean, const float* pre_sc
                       int pre_relu, const void* w, const float* bias, const float* residual, const float* relu_mask,
                       float* y, float out_scale, const float* in_scale, int B, int H, int W, int Cin, int Cout,
                       int ksize, int num_sms, cudaStream_t stream, double* stat_part, const float* stat_pivot);
+// The same inference convolution with fp32 or fp16 (x_f16 / y_f16) NHWC activations: x, and y with the residual, of
+// either type; shapes conv_f16x1_kernel sends to the halo or 1x1 kernel only (FPD_ERR_UNSUPPORTED otherwise).
+int conv_f16x1_io_launch(const void* x, int x_f16, const float* pre_mean, const float* pre_scale,
+                         const float* pre_shift, int pre_relu, const void* w, const float* bias, const void* residual,
+                         void* y, int y_f16, float out_scale, int B, int H, int W, int Cin, int Cout, int ksize,
+                         int num_sms, cudaStream_t stream);
 
 // ---- conv_wgmma.cu : warpgroup-MMA weight-gradient GEMM (K = pixels) reading RAW x and dY; BN-apply + ReLU + tf32 split
 //      fused into the operand staging ----
@@ -110,6 +116,18 @@ int maxpool3x3s2_bwd(const float* x, const float* dy, float* dx, int accumulate,
 int depth_space2(const float* src, float* dst, int B, int H, int W, int C, int to_depth, cudaStream_t stream);
 int deconv_weight_map(const float* src, float* dst, int Cin, int Cout, int k, int pad, int to_deconv, cudaStream_t stream);
 int subsample2(const float* x, float* y, int B, int H, int W, int C, cudaStream_t stream);        // y[ho,wo] = x[2ho,2wo]
+// fp16-in / fp16-out forms of the eval-path glue above (inference precision "fp16_act"): the fp32 kernel's arithmetic
+// on float(x), one saturating fp16_rn per stored value. affine_act_f16 covers affine_act (residual NULL) and
+// affine_add_act.
+int affine_act_f16(const void* x, const float* mean, const float* scale, const float* shift, const void* residual,
+                   int relu, void* y, int64_t P, int C, cudaStream_t stream);
+int fuse_sum_f16(const void* const* terms, const int* shifts, int n, int relu, void* out, int B, int H, int W, int C,
+                 cudaStream_t stream);
+int maxpool2x2_fwd_f16(const void* x, void* y, int B, int H, int W, int C, cudaStream_t stream);
+int upsample2x_add_f16(const void* up1, const void* low, void* out, int B, int H, int W, int C, cudaStream_t stream);
+int subsample2_f16(const void* x, void* y, int B, int H, int W, int C, cudaStream_t stream);
+// y = float(x) for fp16 x of n elements (n % 4 == 0): the widening before a call with no half-precision form
+int half_to_float(const void* x, float* y, int64_t n, cudaStream_t stream);
 int upsample_zero2(const float* dy, float* dx, int B, int Ho, int Wo, int C, cudaStream_t stream);  // adjoint of subsample2
 int nchw_to_nhwc(const float* x, float* y, int B, int C, int H, int W, cudaStream_t stream);
 int nchw_to_nhwc_flipw(const float* x, float* y, int B, int C, int H, int W, cudaStream_t stream);   // + W mirror

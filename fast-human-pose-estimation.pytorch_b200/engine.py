@@ -35,7 +35,7 @@ def precision_passes():
     raise ValueError("FPD_PRECISION must be tf32x3 or tf32, got %r" % mode)
 
 
-INFERENCE_PRECISIONS = ("fp32", "fp16")
+INFERENCE_PRECISIONS = ("fp32", "fp16", "fp16_act")
 TRAINING_PRECISIONS = ("fp32", "fp16")
 
 
@@ -61,10 +61,18 @@ def set_inference_precision(model, precision):
     """Operand precision of `model`'s eval-mode forwards that record no tape (net(x) under no_grad, forward_nhwc,
     FlipTestInference, a frozen FPD teacher): "fp32" (the default: 3xFP16 / 3xTF32, fp32-grade) or "fp16" (single-pass
     FP16 on ops.conv2d_tc_f16x1 for every convolution it takes: about 2^-11 relative operand rounding, one MMA per
-    product instead of three). Training forwards and forwards that record a backward tape follow
-    set_training_precision instead.
+    product instead of three) or "fp16_act" (hourglass and HRNet only: the convolutions of "fp16", with the activations
+    between layers stored as fp16 NHWC tensors -- the kernels compute in fp32 and store one saturating fp16_rn per
+    value; the image, the stem's im2col columns and the network outputs stay fp32). Training forwards and forwards that
+    record a backward tape follow set_training_precision instead.
     `model`: an fpd_b200 hourglass / HRNet / ResNet network or an nn.DataParallel around one. Returns the previous
     setting; a change drops the cached eval operands and bumps the engine generation, so captured graphs capture again."""
+    if precision == "fp16_act":
+        from .lib.models.pose_resnet import PoseResNet
+        net = model.module if isinstance(model, torch.nn.DataParallel) else model
+        if isinstance(net, PoseResNet):
+            raise ValueError('inference precision "fp16_act" supports the hourglass (HourglassNet) and HRNet '
+                             '(PoseHighResolutionNet) networks, not PoseResNet')
     return _set_precision(model, "inference_precision", precision, INFERENCE_PRECISIONS, "inference")
 
 
@@ -277,6 +285,34 @@ def _tc_conv(e, x, k, in_scale=None, **kw):
     return ops.conv2d_tc_fused(x, e.hi, e.lo, k, **kw)
 
 
+def _f32(t):
+    """t as fp32: an fp16 activation widened by one conversion kernel, for the calls that have no fp16 form."""
+    return ops.half_to_float(t) if t is not None and t.dtype == torch.float16 else t
+
+
+def act16_conv_form(e, B, H, W, cin, k, out_f16, res_dtype=None):
+    """-> (kernel, output dtype) of a tensor-core convolution from cin channels at B x H x W with prepared weights e in an
+    eval forward at inference precision "fp16_act": ("halo" or "1x1", fp16 if out_f16 else fp32) where the single-pass
+    kernel has an fp16-activation form (it then reads the input as stored, fp32 or fp16) and the residual (res_dtype,
+    None without one) has the output's type; otherwise ("widen", fp32): the input and the residual are widened and the
+    fp32-activation kernel writes fp32. Host only."""
+    out = torch.float16 if out_f16 else torch.float32
+    if e.kernel == TC_F16X1 and res_dtype in (None, out):
+        kind = ops.conv2d_tc_f16x1_kernel(B, H, W, cin, e.hi.shape[1], k)
+        if kind in ("halo", "1x1"):
+            return kind, out
+    return "widen", torch.float32
+
+
+def _act16_conv(e, x, k, out_f16, residual=None, **kw):
+    """The tensor-core forward of an eval forward at "fp16_act": fp16-activation form or widening (act16_conv_form)."""
+    B, H, W, cin = x.shape
+    kind, out = act16_conv_form(e, B, H, W, cin, k, out_f16, None if residual is None else residual.dtype)
+    if kind != "widen":
+        return ops.conv2d_tc_f16x1_io(x, e.hi, k, residual=residual, out_dtype=out, **kw)
+    return _tc_conv(e, _f32(x), k, residual=_f32(residual), **kw)
+
+
 class Engine:
     """Runs one forward (and optionally records a backward tape) of a hourglass-family module tree."""
 
@@ -331,7 +367,7 @@ class Engine:
         key = self._param_version()
         if self._eval_cache is None or self._eval_cache_key != key:
             passes = precision_passes()
-            w = PreparedWeights(passes, f16x1=self.inference_precision == "fp16")
+            w = PreparedWeights(passes, f16x1=self.inference_precision in ("fp16", "fp16_act"))
             affine = {}
             for name, b in self.bns.items():
                 m = b.mod
@@ -417,7 +453,8 @@ class Engine:
     def bn_act(self, ctx, x, bn_name, relu=True):
         """Materialised y = relu(bn(x)) (stem bn1, fc bn): reference hourglass.py:117-119,161-168."""
         aff = self._bn_affine(ctx, x, bn_name)
-        out = Var(ops.affine_act(x.data, aff[0], aff[1], relu, mean=aff[2]))
+        act = ops.affine_act_f16 if x.data.dtype == torch.float16 else ops.affine_act
+        out = Var(act(x.data, aff[0], aff[1], relu, mean=aff[2]))
         if ctx.tape is not None:
             def bwd():
                 if out.grad is None:
@@ -426,27 +463,32 @@ class Engine:
             ctx.tape.append(bwd)
         return out
 
-    def conv(self, ctx, x, conv_name, bn_name=None, relu=False, residual=None, need_dx=True, out_bn=None):
+    def conv(self, ctx, x, conv_name, bn_name=None, relu=False, residual=None, need_dx=True, out_bn=None, head=False):
         """y = conv(act(bn(x))) + bias (+ residual).  bn_name None -> the conv consumes x raw.
         out_bn: name of a train-mode BatchNorm that will consume y (True: some BatchNorm, name unknown) -- the conv then
-        also emits y's per-channel sums from its epilogue (Var.stat_sums), pivoted on that module's running mean."""
+        also emits y's per-channel sums from its epilogue (Var.stat_sums), pivoted on that module's running mean.
+        head: y is a network output (a heat-map), stored as fp32 at inference precision "fp16_act" too."""
         c = conv_name if isinstance(conv_name, ConvRef) else self.convs[conv_name]
         H, W = x.data.shape[1], x.data.shape[2]
         if (c.pick_first and H % 2 == 0 and W % 2 == 0 and bn_name is None and residual is None
                 and x.data.shape[-1] % 4 == 0 and c.tc_fwd_at(H // 2, W // 2)):
-            return self._conv_at(ctx, self.subsample2(ctx, x), c, None, relu, None, need_dx, out_bn, stride=1)
+            return self._conv_at(ctx, self.subsample2(ctx, x), c, None, relu, None, need_dx, out_bn, stride=1,
+                                 head=head)
         if (c.as_s1 and H % 2 == 0 and W % 2 == 0 and c.cout % 4 == 0 and c.tc_fwd_at(H, W) and residual is None
                 and not (bn_name is None and c.im2col_kpad)):
             # stride 2 = stride-1 convolution on the tensor cores + even-position pick (recorded as two tape entries:
             # the pick's backward scatters dY into a zero tensor, the stride-1 conv's backward is the ordinary one)
-            full = self._conv_at(ctx, x, c, bn_name, relu, None, need_dx, None, stride=1, as_s1=True)
+            full = self._conv_at(ctx, x, c, bn_name, relu, None, need_dx, None, stride=1, as_s1=True, head=head)
             return self.subsample2(ctx, full)
-        return self._conv_at(ctx, x, c, bn_name, relu, residual, need_dx, out_bn, stride=c.stride)
+        return self._conv_at(ctx, x, c, bn_name, relu, residual, need_dx, out_bn, stride=c.stride, head=head)
 
-    def _conv_at(self, ctx, x, c, bn_name, relu, residual, need_dx, out_bn, stride, as_s1=False):
+    def _conv_at(self, ctx, x, c, bn_name, relu, residual, need_dx, out_bn, stride, as_s1=False, head=False):
         """Engine.conv at `stride`: 1 for the stride-2 convolutions that conv routes to the stride-1 kernels (pick_first:
-        x is already the picked tensor; as_s1: a stride-2 3x3 run at stride 1, its dY arrives zero-upsampled)."""
+        x is already the picked tensor; as_s1: a stride-2 3x3 run at stride 1, its dY arrives zero-upsampled).
+        At inference precision "fp16_act" (ctx.act16) the tensor-core forward reads x as stored and writes fp16 (fp32 for
+        a head) where the single-pass kernel has that form; every other call widens its fp16 inputs and writes fp32."""
         Hx, Wx = x.data.shape[1], x.data.shape[2]
+        out_f16 = ctx.act16 and not head
         tc_fwd = c.tc_fwd_at(Hx, Wx) and stride == 1
         scale = shift = mean = None
         aff = None
@@ -464,7 +506,11 @@ class Engine:
                 cols = ops.im2col(x.data, c.k, c.stride, c.pad, kpad)
                 if ctx.shared_stem is not None and "cols_key" not in ctx.shared_stem:
                     ctx.shared_stem["cols_key"], ctx.shared_stem["cols"] = key, cols
-            out = Var(_tc_conv(ctx.weights.fwd(c, cols.shape[1], cols.shape[2]), cols, 1, bias=bias, residual=res))
+            e = ctx.weights.fwd(c, cols.shape[1], cols.shape[2])
+            if ctx.act16:
+                out = Var(_act16_conv(e, cols, 1, out_f16, bias=bias, residual=res))
+            else:
+                out = Var(_tc_conv(e, cols, 1, bias=bias, residual=res))
             if ctx.tape is not None:
                 def bwd_stem():
                     dy = out.grad
@@ -495,11 +541,16 @@ class Engine:
                     stat_sums = (torch.empty((nblk, c.cout, 2), dtype=torch.float64, device=x.data.device), nblk, pivot)
             stats = {} if stat_sums is None else dict(stats_part=stat_sums[0], stats_pivot=stat_sums[2])
             # BN-apply + ReLU + operand split happen inside the conv kernel (no separate HBM pass)
-            y = _tc_conv(e, x.data, c.k, mean=mean, scale=scale, shift=shift, relu=relu, bias=bias, residual=res,
-                         **stats)
+            if ctx.act16:
+                y = _act16_conv(e, x.data, c.k, out_f16, mean=mean, scale=scale, shift=shift, relu=relu, bias=bias,
+                                residual=res)
+            else:
+                y = _tc_conv(e, x.data, c.k, mean=mean, scale=scale, shift=shift, relu=relu, bias=bias, residual=res,
+                             **stats)
         else:
-            a = ops.affine_act(x.data, scale, shift, relu, mean=mean) if bn_name is not None else x.data
-            y = ops.conv2d_simt_fwd(a, c.weight.detach(), bias=bias, residual=res, stride=c.stride, pad=c.pad)
+            xd = _f32(x.data)
+            a = ops.affine_act(xd, scale, shift, relu, mean=mean) if bn_name is not None else xd
+            y = ops.conv2d_simt_fwd(a, c.weight.detach(), bias=bias, residual=_f32(res), stride=c.stride, pad=c.pad)
         out = Var(y)
         if tc_fwd:
             out.stat_sums = stat_sums
@@ -570,7 +621,7 @@ class Engine:
 
     def subsample2(self, ctx, x):
         """Even-position pick that turns a stride-1 3x3 convolution into the stride-2 one (see ConvRef.as_s1)."""
-        out = Var(ops.subsample2(x.data))
+        out = Var((ops.subsample2_f16 if x.data.dtype == torch.float16 else ops.subsample2)(x.data))
         if ctx.tape is not None:
             def bwd():
                 if out.grad is None:
@@ -639,7 +690,7 @@ class Engine:
         return out
 
     def maxpool(self, ctx, x):
-        out = Var(ops.maxpool2x2(x.data))
+        out = Var((ops.maxpool2x2_f16 if x.data.dtype == torch.float16 else ops.maxpool2x2)(x.data))
         if ctx.tape is not None:
             def bwd():
                 if out.grad is None:
@@ -651,7 +702,10 @@ class Engine:
         return out
 
     def upsample_add(self, ctx, up1, low):
-        out = Var(ops.upsample2x_add(up1.data, low.data))
+        if up1.data.dtype == low.data.dtype == torch.float16:
+            out = Var(ops.upsample2x_add_f16(up1.data, low.data))
+        else:
+            out = Var(ops.upsample2x_add(_f32(up1.data), _f32(low.data)))
         if ctx.tape is not None:
             def bwd():
                 if out.grad is None:
@@ -742,7 +796,7 @@ class Engine:
             y = self.residual_seq(ctx, y, "res.%d" % i, nb)
             y = self.conv(ctx, y, "fc.%d.0" % i, out_bn="fc.%d.1" % i)
             y = self.bn_act(ctx, y, "fc.%d.1" % i, relu=True)
-            score = self.conv(ctx, y, "score.%d" % i)
+            score = self.conv(ctx, y, "score.%d" % i, head=True)
             outs.append(score)
             if i < net.num_stacks - 1:
                 t = self.conv(ctx, y, "fc_.%d" % i, residual=x)
@@ -778,6 +832,8 @@ class Engine:
         ctx.sync = self._sync_spec() if training else None
         ctx.passes = precision_passes()
         ctx.tape = [] if record_tape else None
+        # set_inference_precision("fp16_act"): fp16 activations between the layers of an eval forward without a tape
+        ctx.act16 = not training and not record_tape and self.inference_precision == "fp16_act"
         # set_training_precision("fp16"): single-pass FP16 convolutions and single-pass TF32 weight gradients
         f16_train = (training or record_tape) and self.training_precision == "fp16"
         ctx.wgrad_passes = 1 if f16_train else ctx.passes
@@ -833,6 +889,7 @@ class _Ctx:
         self.passes = 3
         self.wgrad_passes = 3
         self.tape = None
+        self.act16 = False      # eval forward without a tape at inference precision "fp16_act"
         self.weights = None
         self.affine = None
         self.pgrads = {}

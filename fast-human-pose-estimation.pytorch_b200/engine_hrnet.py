@@ -7,8 +7,10 @@ HRNet blocks are post-activation (conv-BN-ReLU ... conv-BN, +skip, ReLU), so bes
  * fuse       : y = relu(sum_j nearest_up_{2^k}(t_j)) -- the multi-resolution exchange
 Inside a block the BN+ReLU between two convs is still fused into the consuming conv's operand pass.
 """
+import torch
+
 from . import ops
-from .engine import Engine, Var
+from .engine import Engine, Var, _f32
 
 
 class HRNetEngine(Engine):
@@ -19,7 +21,10 @@ class HRNetEngine(Engine):
     # ------------------------------------------------------------------ extra building blocks
     def bn_add_act(self, ctx, x, bn_name, residual, relu=True):
         aff = self._bn_affine(ctx, x, bn_name)
-        out = Var(ops.affine_add_act(x.data, residual.data, aff[0], aff[1], relu, mean=aff[2]))
+        if x.data.dtype == residual.data.dtype == torch.float16:     # inference precision "fp16_act"
+            out = Var(ops.affine_add_act_f16(x.data, residual.data, aff[0], aff[1], relu, mean=aff[2]))
+        else:
+            out = Var(ops.affine_add_act(_f32(x.data), _f32(residual.data), aff[0], aff[1], relu, mean=aff[2]))
         if ctx.tape is not None:
             def bwd():
                 if out.grad is None:
@@ -33,7 +38,11 @@ class HRNetEngine(Engine):
 
     def fuse(self, ctx, terms):
         """terms: list of (Var, log2 upsampling factor). out = relu(sum), pose_hrnet.py:256-263."""
-        out = Var(ops.fuse_sum([t.data for t, _ in terms], [s for _, s in terms], relu=True))
+        data, shifts = [t.data for t, _ in terms], [s for _, s in terms]
+        if all(d.dtype == torch.float16 for d in data):                # inference precision "fp16_act"
+            out = Var(ops.fuse_sum_f16(data, shifts, relu=True))
+        else:
+            out = Var(ops.fuse_sum([_f32(d) for d in data], shifts, relu=True))
         if ctx.tape is not None:
             def bwd():
                 if out.grad is None:
@@ -143,4 +152,4 @@ class HRNetEngine(Engine):
         for s, sc in zip((2, 3, 4), net.stage_cfgs):
             xs = self.transition(ctx, ys, "transition%d" % (s - 1), sc["num_branches"])
             ys = self.stage(ctx, xs, "stage%d" % s, sc["num_modules"])
-        return [self.conv(ctx, ys[0], "final_layer")]
+        return [self.conv(ctx, ys[0], "final_layer", head=True)]

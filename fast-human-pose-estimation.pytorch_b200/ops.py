@@ -316,6 +316,105 @@ def conv2d_tc_f16x1(x, w, ksize, mean=None, scale=None, shift=None, relu=False, 
     return y
 
 
+# ---- fp16 activation storage (engine.set_inference_precision(model, "fp16_act")): the eval-forward kernels with __half
+# NHWC activations. Each computes what its fp32 form computes, in fp32 from the widened inputs, and stores one
+# fp16_rn per value saturated to +-65504 (NaN stays NaN).
+def _chk_f16(t, name, dtypes=(torch.float16,)):
+    if t is None:
+        return
+    if not (t.is_cuda and t.dtype in dtypes and t.is_contiguous()):
+        raise ValueError("%s must be a contiguous %s CUDA tensor (got %s %s %s)" % (
+            name, " or ".join(str(d) for d in dtypes), t.device, t.dtype, t.is_contiguous()))
+
+
+def conv2d_tc_f16x1_io(x, w, ksize, mean=None, scale=None, shift=None, relu=False, bias=None, residual=None,
+                       out_dtype=torch.float16, out=None, out_scale=1.0):
+    """conv2d_tc_f16x1 (no ReLU mask) with fp32 or fp16 x, and y and the residual of out_dtype (fp32 or fp16): bit for
+    bit conv2d_tc_f16x1 on x.float() and residual.float(), rounded as above when out_dtype is fp16. Only for the shapes
+    conv2d_tc_f16x1_kernel runs on "halo" or "1x1"; others raise."""
+    B, H, W, Cin = x.shape
+    Cout = w.shape[1]
+    if w.dtype != torch.float16:
+        raise ValueError("conv2d_tc_f16x1_io takes the __half weights of weight_prep_f16(split=False), got %s" % w.dtype)
+    both = (torch.float32, torch.float16)
+    if out_dtype not in both:
+        raise ValueError("conv2d_tc_f16x1_io: out_dtype must be torch.float32 or torch.float16, got %s" % out_dtype)
+    _chk_f16(x, "x", both)
+    _chk_f16(residual, "residual", (out_dtype,))
+    y = out if out is not None else torch.empty((B, H, W, Cout), dtype=out_dtype, device=x.device)
+    _chk_f16(y, "out", (out_dtype,))
+    N.check(N.lib().fpd_conv2d_tc_f16x1_io(_p(x), int(x.dtype == torch.float16), _p(mean), _p(scale), _p(shift),
+                                           int(relu), _p(w), _p(bias), _p(residual), _p(y),
+                                           int(out_dtype == torch.float16), float(out_scale), B, H, W, Cin, Cout, ksize,
+                                           _stream()), "conv2d_tc_f16x1_io")
+    return y
+
+
+def affine_act_f16(x, scale=None, shift=None, relu=False, out=None, mean=None):
+    _chk_f16(x, "x")
+    C = x.shape[-1]
+    y = out if out is not None else torch.empty_like(x)
+    N.check(N.lib().fpd_affine_act_f16(_p(x), _p(mean), _p(scale), _p(shift), int(relu), _p(y), x.numel() // C, C,
+                                       _stream()), "affine_act_f16")
+    return y
+
+
+def affine_add_act_f16(x, residual, scale=None, shift=None, relu=True, mean=None, out=None):
+    _chk_f16(x, "x")
+    _chk_f16(residual, "residual")
+    C = x.shape[-1]
+    y = out if out is not None else torch.empty_like(x)
+    N.check(N.lib().fpd_affine_add_act_f16(_p(x), _p(mean), _p(scale), _p(shift), _p(residual), int(relu), _p(y),
+                                           x.numel() // C, C, _stream()), "affine_add_act_f16")
+    return y
+
+
+def fuse_sum_f16(terms, shifts, relu=True, out=None):
+    n = len(terms)
+    for t in terms:
+        _chk_f16(t, "terms")
+    B, C = terms[0].shape[0], terms[0].shape[-1]
+    H, W = terms[0].shape[1] << shifts[0], terms[0].shape[2] << shifts[0]
+    y = out if out is not None else torch.empty((B, H, W, C), dtype=torch.float16, device=terms[0].device)
+    arr = (ctypes.c_void_p * n)(*[t.data_ptr() for t in terms])
+    sh = (ctypes.c_int * n)(*[int(s) for s in shifts])
+    N.check(N.lib().fpd_fuse_sum_f16(arr, sh, n, int(relu), _p(y), B, H, W, C, _stream()), "fuse_sum_f16")
+    return y
+
+
+def maxpool2x2_f16(x, out=None):
+    _chk_f16(x, "x")
+    B, H, W, C = x.shape
+    y = out if out is not None else torch.empty((B, H // 2, W // 2, C), dtype=torch.float16, device=x.device)
+    N.check(N.lib().fpd_maxpool2x2_fwd_f16(_p(x), _p(y), B, H, W, C, _stream()), "maxpool2x2_fwd_f16")
+    return y
+
+
+def upsample2x_add_f16(up1, low, out=None):
+    _chk_f16(up1, "up1")
+    _chk_f16(low, "low")
+    B, H, W, C = up1.shape
+    y = out if out is not None else torch.empty_like(up1)
+    N.check(N.lib().fpd_upsample2x_add_f16(_p(up1), _p(low), _p(y), B, H, W, C, _stream()), "upsample2x_add_f16")
+    return y
+
+
+def subsample2_f16(x, out=None):
+    _chk_f16(x, "x")
+    B, H, W, C = x.shape
+    y = out if out is not None else torch.empty((B, H // 2, W // 2, C), dtype=torch.float16, device=x.device)
+    N.check(N.lib().fpd_subsample2_f16(_p(x), _p(y), B, H, W, C, _stream()), "subsample2_f16")
+    return y
+
+
+def half_to_float(x, out=None):
+    """float(x) of an fp16 activation: the one explicit widening before a call that has no fp16 form."""
+    _chk_f16(x, "x")
+    y = out if out is not None else torch.empty(x.shape, dtype=torch.float32, device=x.device)
+    N.check(N.lib().fpd_half_to_float(_p(x), _p(y), x.numel(), _stream()), "half_to_float")
+    return y
+
+
 def conv2d_simt_fwd(x, w_oihw, bias=None, residual=None, stride=1, pad=0, out=None):
     B, H, W, Cin = x.shape
     Cout, _, k, _ = w_oihw.shape

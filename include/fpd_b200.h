@@ -106,6 +106,17 @@ int fpd_conv2d_tc_f16x1_train(const float* x, const float* pre_mean, const float
                               const float* relu_mask, float* y, float out_scale, const float* in_scale, int B, int H,
                               int W, int Cin, int Cout, int ksize, double* stat_part, const float* stat_pivot,
                               fpd_stream_t stream);
+/* fpd_conv2d_tc_f16x1 with fp16 activation storage (inference precision "fp16_act"): x is fp32 (x_f16 = 0) or __half
+ * (x_f16 = 1) NHWC, y and residual (nullable) are both fp32 (y_f16 = 0) or both __half (y_f16 = 1). The operand is
+ * fp16_rn of the same fp32 transform of float(x), the epilogue the same fp32 expression from float(residual); an fp16 y
+ * stores its fp16_rn saturated to +-65504 (NaN stays NaN). So the output equals, bit for bit, fpd_conv2d_tc_f16x1 on the
+ * widened x and residual, rounded the same way. No ReLU mask. Only the shapes fpd_conv2d_tc_f16x1_kernel sends to the
+ * 3x3 halo kernel (2) or the 1x1 weight-resident kernel (3); others return an error (widen with fpd_half_to_float and
+ * call an fp32 convolution instead). */
+int fpd_conv2d_tc_f16x1_io(const void* x, int x_f16, const float* pre_mean, const float* pre_scale,
+                           const float* pre_shift, int pre_relu, const void* w, const float* bias, const void* residual,
+                           void* y, int y_f16, float out_scale, int B, int H, int W, int Cin, int Cout, int ksize,
+                           fpd_stream_t stream);
 /* Forward ([tap][O][I]) and data-gradient ([taps-1-tap][I][O]) __half hi/lo forms of w * 2^8 from one read of the
  * weights: one launch per convolution and training step instead of two. f_lo and d_lo may both be NULL (the
  * single-pass FP16 forms). */
@@ -268,6 +279,23 @@ int fpd_deconv_weight_map(const float* src, float* dst, int Cin, int Cout, int k
  * then feeds the stride-1 data- and weight-gradient kernels. */
 int fpd_subsample2(const float* x, float* y, int B, int H, int W, int C, fpd_stream_t stream);
 int fpd_upsample_zero2(const float* dy, float* dx, int B, int Ho, int Wo, int C, fpd_stream_t stream);
+/* fp16 activation storage (inference precision "fp16_act"): __half-in / __half-out forms of the eval-forward glue
+ * fpd_affine_act, fpd_affine_add_act, fpd_fuse_sum, fpd_maxpool2x2_fwd, fpd_upsample2x_add and fpd_subsample2, with the
+ * same arguments (every activation pointer __half; mean / scale / shift stay fp32). Each computes what its fp32 form
+ * computes, in fp32 from the widened inputs, and stores one fp16_rn per value saturated to +-65504 (NaN stays NaN): the
+ * output equals, bit for bit, the fp32 form on the widened inputs rounded the same way. fpd_half_to_float widens n
+ * (% 4 == 0) __half values to fp32, for the calls that have no half form. */
+int fpd_affine_act_f16(const void* x, const float* mean, const float* scale, const float* shift, int relu, void* y,
+                       int64_t P, int C, fpd_stream_t stream);
+int fpd_affine_add_act_f16(const void* x, const float* mean, const float* scale, const float* shift,
+                           const void* residual, int relu, void* y, int64_t P, int C, fpd_stream_t stream);
+int fpd_fuse_sum_f16(const void* const* terms_host, const int* shifts_host, int n, int relu, void* out, int B, int H,
+                     int W, int C, fpd_stream_t stream);
+int fpd_maxpool2x2_fwd_f16(const void* x, void* y, int B, int H, int W, int C, fpd_stream_t stream);
+int fpd_upsample2x_add_f16(const void* up1, const void* low, void* out, int B, int H, int W, int C,
+                           fpd_stream_t stream); /* H,W = output size */
+int fpd_subsample2_f16(const void* x, void* y, int B, int H, int W, int C, fpd_stream_t stream);
+int fpd_half_to_float(const void* x, float* y, int64_t n, fpd_stream_t stream);
 int fpd_nchw_to_nhwc(const float* x, float* y, int B, int C, int H, int W, fpd_stream_t stream);
 /* Same, with the image mirrored along W on the way (the flipped input of the flip test, lib/core/function.py:218-221:
  * np.flip(input, 3)), so the second forward needs no separate flip pass. */

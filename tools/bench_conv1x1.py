@@ -9,8 +9,11 @@ one: weights are read from L2) and the achieved share of 3.35 TB/s, with the car
 With --single-pass, the forward forms instead run on the 3-pass weight-resident kernel against the single-pass one
 (ops.conv2d_tc_f16x1, pw_conv_f16x1_kernel); the HBM share is then the single-pass kernel's. --train adds the data
 gradients, single-pass with their power-of-two input scale as the training precision "fp16" runs them.
+With --half-io, the forward forms run on the single-pass kernel with fp16 activations (ops.conv2d_tc_f16x1_io: fp16 x,
+residual and y, inference precision "fp16_act") against the same kernel with fp32 activations; the least bytes and the
+HBM share are then those of the fp16 form (2 bytes per activation).
 
-    python tools/bench_conv1x1.py [--windows 7] [--per 8] [--single-pass [--train]]
+    python tools/bench_conv1x1.py [--windows 7] [--per 8] [--single-pass [--train] | --half-io]
 """
 import argparse
 import os
@@ -41,10 +44,11 @@ def card():
     return q
 
 
-def setup(B, H, W, Cin, Cout, form, g, single=False):
+def setup(B, H, W, Cin, Cout, form, g, single=False, half=False):
     from fpd_b200 import ops
-    xs = [torch.randn(B, H, W, Cin, device="cuda", generator=g) for _ in range(2)]
-    ys = [torch.empty(B, H, W, Cout, device="cuda") for _ in range(2)]
+    dt = torch.float16 if half else torch.float32
+    xs = [torch.randn(B, H, W, Cin, device="cuda", generator=g).to(dt) for _ in range(2)]
+    ys = [torch.empty(B, H, W, Cout, device="cuda", dtype=dt) for _ in range(2)]
     w = torch.randn(Cout, Cin, 1, 1, device="cuda", generator=g) * (1.0 / Cin ** 0.5)
     w_hi, w_lo = ops.weight_prep_f16(w)
     kw = {}
@@ -55,15 +59,18 @@ def setup(B, H, W, Cin, Cout, form, g, single=False):
         kw["bias"] = torch.randn(Cout, device="cuda", generator=g)
     else:
         kw["in_scale"] = torch.tensor([256.0, 1.0 / 256.0], device="cuda")
-    res = [torch.randn(B, H, W, Cout, device="cuda", generator=g) for _ in range(2)] if form.endswith("res") else None
-    nbytes = 4 * B * H * W * (Cin + Cout * (2 if res else 1))
+    res = [torch.randn(B, H, W, Cout, device="cuda", generator=g).to(dt) for _ in range(2)] if form.endswith("res") else None
+    nbytes = (2 if half else 4) * B * H * W * (Cin + Cout * (2 if res else 1))
 
     def launch(i):
-        if single:
+        if half:
+            ops.conv2d_tc_f16x1_io(xs[i % 2], w1, 1, residual=res[i % 2] if res else None, out=ys[i % 2],
+                                   out_dtype=torch.float16, **kw)
+        elif single:
             ops.conv2d_tc_f16x1(xs[i % 2], w1, 1, residual=res[i % 2] if res else None, out=ys[i % 2], **kw)
         else:
             ops.conv2d_tc_h(xs[i % 2], w_hi, w_lo, 1, residual=res[i % 2] if res else None, out=ys[i % 2], **kw)
-    w1 = ops.weight_prep_f16(w, split=False)[0] if single else None
+    w1 = ops.weight_prep_f16(w, split=False)[0] if (single or half) else None
     return launch, nbytes
 
 
@@ -91,6 +98,7 @@ def main():
     ap.add_argument("--hw", type=int, default=64)
     ap.add_argument("--single-pass", action="store_true")
     ap.add_argument("--train", action="store_true")
+    ap.add_argument("--half-io", action="store_true")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "bench_conv1x1 measures on the GPU"
     import fpd_b200  # noqa: F401
@@ -99,7 +107,7 @@ def main():
     B, H, W = args.batch, args.hw, args.hw
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
     g = torch.Generator(device="cuda").manual_seed(0)
-    names = ("1-pass", "3-pass") if args.single_pass else ("pw", "staged")
+    names = ("f16-io", "f32-io") if args.half_io else ("1-pass", "3-pass") if args.single_pass else ("pw", "staged")
     print("%-22s %6s %10s %22s %10s %22s %8s %9s %7s" % (
         "shape (Cin->Cout form)", "x/step", names[0] + " us", names[0] + " range", names[1] + " us",
         names[1] + " range", "speedup", "least MB", "HBM %"))
@@ -107,13 +115,19 @@ def main():
     tot_pw = tot_st = 0.0
     try:
         for (Cin, Cout, form, n) in SHAPES:
-            if args.single_pass and form == "dgrad" and not args.train:
+            if (args.single_pass or args.half_io) and form == "dgrad" and not args.train:
                 continue
-            launch, nbytes = setup(B, H, W, Cin, Cout, form, g)
-            graphs = {}
-            for on in (True, False):
-                ops.set_conv1x1(on)
-                graphs[on] = capture(launch, args.per)
+            if args.half_io:       # True: fp16 activations, False: fp32 activations, both single pass
+                launch, nbytes = setup(B, H, W, Cin, Cout, form, g, half=True)
+                graphs = {True: capture(launch, args.per),
+                          False: capture(setup(B, H, W, Cin, Cout, form, g, single=True)[0], args.per)}
+            else:
+                launch, nbytes = setup(B, H, W, Cin, Cout, form, g)
+            if not args.half_io:
+                graphs = {}
+                for on in (True, False):
+                    ops.set_conv1x1(on)
+                    graphs[on] = capture(launch, args.per)
             if args.single_pass:   # True: single pass, False: the 3-pass weight-resident kernel
                 ops.set_conv1x1(True)
                 graphs = {False: graphs[True], True: capture(setup(B, H, W, Cin, Cout, form, g, single=True)[0],

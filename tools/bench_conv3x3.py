@@ -12,8 +12,11 @@ With --single-pass, each forward form also runs on ops.conv2d_tc_f16x1 (single-p
 the two alternating window by window, and the single-pass share of the fp16 peak counts 1 x the algorithmic FLOPs.
 With --train, the single-pass calls are the training precision "fp16" ones: the statistics forms keep their epilogue
 statistics and the data gradients run too, with their power-of-two input scale.
+With --half-io, each forward form (without statistics) runs on the single-pass kernel with fp32 activations against the
+same kernel with fp16 activations (ops.conv2d_tc_f16x1_io: fp16 x, residual and y, inference precision "fp16_act"),
+and the share of the HBM bound (3.35 TB/s) is that of the fp16 form's least bytes (2 per activation read or written).
 
-    python tools/bench_conv3x3.py [--windows 7] [--per 8] [--single-pass [--train]]
+    python tools/bench_conv3x3.py [--windows 7] [--per 8] [--single-pass [--train] | --half-io]
 """
 import argparse
 import collections
@@ -27,6 +30,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 F16_FLOPS = 989e12   # H100 SXM data sheet, dense fp16
+HBM_BYTES_PER_S = 3.35e12   # H100 SXM data sheet
 
 
 def card():
@@ -146,6 +150,7 @@ def main():
     ap.add_argument("--per", type=int, default=8)
     ap.add_argument("--single-pass", action="store_true")
     ap.add_argument("--train", action="store_true")
+    ap.add_argument("--half-io", action="store_true")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "bench_conv3x3 measures on the GPU"
     import fpd_b200  # noqa: F401
@@ -153,6 +158,8 @@ def main():
     shapes = step_shapes()
     if args.single_pass:
         return single_pass(shapes, args)
+    if args.half_io:
+        return half_io(shapes, args)
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
     g = torch.Generator(device="cuda").manual_seed(0)
     print("%-40s %6s %10s %18s %8s" % ("shape (B,H,W,Cin->Cout form)", "x/step", "us", "range", "%F16"))
@@ -221,6 +228,56 @@ def single_pass(shapes, args):
         torch.cuda.empty_cache()
     print("3x3 %s convolutions of one hg_fpd step: 3-pass %.2f ms, single-pass %.2f ms" % (
         "forward and data-gradient" if args.train else "forward", tot3 / 1000.0, tot1 / 1000.0))
+    print("device: %s (name, power limit, SM clock, max SM clock)" % card())
+
+
+def half_io(shapes, args):
+    """The step's forward forms (statistics dropped: eval forwards carry none) on the single-pass kernel with fp32
+    activations against fp16 activations, windows alternating."""
+    from fpd_b200 import ops
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
+    g = torch.Generator(device="cuda").manual_seed(0)
+    print("%-40s %6s %10s %14s %10s %14s %8s %9s %7s" % ("shape (B,H,W,Cin->Cout form)", "x/step", "f32-io us", "range",
+                                                         "f16-io us", "range", "speedup", "least MB", "HBM %"))
+    forms = collections.Counter()
+    for (B, H, W, Cin, Cout, form), n in shapes.items():
+        if not form.startswith("dgrad"):
+            forms[(B, H, W, Cin, Cout, "+".join(f for f in form.split("+") if f not in ("stats", "mask")) or "plain")] += n
+    tot32 = tot16 = 0.0
+    for shape, n in sorted(forms.items(), key=lambda kv: -kv[0][0] * kv[0][1] * kv[0][2] * kv[0][3] * kv[0][4] * kv[1]):
+        B, H, W, Cin, Cout, form = shape
+        launch32 = setup(shape, g, single=True)[1]
+        xs = [torch.randn(B, H, W, Cin, device="cuda", generator=g).half() for _ in range(2)]
+        ys = [torch.empty(B, H, W, Cout, device="cuda", dtype=torch.float16) for _ in range(2)]
+        res = [torch.randn(B, H, W, Cout, device="cuda", generator=g).half() for _ in range(2)] if "res" in form else None
+        w1, _ = ops.weight_prep_f16(torch.randn(Cout, Cin, 3, 3, device="cuda", generator=g) * 0.05, split=False)
+        kw = {}
+        if "bn" in form:
+            kw.update(mean=torch.randn(Cin, device="cuda", generator=g), scale=torch.rand(Cin, device="cuda", generator=g),
+                      shift=torch.randn(Cin, device="cuda", generator=g), relu=True)
+        if "bias" in form:
+            kw["bias"] = torch.randn(Cout, device="cuda", generator=g)
+
+        def launch16(i):
+            ops.conv2d_tc_f16x1_io(xs[i % 2], w1, 3, residual=res[i % 2] if res else None, out=ys[i % 2],
+                                   out_dtype=torch.float16, **kw)
+        graphs = [capture(launch32, args.per), capture(launch16, args.per)]
+        times = [[], []]
+        for _ in range(args.windows):
+            for i, gr in enumerate(graphs):
+                times[i].append(window(gr, args.per, flush))
+        med = [sorted(t)[len(t) // 2] for t in times]
+        tot32 += n * med[0]
+        tot16 += n * med[1]
+        nbytes = 2 * B * H * W * (Cin + Cout * (2 if res else 1))
+        print("%-40s %6d %10.1f %14s %10.1f %14s %7.2fx %9.1f %6.0f%%" % (
+            "%d,%d,%d,%d->%d %s" % (B, H, W, Cin, Cout, form), n, med[0], "%.1f-%.1f" % (min(times[0]), max(times[0])),
+            med[1], "%.1f-%.1f" % (min(times[1]), max(times[1])), med[0] / med[1], nbytes / 1e6,
+            100.0 * nbytes / HBM_BYTES_PER_S * 1e6 / med[1]), flush=True)
+        del graphs
+        torch.cuda.empty_cache()
+    print("3x3 forward convolutions of one hg_fpd step, single pass: fp32 activations %.2f ms, fp16 activations %.2f ms"
+          % (tot32 / 1000.0, tot16 / 1000.0))
     print("device: %s (name, power limit, SM clock, max SM clock)" % card())
 
 

@@ -1,5 +1,6 @@
-"""Inference precision "fp32" (3xFP16 / 3xTF32, the default) against "fp16" (single-pass FP16,
-engine.set_inference_precision) on the benchmark workloads, the two alternating window by window:
+"""Inference precisions "fp32" (3xFP16 / 3xTF32, the default), "fp16" (single-pass FP16) and "fp16_act" (single-pass
+FP16 with fp16 activation storage; engine.set_inference_precision) on the benchmark workloads, alternating window by
+window:
 
   hg_infer      hourglass s4 f128 flip-test inference (FlipTestInference graph), batch 128
   hrnet_infer   HRNet-w32 flip test, 256x192, batch 24
@@ -7,10 +8,11 @@ engine.set_inference_precision) on the benchmark workloads, the two alternating 
   hg_fpd        FPDTrainStep, student s4 f128 + teacher s8 f256 in the given precision, batch 32
   hrnet_fpd     FPDTrainStep, student w32 + teacher w48, batch 24
 
-Prints ms per call, median (min-max) over the windows, and, for the inference workloads, the arg-max agreement of the
-two precisions on the timed batch, with the card's name, power limit and SM clock.
+Prints ms per call, median (min-max) over the windows, the speed-up of each reduced precision over "fp32", and, for the
+inference workloads, the arg-max agreement of each with "fp32" on the timed batch, with the card's name, power limit
+and SM clock.
 
-    python tools/bench_infer_precision.py [--windows 7] [--steps 10] [--only hg_infer,...]
+    python tools/bench_infer_precision.py [--windows 7] [--steps 10] [--only hg_infer,...] [--modes fp32,fp16,fp16_act]
 """
 import argparse
 import os
@@ -55,7 +57,9 @@ def main():
     ap.add_argument("--windows", type=int, default=7)
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--only", default="hg_infer,hrnet_infer,diag_teacher,hg_fpd,hrnet_fpd")
+    ap.add_argument("--modes", default="fp32,fp16,fp16_act")
     args = ap.parse_args()
+    modes = args.modes.split(",")
     import fpd_b200  # noqa: F401
     from fpd_b200.engine import set_inference_precision
     assert torch.cuda.is_available(), "bench_infer_precision needs a CUDA device"
@@ -63,9 +67,9 @@ def main():
     print("device: %s (name, power limit, SM clock, max SM clock)" % card())
     for name in args.only.split(","):
         net, run, outputs = workload(name, dev)
-        times = {"fp32": [], "fp16": []}
+        times = {m: [] for m in modes}
         outs = {}
-        for prec in ("fp32", "fp16"):       # warm-up: capture each precision's graph once
+        for prec in modes:                  # warm-up: capture each precision's graph once
             set_inference_precision(net, prec)
             for _ in range(3):
                 run()
@@ -73,7 +77,7 @@ def main():
             if outputs is not None:
                 outs[prec] = outputs()
         for _ in range(args.windows):
-            for prec in ("fp32", "fp16"):
+            for prec in modes:
                 set_inference_precision(net, prec)
                 run()                         # the switch re-captures: keep that out of the window
                 torch.cuda.synchronize()
@@ -84,16 +88,19 @@ def main():
                 e1.record()
                 torch.cuda.synchronize()
                 times[prec].append(e0.elapsed_time(e1) / args.steps)
+        med = {m: sorted(times[m])[len(times[m]) // 2] for m in modes}
         line = name
-        for prec in ("fp32", "fp16"):
+        for prec in modes:
             t = sorted(times[prec])
-            line += "  %s %.2f ms (%.2f-%.2f)" % (prec, t[len(t) // 2], t[0], t[-1])
-        line += "  speed-up %.2fx" % (sorted(times["fp32"])[len(t) // 2] / sorted(times["fp16"])[len(t) // 2])
+            line += "  %s %.2f ms (%.2f-%.2f)" % (prec, med[prec], t[0], t[-1])
+        for prec in modes[1:]:
+            line += "  %s speed-up %.2fx" % (prec, med[modes[0]] / med[prec])
         if outputs is not None:
-            (i32, m32), (i16, m16) = outs["fp32"], outs["fp16"]
-            same = (i32 == i16).float().mean().item()
-            line += "  arg-max identical %.2f %% of (b, j), max |dmaxval| %.2e" % (
-                100 * same, (m32 - m16).abs().max().item())
+            i32, m32 = outs[modes[0]]
+            for prec in modes[1:]:
+                i16, m16 = outs[prec]
+                line += "  %s arg-max identical %.2f %% of (b, j), max |dmaxval| %.2e" % (
+                    prec, 100 * (i32 == i16).float().mean().item(), (m32 - m16).abs().max().item())
         print(line, flush=True)
         set_inference_precision(net, "fp32")
         del net, run, outputs
