@@ -14,7 +14,7 @@ OUT = os.path.join(HERE, "libfpd_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
          "--expt-relaxed-constexpr", "-Xptxas", "-v"]
-SOURCES = ["api.cu", "conv_wgmma.cu", "conv_simt.cu", "elementwise.cu", "loss.cu", "decode.cu", "nms.cu", "adam.cu", "augment.cu"]
+SOURCES = ["conv_wgmma.cu", "conv_simt.cu", "elementwise.cu", "loss.cu", "decode.cu", "nms.cu", "adam.cu", "augment.cu"]
 
 
 def _newer(a, b):
@@ -24,7 +24,7 @@ def _newer(a, b):
 def build(force=False, verbose=False):
     bdir = os.path.join(CSRC, "_build")
     os.makedirs(bdir, exist_ok=True)
-    headers = [os.path.join(CSRC, h) for h in ("common.cuh", "kernels.h", "wgmma.cuh")] + [
+    headers = [os.path.join(CSRC, h) for h in ("common.cuh", "wgmma.cuh")] + [
         os.path.join(HERE, "..", "include", "fpd_b200.h")]
     hdr_m = max(os.path.getmtime(h) for h in headers)
     jobs = []

@@ -4,7 +4,6 @@
 //   m = b1*m + (1-b1)*g ; v = b2*v + (1-b2)*g*g
 //   p -= (lr / (1-b1^t)) * m / (sqrt(v)/sqrt(1-b2^t) + eps)
 #include "common.cuh"
-#include "kernels.h"
 
 namespace fpd {
 namespace {
@@ -24,9 +23,14 @@ __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, 
   }
 }
 }  // namespace
+}  // namespace fpd
 
-int adam_flat(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, int64_t n, float lr, float beta1,
-              float beta2, float eps, float weight_decay, int step, float grad_scale, cudaStream_t stream) {
+using namespace fpd;
+
+extern "C" {
+
+int fpd_adam_flat(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, int64_t n, float lr, float beta1,
+                  float beta2, float eps, float weight_decay, int step, float grad_scale, fpd_stream_t stream) {
   FPD_REQUIRE(step >= 1, "adam_flat: step must be >= 1");
   const double bc1 = 1.0 - pow((double)beta1, (double)step);
   const double bc2 = 1.0 - pow((double)beta2, (double)step);
@@ -38,4 +42,5 @@ int adam_flat(float* param, const float* grad, float* exp_avg, float* exp_avg_sq
   FPD_LAUNCH_CHECK();
   return FPD_OK;
 }
-}  // namespace fpd
+
+}  // extern "C"

@@ -8,7 +8,6 @@
 #include <cmath>
 
 #include "common.cuh"
-#include "kernels.h"
 
 namespace fpd {
 namespace {
@@ -19,6 +18,7 @@ constexpr int kInterBits = 5;                                   // cv2 INTER_BIT
 constexpr int kRoundDelta = (1 << kAbBits) / (1 << kInterBits) / 2;
 constexpr double kAbScale = 1 << kAbBits;
 constexpr int kMaxImageSide = 32767;                            // cv2 keeps integer tap positions in int16
+constexpr int kCropDescLen = 7;                                 // byte offset, region x, y, w, h, image w, h
 
 struct Norm {
   float mean[3], std[3];
@@ -68,10 +68,15 @@ double fixed_extent(double a, double b, int tmax) {
 }
 
 }  // namespace
+}  // namespace fpd
 
-int crop_affine_normalize(const uint8_t* src, size_t src_bytes, const int64_t* desc, const double* inv,
-                          const int64_t* desc_host, const double* inv_host, const float* mean_std_host, float* out, int N,
-                          int out_h, int out_w, cudaStream_t stream) {
+using namespace fpd;
+
+extern "C" {
+
+int fpd_crop_affine_normalize(const uint8_t* src, size_t src_bytes, const int64_t* desc, const double* inv,
+                              const int64_t* desc_host, const double* inv_host, const float* mean_std_host, float* out,
+                              int N, int out_h, int out_w, fpd_stream_t stream) {
   FPD_REQUIRE(N >= 0, "crop_affine_normalize: N=%d < 0", N);
   FPD_REQUIRE(out_h >= 1 && out_w >= 1, "crop_affine_normalize: empty output %dx%d", out_h, out_w);
   FPD_REQUIRE(N <= 65535 && (int64_t)out_h * out_w <= (1 << 24),
@@ -114,4 +119,4 @@ int crop_affine_normalize(const uint8_t* src, size_t src_bytes, const int64_t* d
   return FPD_OK;
 }
 
-}  // namespace fpd
+}  // extern "C"

@@ -7,16 +7,14 @@
 #include <cstdio>
 #include <type_traits>
 
+#include "../../include/fpd_b200.h"
+
 namespace fpd {
 
 // ------------------------------------------------------------------------------------------------
-// error plumbing (thread-local last-error string; see api.cu)
+// error plumbing (thread-local last-error string, return codes of fpd_b200.h; see elementwise.cu)
 // ------------------------------------------------------------------------------------------------
 void set_last_error(const char* fmt, ...);
-#define FPD_OK 0
-#define FPD_ERR_INVALID -1
-#define FPD_ERR_CUDA -2
-#define FPD_ERR_UNSUPPORTED -3
 
 #define FPD_CUDA_CHECK(expr)                                                                       \
   do {                                                                                             \
@@ -48,6 +46,12 @@ void count_launch();
 // flight for HBM; fixed caps keep the reductions' partial buffers, and so their summation order, independent of the
 // device they run on).
 constexpr int kNumSMs = 132;
+// SMs of the current device (kNumSMs when it cannot be queried): the persistent grids of the tensor-core kernels
+int device_sm_count();
+
+// 3xFP16 and single-pass FP16 weights are stored as __half of w * 2^kF16WeightScaleLog2 (fpd_weight_prep_f16); the
+// convolution epilogues multiply by 2^-kF16WeightScaleLog2
+constexpr int kF16WeightScaleLog2 = 8;
 
 // ------------------------------------------------------------------------------------------------
 // numeric helpers

@@ -9,7 +9,6 @@
 // read-only path (neighbouring threads share pixels, so they hit L1). The weight gradient is a two-stage,
 // fixed-order (deterministic) reduction: per-CTA partials over a pixel chunk, then a sum over chunks.
 #include "common.cuh"
-#include "kernels.h"
 
 namespace fpd {
 namespace {
@@ -263,9 +262,14 @@ inline WgradGeom wgrad_geom(int64_t P, int Cin, int Cout, int k) {
 }
 
 }  // namespace
+}  // namespace fpd
 
-int conv_simt_fwd(const float* x, const float* w_oihw, const float* bias, const float* residual, float* y, int B,
-                  int H, int W, int Cin, int Cout, int k, int stride, int pad, cudaStream_t stream) {
+using namespace fpd;
+
+extern "C" {
+
+int fpd_conv2d_simt_fwd(const float* x, const float* w_oihw, const float* bias, const float* residual, float* y,
+                        int B, int H, int W, int Cin, int Cout, int k, int stride, int pad, fpd_stream_t stream) {
   FPD_REQUIRE(k >= 1 && stride >= 1 && pad >= 0, "conv_simt_fwd: bad geometry");
   const int Ho = (H + 2 * pad - k) / stride + 1, Wo = (W + 2 * pad - k) / stride + 1;
   const int CoutP = (Cout + 3) & ~3;
@@ -287,8 +291,8 @@ int conv_simt_fwd(const float* x, const float* w_oihw, const float* bias, const 
   return FPD_OK;
 }
 
-int conv_simt_dgrad(const float* dy, const float* w_oihw, float* dx, int B, int H, int W, int Cin, int Cout, int k,
-                    int stride, int pad, cudaStream_t stream) {
+int fpd_conv2d_simt_dgrad(const float* dy, const float* w_oihw, float* dx, int B, int H, int W, int Cin, int Cout,
+                          int k, int stride, int pad, fpd_stream_t stream) {
   const int Ho = (H + 2 * pad - k) / stride + 1, Wo = (W + 2 * pad - k) / stride + 1;
   const int CinP = (Cin + 3) & ~3;
   const int64_t n = (int64_t)B * H * W * (CinP / 4);
@@ -309,13 +313,14 @@ int conv_simt_dgrad(const float* dy, const float* w_oihw, float* dx, int B, int 
   return FPD_OK;
 }
 
-size_t conv_simt_wgrad_workspace_bytes(int B, int H, int W, int Cin, int Cout, int k, int stride, int pad) {
+size_t fpd_conv2d_simt_wgrad_workspace_bytes(int B, int H, int W, int Cin, int Cout, int k, int stride, int pad) {
   const int Ho = (H + 2 * pad - k) / stride + 1, Wo = (W + 2 * pad - k) / stride + 1;
   return wgrad_geom((int64_t)B * Ho * Wo, Cin, Cout, k).bytes;
 }
 
-int conv_simt_wgrad(const float* x, const float* dy, float* dw_oihw, float scale, int B, int H, int W, int Cin,
-                    int Cout, int k, int stride, int pad, void* workspace, size_t ws_bytes, cudaStream_t stream) {
+int fpd_conv2d_simt_wgrad(const float* x, const float* dy, float* dw_oihw, float scale, int B, int H, int W,
+                          int Cin, int Cout, int k, int stride, int pad, void* workspace, size_t ws_bytes,
+                          fpd_stream_t stream) {
   const int Ho = (H + 2 * pad - k) / stride + 1, Wo = (W + 2 * pad - k) / stride + 1;
   const int64_t P = (int64_t)B * Ho * Wo;
   const WgradGeom g = wgrad_geom(P, Cin, Cout, k);
@@ -338,4 +343,4 @@ int conv_simt_wgrad(const float* x, const float* dy, float* dw_oihw, float scale
   return FPD_OK;
 }
 
-}  // namespace fpd
+}  // extern "C"

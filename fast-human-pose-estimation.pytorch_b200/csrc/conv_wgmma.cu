@@ -1,10 +1,10 @@
 // conv_wgmma.cu -- implicit-GEMM convolution and convolution weight gradient on the sm_90a warpgroup tensor cores
 // (wgmma.mma_async), operand preparation fused in.
 //
-// Forward (conv_tc_ts_* and conv_tc_h_*): y = conv(relu?((x - mean) * scale + shift)) (+ bias, + residual, ReLU mask),
-// stride 1, "same" padding, NHWC activations, weights [tap][Cout][Cin] as hi/lo pairs (3xTF32: fp32 containers from
-// weight_prep; 3xFP16: __half from weight_prep_f16, pre-scaled by 2^kF16WeightScaleLog2). BatchNorm2d-apply + ReLU +
-// Conv2d of lib/models/hourglass.py:34-44: padding positions are zero AFTER the affine.
+// Forward (fpd_conv2d_tc_ts, fpd_conv2d_tc_h*): y = conv(relu?((x - mean) * scale + shift)) (+ bias, + residual, ReLU
+// mask), stride 1, "same" padding, NHWC activations, weights [tap][Cout][Cin] as hi/lo pairs (3xTF32: fp32 containers
+// from fpd_weight_prep; 3xFP16: __half from fpd_weight_prep_f16, pre-scaled by 2^kF16WeightScaleLog2). BatchNorm2d-apply
+// + ReLU + Conv2d of lib/models/hourglass.py:34-44: padding positions are zero AFTER the affine.
 //   GEMM: M = 128 output pixels (two warpgroups x 64 rows), N = one Cout slice (<= 128), K = taps x Cin in steps of one
 //   128-byte operand row (32 tf32 or 64 fp16 channels of one tap). Every thread loads its share of the raw x rows into
 //   registers one K step ahead, applies the affine + ReLU + hi/lo split and stores the result into the swizzled
@@ -13,16 +13,16 @@
 //   products are summed into the fp32 accumulators outside the tensor core (see mma_row).
 //   Split operands: acc += A_lo * B_hi + A_hi * B_lo + A_hi * B_hi (the lo * lo term is below fp32 rounding).
 //   Optional epilogue statistics: per output channel {sum (y - pivot), sum (y - pivot)^2} in fp64, per-warp shared
-//   accumulators merged in a fixed order (deterministic), one [Cout][2] block per CTA for bn_finalize_sums.
+//   accumulators merged in a fixed order (deterministic), one [Cout][2] block per CTA for fpd_bn_finalize_sums.
 //   3x3 with 3xFP16 operands (conv_halo_kernel, where conv_plan finds it fits in shared memory): the same GEMM
 //   with the A operand of a tile loaded and transformed once into a halo in shared memory and fed from registers.
-//   Single-pass FP16 (conv_f16x1_*): the halo and 1x1 weight-resident kernels with kSplit = false
+//   Single-pass FP16 (fpd_conv2d_tc_f16x1*): the halo and 1x1 weight-resident kernels with kSplit = false
 //   (conv_halo_f16x1_kernel, pw_conv_f16x1_kernel), one MMA per k16 straight into the accumulators. Inference calls,
 //   and the training precision "fp16": forward calls with epilogue statistics, data gradients with in_scale. Their
 //   TIn / TOut template parameters (float or __half) are the activation types of x and of y with the residual: the
-//   inference precision "fp16_act" (conv_f16x1_io_launch) stores activations in fp16.
+//   inference precision "fp16_act" (fpd_conv2d_tc_f16x1_io) stores activations in fp16.
 //
-// Weight gradient (wgrad_tc_*):
+// Weight gradient (fpd_conv2d_wgrad_tc*):
 //   dW[co][ci][tap] = scale * sum_{pixels p} dY[p][co] * A[p (+) tap][ci],  A = relu?((x - mean) * scale + shift)
 //   GEMM: M = 128 output channels, N = one input-channel tile, K = pixels in steps of 32, one tap per CTA, split-K over
 //   pixel ranges. tf32 wgmma takes K-major operands only, so the transform threads write both operands transposed
@@ -38,7 +38,6 @@
 #include <type_traits>
 
 #include "common.cuh"
-#include "kernels.h"
 #include "wgmma.cuh"
 
 namespace fpd {
@@ -930,6 +929,15 @@ __global__ void __launch_bounds__(kThreads, 1) pw_conv_f16x1_kernel(const __grid
   pw_conv_body<kN, false, TIn, TOut>(p);
 }
 
+// Output channels are processed in slices of nt columns: the widest divisor of Cout that is a multiple of 16 and at
+// most 128 (one wgmma N per slice; the accumulators of a 64 x 128 warpgroup tile take 64 registers per thread).
+int conv_tc_ts_slice(int Cout) {
+  if (Cout <= 128) return Cout % 16 == 0 ? Cout : 0;
+  for (int nt = 128; nt >= 16; nt -= 16)
+    if (Cout % nt == 0) return nt;
+  return 0;
+}
+
 bool conv_shape_ok(int Cin, int Cout, int ksize, int f16, int max_cin, int max_cout) {
   return (ksize == 1 || ksize == 3) && Cin >= 4 && Cin <= max_cin && Cin % (f16 ? 8 : 4) == 0 && Cout >= 16 &&
          Cout <= max_cout && Cout % 16 == 0 && conv_tc_ts_slice(Cout) > 0;
@@ -1071,9 +1079,9 @@ struct ConvPlan {
 //   1x1: the weight-resident kernel (pw_conv_wgmma_kernel, pw_conv_f16x1_kernel) wherever the slice's weights, the A
 //   stages and the statistics scratch fit; only the single-pass kernel carries statistics.
 //   Everything else: the staged conv_wgmma_kernel.
-// The halo and 1x1 kernels take the 3xFP16 calls (f16 with w_lo), under the set_conv_halo / set_conv1x1 toggles, and
-// the single-pass calls (conv_f16x1_*), regardless of the toggles. TF32 calls and conv_tc_h's fp16 calls without w_lo
-// stay on the staged kernel.
+// The halo and 1x1 kernels take the 3xFP16 calls (f16 with w_lo), under the fpd_set_conv_halo / fpd_set_conv1x1 toggles,
+// and the single-pass calls (fpd_conv2d_tc_f16x1*), regardless of the toggles. TF32 calls and fpd_conv2d_tc_h's fp16
+// calls without w_lo stay on the staged kernel.
 ConvPlan conv_plan(ConvParams& p, bool f16, bool single_pass, bool stats, int num_sms) {
   const bool split = p.passes == 3;
   const bool fast = single_pass || (f16 && split);
@@ -1121,12 +1129,12 @@ int with_act_types(bool x_f16, bool y_f16, F&& f) {
 }
 
 // Every forward convolution: checks the call, plans it and launches the planned kernel. w_lo == nullptr: hi operands
-// only; single_pass: a conv_f16x1_* call. x_f16 / y_f16: x, or y and the residual, are __half (single-pass calls on the
-// halo and 1x1 kernels without statistics only).
+// only; single_pass: an fpd_conv2d_tc_f16x1* call. x_f16 / y_f16: x, or y and the residual, are __half (single-pass
+// calls on the halo and 1x1 kernels without statistics only).
 int conv_launch(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift, int pre_relu,
                 const void* w_hi, const void* w_lo, int f16, bool single_pass, const float* bias,
                 const float* residual, const float* relu_mask, float* y, float out_scale, const float* in_scale, int B,
-                int H, int W, int Cin, int Cout, int ksize, int num_sms, cudaStream_t stream, double* stat_part,
+                int H, int W, int Cin, int Cout, int ksize, cudaStream_t stream, double* stat_part,
                 const float* stat_pivot, bool x_f16 = false, bool y_f16 = false) {
   FPD_REQUIRE(x && w_hi && y, "conv_wgmma: null operand");
   FPD_REQUIRE((double)B * H * W * Cout < 4294967296.0, "conv_wgmma: output has 2^32 or more elements");
@@ -1134,7 +1142,7 @@ int conv_launch(const float* x, const float* pre_mean, const float* pre_scale, c
   FPD_REQUIRE(pre_scale != nullptr || pre_mean == nullptr, "conv_wgmma: pre_mean needs pre_scale/pre_shift");
   FPD_REQUIRE(stat_part == nullptr || Cout <= kMaxStatCout, "conv_wgmma: statistics need Cout <= %d", kMaxStatCout);
   ConvParams p = conv_shape_params(B, H, W, Cin, Cout, ksize, f16, w_lo ? 3 : 1);
-  const ConvPlan pl = conv_plan(p, f16, single_pass, stat_part != nullptr, num_sms);
+  const ConvPlan pl = conv_plan(p, f16, single_pass, stat_part != nullptr, device_sm_count());
   FPD_REQUIRE(pl.kernel != kConvNone, "conv_wgmma: shared memory plan %zu B too large", pl.smem);
   FPD_REQUIRE(!(x_f16 || y_f16) || (single_pass && !w_lo && !stat_part && (pl.kernel == kConvHalo || pl.kernel == kConvPw)),
               "conv_wgmma: half-precision activations need a single-pass halo or 1x1 launch without statistics");
@@ -1173,6 +1181,41 @@ int conv_launch(const float* x, const float* pre_mean, const float* pre_scale, c
 bool conv_f16x1_supported(int B, int H, int W, int Cin, int Cout, int ksize, bool stats) {
   return conv_shape_ok(Cin, Cout, ksize, 1, kMaxCinH, 2048) && B >= 1 && H >= 1 && W >= 1 &&
          (double)B * H * W * Cout < 4294967296.0 && (!stats || Cout <= kMaxStatCout);
+}
+
+// The checked 3xTF32 / 3xFP16 forward of fpd_conv2d_tc_h and fpd_conv2d_tc_h_stats.
+int conv_tc_h_launch(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
+                     int pre_relu, const void* w_hi, const void* w_lo, int f16, const float* bias,
+                     const float* residual, const float* relu_mask, float* y, float out_scale, const float* in_scale,
+                     int B, int H, int W, int Cin, int Cout, int ksize, cudaStream_t stream, double* stat_part,
+                     const float* stat_pivot) {
+  FPD_REQUIRE(fpd_conv2d_tc_h_supported(Cin, Cout, ksize, H, W, f16),
+              "conv_tc_h: unsupported shape Cin=%d Cout=%d k=%d H=%d W=%d f16=%d", Cin, Cout, ksize, H, W, f16);
+  return conv_launch(x, pre_mean, pre_scale, pre_shift, pre_relu, w_hi, w_lo, f16, false, bias, residual, relu_mask,
+                     y, out_scale, in_scale, B, H, W, Cin, Cout, ksize, stream, stat_part, stat_pivot);
+}
+
+// The kernel (ConvKernel) a single-pass call with (stats != 0) or without statistics runs on, and in *stat_blocks
+// (nullable) the partial blocks a statistics launch writes: 0 without statistics or when unsupported.
+int conv_f16x1_kernel(int B, int H, int W, int Cin, int Cout, int ksize, int stats, int num_sms, int* stat_blocks) {
+  if (stat_blocks) *stat_blocks = 0;
+  if (!conv_f16x1_supported(B, H, W, Cin, Cout, ksize, stats != 0)) return 0;
+  ConvParams p = conv_shape_params(B, H, W, Cin, Cout, ksize, 1, 1);
+  const ConvPlan pl = conv_plan(p, true, true, stats != 0, num_sms);
+  if (pl.kernel != kConvNone && stats && stat_blocks) *stat_blocks = pl.grid;
+  return pl.kernel;
+}
+
+// The checked single-pass FP16 forward of fpd_conv2d_tc_f16x1 and fpd_conv2d_tc_f16x1_train.
+int conv_f16x1_launch(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
+                      int pre_relu, const void* w, const float* bias, const float* residual, const float* relu_mask,
+                      float* y, float out_scale, const float* in_scale, int B, int H, int W, int Cin, int Cout,
+                      int ksize, cudaStream_t stream, double* stat_part, const float* stat_pivot) {
+  FPD_REQUIRE(conv_f16x1_supported(B, H, W, Cin, Cout, ksize, stat_part != nullptr),
+              "conv_f16x1: unsupported shape B=%d H=%d W=%d Cin=%d Cout=%d k=%d (statistics: %d, Cout <= %d)", B, H,
+              W, Cin, Cout, ksize, stat_part != nullptr, kMaxStatCout);
+  return conv_launch(x, pre_mean, pre_scale, pre_shift, pre_relu, w, nullptr, 1, true, bias, residual, relu_mask, y,
+                     out_scale, in_scale, B, H, W, Cin, Cout, ksize, stream, stat_part, stat_pivot);
 }
 
 // ================================================= weight gradient =================================================
@@ -1571,10 +1614,10 @@ WgradPlan wgrad_plan(int B, int H, int W, int Cin, int Cout, int ksize, int num_
 
 std::atomic<int> g_wgrad_halo{1};
 
-// wgrad_halo_kernel takes every 3x3 shape of wgrad_tc_supported, and the 1x1 shapes whose input channels fill whole
-// 64-row warpgroups and whose Cout is 32 or 64, where wgrad_wgmma_kernel's 128-row tile is at most half used. (At
-// Cout >= 128 that tile is full, and the per-tap kernel was faster on the H100: 128 -> 128 at 64x64, batch 32, 128.5
-// against 151.9 µs.)
+// wgrad_halo_kernel takes every 3x3 shape of fpd_conv2d_wgrad_tc_supported, and the 1x1 shapes whose input channels
+// fill whole 64-row warpgroups and whose Cout is 32 or 64, where wgrad_wgmma_kernel's 128-row tile is at most half
+// used. (At Cout >= 128 that tile is full, and the per-tap kernel was faster on the H100: 128 -> 128 at 64x64, batch
+// 32, 128.5 against 151.9 µs.)
 bool wgrad_halo_ok(int Cin, int Cout, int ksize) {
   if (!g_wgrad_halo.load(std::memory_order_relaxed)) return false;
   if (ksize == 3) return true;
@@ -1608,83 +1651,92 @@ int wgrad_halo_launch(WgradParams p, const WgradPlan& pl, cudaStream_t stream) {
 }
 
 }  // namespace
+}  // namespace fpd
+
+using namespace fpd;
+
+extern "C" {
 
 // ------------------------------------------------- forward entry points -------------------------------------------------
 
-// Output channels are processed in slices of nt columns: the widest divisor of Cout that is a multiple of 16 and at
-// most 128 (one wgmma N per slice; the accumulators of a 64 x 128 warpgroup tile take 64 registers per thread).
-int conv_tc_ts_slice(int Cout) {
-  if (Cout <= 128) return Cout % 16 == 0 ? Cout : 0;
-  for (int nt = 128; nt >= 16; nt -= 16)
-    if (Cout % nt == 0) return nt;
-  return 0;
+int fpd_conv2d_tc_ts_supported(int Cin, int Cout, int ksize) {
+  return conv_shape_ok(Cin, Cout, ksize, 0, kMaxCinTs, 1024);
 }
 
-bool conv_tc_ts_supported(int Cin, int Cout, int ksize) { return conv_shape_ok(Cin, Cout, ksize, 0, kMaxCinTs, 1024); }
-
-int conv_tc_ts_launch(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
-                      int pre_relu, const float* w_hi, const float* w_lo, const float* bias, const float* residual,
-                      const float* relu_mask, float* y, float out_scale, int B, int H, int W, int Cin, int Cout,
-                      int ksize, int num_sms, cudaStream_t stream) {
-  FPD_REQUIRE(conv_tc_ts_supported(Cin, Cout, ksize), "conv_tc_ts: unsupported shape Cin=%d Cout=%d k=%d", Cin, Cout,
-              ksize);
+int fpd_conv2d_tc_ts(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
+                     int pre_relu, const float* w_hi, const float* w_lo, const float* bias, const float* residual,
+                     const float* relu_mask, float* y, float out_scale, int B, int H, int W, int Cin, int Cout,
+                     int ksize, fpd_stream_t stream) {
+  FPD_REQUIRE(fpd_conv2d_tc_ts_supported(Cin, Cout, ksize), "conv_tc_ts: unsupported shape Cin=%d Cout=%d k=%d", Cin,
+              Cout, ksize);
   return conv_launch(x, pre_mean, pre_scale, pre_shift, pre_relu, w_hi, w_lo, 0, false, bias, residual, relu_mask, y,
-                     out_scale, nullptr, B, H, W, Cin, Cout, ksize, num_sms, stream, nullptr, nullptr);
+                     out_scale, nullptr, B, H, W, Cin, Cout, ksize, stream, nullptr, nullptr);
 }
 
-int set_conv1x1(int enabled) { return g_conv1x1.exchange(enabled ? 1 : 0); }
-int set_conv_halo(int enabled) { return g_conv_halo.exchange(enabled ? 1 : 0); }
+int fpd_set_conv1x1(int enabled) { return g_conv1x1.exchange(enabled ? 1 : 0); }
+int fpd_set_conv_halo(int enabled) { return g_conv_halo.exchange(enabled ? 1 : 0); }
 
-bool conv_tc_h_supported(int Cin, int Cout, int ksize, int H, int W, int f16) {
+int fpd_conv2d_tc_h_supported(int Cin, int Cout, int ksize, int H, int W, int f16) {
   (void)H; (void)W;
   return conv_shape_ok(Cin, Cout, ksize, f16, kMaxCinH, 2048);
 }
 
-int conv_tc_h_stats_grid(int B, int H, int W, int Cin, int Cout, int ksize, int f16, int num_sms) {
-  if (!conv_tc_h_supported(Cin, Cout, ksize, H, W, f16) || Cout > kMaxStatCout) return 0;
+int fpd_conv2d_tc_h_stats_blocks(int B, int H, int W, int Cin, int Cout, int ksize, int f16) {
+  if (!fpd_conv2d_tc_h_supported(Cin, Cout, ksize, H, W, f16) || Cout > kMaxStatCout) return 0;
   ConvParams p = conv_shape_params(B, H, W, Cin, Cout, ksize, f16, 3);   // the grid is the same with hi operands only
-  const ConvPlan pl = conv_plan(p, f16, false, true, num_sms);
+  const ConvPlan pl = conv_plan(p, f16, false, true, device_sm_count());
   return pl.kernel != kConvNone ? pl.grid : 0;
 }
 
-int conv_tc_h_launch(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
-                     int pre_relu, const void* w_hi, const void* w_lo, int f16, const float* bias,
-                     const float* residual, const float* relu_mask, float* y, float out_scale, const float* in_scale,
-                     int B, int H, int W, int Cin, int Cout, int ksize, int num_sms, cudaStream_t stream,
-                     double* stat_part, const float* stat_pivot) {
-  FPD_REQUIRE(conv_tc_h_supported(Cin, Cout, ksize, H, W, f16),
-              "conv_tc_h: unsupported shape Cin=%d Cout=%d k=%d H=%d W=%d f16=%d", Cin, Cout, ksize, H, W, f16);
-  return conv_launch(x, pre_mean, pre_scale, pre_shift, pre_relu, w_hi, w_lo, f16, false, bias, residual, relu_mask,
-                     y, out_scale, in_scale, B, H, W, Cin, Cout, ksize, num_sms, stream, stat_part, stat_pivot);
+int fpd_conv2d_tc_h(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
+                    int pre_relu, const void* w_hi, const void* w_lo, int f16, const float* bias,
+                    const float* residual, const float* relu_mask, float* y, float out_scale, const float* in_scale,
+                    int B, int H, int W, int Cin, int Cout, int ksize, fpd_stream_t stream) {
+  return conv_tc_h_launch(x, pre_mean, pre_scale, pre_shift, pre_relu, w_hi, w_lo, f16, bias, residual, relu_mask, y,
+                          out_scale, in_scale, B, H, W, Cin, Cout, ksize, stream, nullptr, nullptr);
 }
 
-int conv_f16x1_kernel(int B, int H, int W, int Cin, int Cout, int ksize, int stats, int num_sms, int* stat_blocks) {
-  if (stat_blocks) *stat_blocks = 0;
-  if (!conv_f16x1_supported(B, H, W, Cin, Cout, ksize, stats != 0)) return 0;
-  ConvParams p = conv_shape_params(B, H, W, Cin, Cout, ksize, 1, 1);
-  const ConvPlan pl = conv_plan(p, true, true, stats != 0, num_sms);
-  if (pl.kernel != kConvNone && stats && stat_blocks) *stat_blocks = pl.grid;
-  return pl.kernel;
+int fpd_conv2d_tc_h_stats(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
+                          int pre_relu, const void* w_hi, const void* w_lo, int f16, const float* bias,
+                          const float* residual, float* y, float out_scale, int B, int H, int W, int Cin, int Cout,
+                          int ksize, double* stat_part, const float* stat_pivot, fpd_stream_t stream) {
+  FPD_REQUIRE(stat_part != nullptr, "fpd_conv2d_tc_h_stats: stat_part is NULL (use fpd_conv2d_tc_h)");
+  return conv_tc_h_launch(x, pre_mean, pre_scale, pre_shift, pre_relu, w_hi, w_lo, f16, bias, residual, nullptr, y,
+                          out_scale, nullptr, B, H, W, Cin, Cout, ksize, stream, stat_part, stat_pivot);
 }
 
-int conv_f16x1_launch(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
-                      int pre_relu, const void* w, const float* bias, const float* residual, const float* relu_mask,
-                      float* y, float out_scale, const float* in_scale, int B, int H, int W, int Cin, int Cout,
-                      int ksize, int num_sms, cudaStream_t stream, double* stat_part, const float* stat_pivot) {
-  FPD_REQUIRE(conv_f16x1_supported(B, H, W, Cin, Cout, ksize, stat_part != nullptr),
-              "conv_f16x1: unsupported shape B=%d H=%d W=%d Cin=%d Cout=%d k=%d (statistics: %d, Cout <= %d)", B, H,
-              W, Cin, Cout, ksize, stat_part != nullptr, kMaxStatCout);
-  return conv_launch(x, pre_mean, pre_scale, pre_shift, pre_relu, w, nullptr, 1, true, bias, residual, relu_mask, y,
-                     out_scale, in_scale, B, H, W, Cin, Cout, ksize, num_sms, stream, stat_part, stat_pivot);
+int fpd_conv2d_tc_f16x1_kernel(int B, int H, int W, int Cin, int Cout, int ksize) {
+  return conv_f16x1_kernel(B, H, W, Cin, Cout, ksize, 0, 0, nullptr);
 }
 
-int conv_f16x1_io_launch(const void* x, int x_f16, const float* pre_mean, const float* pre_scale,
-                         const float* pre_shift, int pre_relu, const void* w, const float* bias, const void* residual,
-                         void* y, int y_f16, float out_scale, int B, int H, int W, int Cin, int Cout, int ksize,
-                         int num_sms, cudaStream_t stream) {
+int fpd_conv2d_tc_f16x1_train_plan(int B, int H, int W, int Cin, int Cout, int ksize, int stats, int* stat_blocks) {
+  return conv_f16x1_kernel(B, H, W, Cin, Cout, ksize, stats, device_sm_count(), stat_blocks);
+}
+
+int fpd_conv2d_tc_f16x1(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
+                        int pre_relu, const void* w, const float* bias, const float* residual, const float* relu_mask,
+                        float* y, float out_scale, int B, int H, int W, int Cin, int Cout, int ksize,
+                        fpd_stream_t stream) {
+  return conv_f16x1_launch(x, pre_mean, pre_scale, pre_shift, pre_relu, w, bias, residual, relu_mask, y, out_scale,
+                           nullptr, B, H, W, Cin, Cout, ksize, stream, nullptr, nullptr);
+}
+
+int fpd_conv2d_tc_f16x1_train(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
+                              int pre_relu, const void* w, const float* bias, const float* residual,
+                              const float* relu_mask, float* y, float out_scale, const float* in_scale, int B, int H,
+                              int W, int Cin, int Cout, int ksize, double* stat_part, const float* stat_pivot,
+                              fpd_stream_t stream) {
+  return conv_f16x1_launch(x, pre_mean, pre_scale, pre_shift, pre_relu, w, bias, residual, relu_mask, y, out_scale,
+                           in_scale, B, H, W, Cin, Cout, ksize, stream, stat_part, stat_pivot);
+}
+
+int fpd_conv2d_tc_f16x1_io(const void* x, int x_f16, const float* pre_mean, const float* pre_scale,
+                           const float* pre_shift, int pre_relu, const void* w, const float* bias, const void* residual,
+                           void* y, int y_f16, float out_scale, int B, int H, int W, int Cin, int Cout, int ksize,
+                           fpd_stream_t stream) {
   FPD_REQUIRE(conv_f16x1_supported(B, H, W, Cin, Cout, ksize, false),
               "conv_f16x1_io: unsupported shape B=%d H=%d W=%d Cin=%d Cout=%d k=%d", B, H, W, Cin, Cout, ksize);
-  const int kind = conv_f16x1_kernel(B, H, W, Cin, Cout, ksize, 0, num_sms, nullptr);
+  const int kind = fpd_conv2d_tc_f16x1_kernel(B, H, W, Cin, Cout, ksize);
   if (kind != kConvHalo && kind != kConvPw) {
     set_last_error("conv_f16x1_io: B=%d H=%d W=%d Cin=%d Cout=%d k=%d runs on the staged kernel, which has no "
                    "half-precision activation form", B, H, W, Cin, Cout, ksize);
@@ -1692,7 +1744,7 @@ int conv_f16x1_io_launch(const void* x, int x_f16, const float* pre_mean, const 
   }
   return conv_launch(static_cast<const float*>(x), pre_mean, pre_scale, pre_shift, pre_relu, w, nullptr, 1, true, bias,
                      static_cast<const float*>(residual), nullptr, static_cast<float*>(y), out_scale, nullptr, B, H, W,
-                     Cin, Cout, ksize, num_sms, stream, nullptr, nullptr, x_f16 != 0, y_f16 != 0);
+                     Cin, Cout, ksize, stream, nullptr, nullptr, x_f16 != 0, y_f16 != 0);
 }
 
 // ---------------------------------------------- weight-gradient entry points ----------------------------------------------
@@ -1700,33 +1752,34 @@ int conv_f16x1_io_launch(const void* x, int x_f16, const float* pre_mean, const 
 // Shapes taken per launch: 3x3 with Cin in {32, 64, 128} and Cout a multiple of 32 up to 256; 1x1 with Cin <= 256 and
 // any Cout % 4 == 0. Wider layers go through ops.conv2d_wgrad_tc_chunked in channel chunks of these sizes, which keeps
 // the per-launch partial-sum workspace (splits x taps x Cin x Cout) small.
-bool wgrad_tc_supported(int Cin, int Cout, int ksize) {
+int fpd_conv2d_wgrad_tc_supported(int Cin, int Cout, int ksize) {
   if (ksize == 3) return (Cin == 32 || Cin == 64 || Cin == 128) && Cout % 32 == 0 && Cout >= 32 && Cout <= 256;
   return ksize == 1 && Cout % 4 == 0 && Cin % 4 == 0 && Cin >= 4 && Cin <= 256;
 }
 
-int set_wgrad_halo(int enabled) { return g_wgrad_halo.exchange(enabled ? 1 : 0); }
+int fpd_set_wgrad_halo(int enabled) { return g_wgrad_halo.exchange(enabled ? 1 : 0); }
 
-bool wgrad_tc3_supported(int H, int W, int Cin, int Cout, int ksize) {
+int fpd_conv2d_wgrad_tc3_supported(int H, int W, int Cin, int Cout, int ksize) {
   (void)H; (void)W;
-  return ksize == 3 && wgrad_tc_supported(Cin, Cout, ksize);
+  return ksize == 3 && fpd_conv2d_wgrad_tc_supported(Cin, Cout, ksize);
 }
 
-size_t wgrad_tc_workspace_bytes(int B, int H, int W, int Cin, int Cout, int ksize, int num_sms) {
-  if (!wgrad_tc_supported(Cin, Cout, ksize)) return 0;
-  const WgradPlan pl = wgrad_plan(B, H, W, Cin, Cout, ksize, num_sms);
+size_t fpd_conv2d_wgrad_tc_workspace_bytes(int B, int H, int W, int Cin, int Cout, int ksize) {
+  if (!fpd_conv2d_wgrad_tc_supported(Cin, Cout, ksize)) return 0;
+  const WgradPlan pl = wgrad_plan(B, H, W, Cin, Cout, ksize, device_sm_count());
   return (size_t)pl.splits * pl.taps * Cin * Cout * sizeof(float);
 }
 
-int wgrad_tc_fused_launch(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
-                          int pre_relu, const float* dy, int passes, float* dw_oihw, float scale, int B, int H, int W,
-                          int Cin, int Cout, int ksize, void* workspace, size_t workspace_bytes, int num_sms,
-                          cudaStream_t stream) {
-  FPD_REQUIRE(wgrad_tc_supported(Cin, Cout, ksize), "wgrad_tc: unsupported shape Cin=%d Cout=%d k=%d", Cin, Cout, ksize);
+int fpd_conv2d_wgrad_tc_fused(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
+                              int pre_relu, const float* dy, int passes, float* dw_oihw, float scale, int B, int H,
+                              int W, int Cin, int Cout, int ksize, void* workspace, size_t workspace_bytes,
+                              fpd_stream_t stream) {
+  FPD_REQUIRE(fpd_conv2d_wgrad_tc_supported(Cin, Cout, ksize), "wgrad_tc: unsupported shape Cin=%d Cout=%d k=%d", Cin,
+              Cout, ksize);
   FPD_REQUIRE(x && dy && dw_oihw, "wgrad_tc: null operand");
   FPD_REQUIRE(passes == 1 || passes == 3, "wgrad_tc_fused: passes must be 1 or 3");
   FPD_REQUIRE((pre_scale == nullptr) == (pre_shift == nullptr), "wgrad_tc_fused: pre_scale/pre_shift come in pairs");
-  const WgradPlan pl = wgrad_plan(B, H, W, Cin, Cout, ksize, num_sms);
+  const WgradPlan pl = wgrad_plan(B, H, W, Cin, Cout, ksize, device_sm_count());
   WgradParams p{};
   p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.Cout = Cout; p.ksize = ksize; p.taps = pl.taps; p.P = B * H * W;
   p.passes = passes;
@@ -1752,4 +1805,4 @@ int wgrad_tc_fused_launch(const float* x, const float* pre_mean, const float* pr
   return FPD_OK;
 }
 
-}  // namespace fpd
+}  // extern "C"

@@ -13,7 +13,6 @@
 // Every floating-point step is an explicitly rounded intrinsic in the order the host (numpy / torch) evaluates it, so
 // the results are bit-identical to lib/core/inference.py::get_final_preds and lib/core/evaluate.py::accuracy.
 #include "common.cuh"
-#include "kernels.h"
 
 namespace fpd {
 namespace {
@@ -176,9 +175,14 @@ __global__ void pck_counts_kernel(const int* __restrict__ idx, const float* __re
 }
 
 }  // namespace
+}  // namespace fpd
 
-int flip_merge_argmax(const float* hm, const float* hm_flip, const int* flip_perm, int shift, float* avg_nhwc,
-                      int* idx, float* maxval, int B, int J, int h, int w, cudaStream_t stream) {
+using namespace fpd;
+
+extern "C" {
+
+int fpd_flip_merge_argmax(const float* hm, const float* hm_flip, const int* flip_perm, int shift, float* avg_nhwc,
+                          int* idx, float* maxval, int B, int J, int h, int w, fpd_stream_t stream) {
   FPD_REQUIRE(J >= 1 && J <= 64, "flip_merge_argmax: J=%d out of range", J);
   const int threads = (512 / J) * J;
   const size_t smem = (size_t)threads * sizeof(Best);
@@ -188,7 +192,7 @@ int flip_merge_argmax(const float* hm, const float* hm_flip, const int* flip_per
   return FPD_OK;
 }
 
-int argmax_nchw(const float* hm, int* idx, float* maxval, int BJ, int hw, cudaStream_t stream) {
+int fpd_argmax_nchw(const float* hm, int* idx, float* maxval, int BJ, int hw, fpd_stream_t stream) {
   const int threads = 256;
   const int blocks = (BJ * 32 + threads - 1) / threads;
   argmax_nchw_kernel<<<blocks, threads, 0, stream>>>(hm, idx, maxval, BJ, hw);
@@ -196,8 +200,8 @@ int argmax_nchw(const float* hm, int* idx, float* maxval, int BJ, int hw, cudaSt
   return FPD_OK;
 }
 
-int final_preds(const float* avg_nhwc, const int* idx, const float* maxval, const double* inv, int post_process,
-                float* preds, int B, int J, int h, int w, cudaStream_t stream) {
+int fpd_final_preds(const float* avg_nhwc, const int* idx, const float* maxval, const double* inv, int post_process,
+                    float* preds, int B, int J, int h, int w, fpd_stream_t stream) {
   FPD_REQUIRE(B >= 0 && J >= 1 && J <= 64, "final_preds: B=%d J=%d out of range", B, J);
   FPD_REQUIRE(h >= 1 && w >= 1, "final_preds: empty %dx%d heat-map", h, w);
   FPD_REQUIRE(!post_process || (h >= 3 && w >= 3), "final_preds: post_process needs a heat-map of at least 3x3, got %dx%d",
@@ -211,8 +215,8 @@ int final_preds(const float* avg_nhwc, const int* idx, const float* maxval, cons
   return FPD_OK;
 }
 
-int pck_counts(const int* idx, const float* maxval, const float* target_nchw, int* counts, float* pred_hm, int B, int J,
-               int h, int w, cudaStream_t stream) {
+int fpd_pck_counts(const int* idx, const float* maxval, const float* target_nchw, int* counts, float* pred_hm, int B,
+                   int J, int h, int w, fpd_stream_t stream) {
   FPD_REQUIRE(B >= 0 && J >= 1 && J <= 64, "pck_counts: B=%d J=%d out of range", B, J);
   FPD_REQUIRE(h >= 1 && w >= 1, "pck_counts: empty %dx%d heat-map", h, w);
   FPD_REQUIRE(idx && maxval && target_nchw && counts, "pck_counts: null pointer");
@@ -225,4 +229,4 @@ int pck_counts(const int* idx, const float* maxval, const float* target_nchw, in
   return FPD_OK;
 }
 
-}  // namespace fpd
+}  // extern "C"

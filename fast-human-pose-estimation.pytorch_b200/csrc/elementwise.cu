@@ -4,10 +4,13 @@
 // (hourglass.py:82,124), nearest-2x upsample + add (hourglass.py:60,90-91), layout converts, weight
 // re-layout. All kernels are vectorised (float4 along the channel axis = the contiguous NHWC axis) and
 // sized for >= 2 waves of the H100's 132 SMs (kNumSMs); reductions are deterministic (fixed-order partial buffers, no atomics).
+// Also the library's state behind fpd_last_error, fpd_launch_count and fpd_sm_count.
 #include <cuda_fp16.h>
 
+#include <atomic>
+#include <cstdarg>
+
 #include "common.cuh"
-#include "kernels.h"
 
 namespace fpd {
 
@@ -1109,242 +1112,33 @@ inline int grid_for(int64_t n, int threads) {
 }  // namespace
 
 // =================================================================================================
-// launchers
+// library state: the calling thread's last error, the launch counter and the device's SM count
 // =================================================================================================
-size_t bn_stats_workspace_bytes(int64_t P, int C) {
-  RedGeom g = red_geom(P, C);
-  return (size_t)g.nblocks * C * 2 * sizeof(double);
+static thread_local char g_err[512] = "";
+static std::atomic<long long> g_launches{0};
+
+void set_last_error(const char* fmt, ...) {
+  va_list ap;
+  va_start(ap, fmt);
+  vsnprintf(g_err, sizeof(g_err), fmt, ap);
+  va_end(ap);
 }
 
-int bn_stats(const float* x, int64_t P, int C, float* mean, float* var_biased, void* workspace, size_t ws_bytes,
-             cudaStream_t stream) {
-  FPD_REQUIRE(C % 4 == 0 && C >= 4 && C <= 4096, "bn_stats: C=%d must be a multiple of 4 in [4,4096]", C);
-  FPD_REQUIRE(P > 0, "bn_stats: empty tensor");
-  RedGeom g = red_geom(P, C);
-  FPD_REQUIRE(ws_bytes >= (size_t)g.nblocks * C * 2 * sizeof(double), "bn_stats: workspace too small");
-  const size_t smem = ((size_t)g.R * C * 2 + g.R) * sizeof(double);
-  static bool attr = false;
-  if (!attr) {
-    FPD_CUDA_CHECK(cudaFuncSetAttribute(bn_stats_partial_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        160 * 1024));
-    FPD_CUDA_CHECK(cudaFuncSetAttribute(bn_stats_partial_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        160 * 1024));
-    attr = true;
+void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
+
+int device_sm_count() {
+  static int n = 0;
+  if (n == 0) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess) return kNumSMs;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = kNumSMs;
   }
-  if (C > 4 * kRedThreads)
-    bn_stats_partial_kernel<true><<<g.nblocks, kRedThreads, smem, stream>>>(x, P, C, g.L, g.R, g.rows_per_block,
-                                                                            (double*)workspace);
-  else
-    bn_stats_partial_kernel<false><<<g.nblocks, kRedThreads, smem, stream>>>(x, P, C, g.L, g.R, g.rows_per_block,
-                                                                             (double*)workspace);
-  FPD_LAUNCH_CHECK();
-  bn_stats_final_kernel<<<(C * 32 + 127) / 128, 128, 0, stream>>>((const double*)workspace, g.nblocks,
-                                                             g.rows_per_block, P, C, mean, var_biased);
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
+  return n;
 }
 
-int bn_finalize(const float* mean, const float* var_biased, const float* gamma, const float* beta, float eps,
-                int64_t count, float* scale, float* shift, float* invstd, float* running_mean, float* running_var,
-                float momentum, int C, cudaStream_t stream) {
-  FPD_REQUIRE((running_mean == nullptr) == (running_var == nullptr), "bn_finalize: running stats must come in pairs");
-  bn_finalize_kernel<<<(C + 127) / 128, 128, 0, stream>>>(mean, var_biased, gamma, beta, eps, count, scale, shift,
-                                                          invstd, running_mean, running_var, momentum, C);
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
-}
-
-int affine_act_split(const float* x, const float* mean, const float* scale, const float* shift, int relu,
-                     float* a_hi, float* a_lo, int64_t P, int C, cudaStream_t stream) {
-  FPD_REQUIRE(C % 4 == 0, "affine_act_split: C=%d must be a multiple of 4", C);
-  FPD_REQUIRE((scale == nullptr) == (shift == nullptr), "affine_act_split: scale/shift must come in pairs");
-  const int64_t n4 = P * C / 4;
-  affine_act_split_kernel<<<grid_for(n4, 256), 256, 0, stream>>>((const float4*)x, mean, scale, shift, relu,
-                                                                 (float4*)a_hi, (float4*)a_lo, n4, C / 4, 1);
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
-}
-
-int affine_act(const float* x, const float* mean, const float* scale, const float* shift, int relu, float* y,
-               int64_t P, int C, cudaStream_t stream) {
-  FPD_REQUIRE(C % 4 == 0, "affine_act: C=%d must be a multiple of 4", C);
-  FPD_REQUIRE((scale == nullptr) == (shift == nullptr), "affine_act: scale/shift must come in pairs");
-  const int64_t n4 = P * C / 4;
-  affine_act_split_kernel<<<grid_for(n4, 256), 256, 0, stream>>>((const float4*)x, mean, scale, shift, relu,
-                                                                 (float4*)y, nullptr, n4, C / 4, 0);
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
-}
-
-int affine_act_f16(const void* x, const float* mean, const float* scale, const float* shift, const void* residual,
-                   int relu, void* y, int64_t P, int C, cudaStream_t stream) {
-  FPD_REQUIRE(C % 4 == 0, "affine_act_f16: C=%d must be a multiple of 4", C);
-  FPD_REQUIRE((scale == nullptr) == (shift == nullptr), "affine_act_f16: scale/shift must come in pairs");
-  const int64_t n4 = P * C / 4;
-  affine_act_f16_kernel<<<grid_for(n4, 256), 256, 0, stream>>>((const __half*)x, mean, scale, shift, relu,
-                                                               (const __half*)residual, (__half*)y, n4, C / 4);
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
-}
-
-int half_to_float(const void* x, float* y, int64_t n, cudaStream_t stream) {
-  FPD_REQUIRE(n % 4 == 0, "half_to_float: n=%lld must be a multiple of 4", (long long)n);
-  half_to_float_kernel<<<grid_for(n / 4, 256), 256, 0, stream>>>((const __half*)x, y, n / 4);
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
-}
-
-int maxpool2x2_fwd(const float* x, float* y, int B, int H, int W, int C, cudaStream_t stream) {
-  FPD_REQUIRE(C % 4 == 0 && H % 2 == 0 && W % 2 == 0, "maxpool2x2: bad shape H=%d W=%d C=%d", H, W, C);
-  const int64_t n = (int64_t)B * (H / 2) * (W / 2) * (C / 4);
-  maxpool2x2_fwd_kernel<<<grid_for(n, 256), 256, 0, stream>>>(x, y, B, H / 2, W / 2, C / 4);
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
-}
-
-int maxpool2x2_fwd_f16(const void* x, void* y, int B, int H, int W, int C, cudaStream_t stream) {
-  FPD_REQUIRE(C % 4 == 0 && H % 2 == 0 && W % 2 == 0, "maxpool2x2_f16: bad shape H=%d W=%d C=%d", H, W, C);
-  const int64_t n = (int64_t)B * (H / 2) * (W / 2) * (C / 4);
-  maxpool2x2_fwd_kernel<<<grid_for(n, 256), 256, 0, stream>>>((const __half*)x, (__half*)y, B, H / 2, W / 2, C / 4);
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
-}
-
-int maxpool2x2_bwd(const float* x, const float* dy, float* dx, int accumulate, int B, int H, int W, int C,
-                   cudaStream_t stream) {
-  FPD_REQUIRE(C % 4 == 0 && H % 2 == 0 && W % 2 == 0, "maxpool2x2_bwd: bad shape H=%d W=%d C=%d", H, W, C);
-  const int64_t n = (int64_t)B * (H / 2) * (W / 2) * (C / 4);
-  maxpool2x2_bwd_kernel<<<grid_for(n, 256), 256, 0, stream>>>((const float4*)x, (const float4*)dy, (float4*)dx,
-                                                              accumulate, B, H / 2, W / 2, C / 4);
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
-}
-
-int upsample2x_add(const float* up1, const float* low, float* out, int B, int H, int W, int C, cudaStream_t stream) {
-  FPD_REQUIRE(C % 4 == 0 && H % 2 == 0 && W % 2 == 0, "upsample2x_add: bad shape H=%d W=%d C=%d", H, W, C);
-  const int64_t n = (int64_t)B * H * W * (C / 4);
-  upsample2x_add_kernel<<<grid_for(n, 256), 256, 0, stream>>>(up1, low, out, B, H, W, C / 4);
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
-}
-
-int upsample2x_add_f16(const void* up1, const void* low, void* out, int B, int H, int W, int C, cudaStream_t stream) {
-  FPD_REQUIRE(C % 4 == 0 && H % 2 == 0 && W % 2 == 0, "upsample2x_add_f16: bad shape H=%d W=%d C=%d", H, W, C);
-  const int64_t n = (int64_t)B * H * W * (C / 4);
-  upsample2x_add_kernel<<<grid_for(n, 256), 256, 0, stream>>>((const __half*)up1, (const __half*)low, (__half*)out, B,
-                                                              H, W, C / 4);
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
-}
-
-int upsample2x_bwd(const float* dout, float* dlow, int B, int H, int W, int C, cudaStream_t stream) {
-  FPD_REQUIRE(C % 4 == 0 && H % 2 == 0 && W % 2 == 0, "upsample2x_bwd: bad shape H=%d W=%d C=%d", H, W, C);
-  const int64_t n = (int64_t)B * (H / 2) * (W / 2) * (C / 4);
-  upsample2x_bwd_kernel<<<grid_for(n, 256), 256, 0, stream>>>((const float4*)dout, (float4*)dlow, B, H / 2, W / 2,
-                                                              C / 4);
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
-}
-
-int subsample2(const float* x, float* y, int B, int H, int W, int C, cudaStream_t stream) {
-  FPD_REQUIRE(C % 4 == 0 && H % 2 == 0 && W % 2 == 0, "subsample2: need C %% 4 == 0 and even H, W (C=%d H=%d W=%d)", C, H, W);
-  const int64_t n = (int64_t)B * (H / 2) * (W / 2) * (C / 4);
-  subsample2_kernel<<<grid_for(n, 256), 256, 0, stream>>>(x, y, B, H / 2, W / 2, C / 4);
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
-}
-
-int subsample2_f16(const void* x, void* y, int B, int H, int W, int C, cudaStream_t stream) {
-  FPD_REQUIRE(C % 4 == 0 && H % 2 == 0 && W % 2 == 0, "subsample2_f16: need C %% 4 == 0 and even H, W (C=%d H=%d W=%d)",
-              C, H, W);
-  const int64_t n = (int64_t)B * (H / 2) * (W / 2) * (C / 4);
-  subsample2_kernel<<<grid_for(n, 256), 256, 0, stream>>>((const __half*)x, (__half*)y, B, H / 2, W / 2, C / 4);
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
-}
-
-int upsample_zero2(const float* dy, float* dx, int B, int Ho, int Wo, int C, cudaStream_t stream) {
-  FPD_REQUIRE(C % 4 == 0, "upsample_zero2: C=%d must be a multiple of 4", C);
-  const int64_t n = (int64_t)B * (2 * Ho) * (2 * Wo) * (C / 4);
-  upsample_zero2_kernel<<<grid_for(n, 256), 256, 0, stream>>>((const float4*)dy, (float4*)dx, B, Ho, Wo, C / 4);
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
-}
-
-int maxpool3x3s2_fwd(const float* x, float* y, int B, int H, int W, int C, cudaStream_t stream) {
-  FPD_REQUIRE(C % 4 == 0 && H >= 1 && W >= 1, "maxpool3x3s2: bad shape H=%d W=%d C=%d", H, W, C);
-  const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
-  const int64_t n = (int64_t)B * Ho * Wo * (C / 4);
-  maxpool3x3s2_fwd_kernel<<<grid_for(n, 256), 256, 0, stream>>>((const float4*)x, (float4*)y, B, H, W, Ho, Wo, C / 4);
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
-}
-
-int maxpool3x3s2_bwd(const float* x, const float* dy, float* dx, int accumulate, int B, int H, int W, int C,
-                     cudaStream_t stream) {
-  FPD_REQUIRE(C % 4 == 0 && H >= 1 && W >= 1, "maxpool3x3s2_bwd: bad shape H=%d W=%d C=%d", H, W, C);
-  const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
-  const int64_t n = (int64_t)B * H * W * (C / 4);
-  maxpool3x3s2_bwd_kernel<<<grid_for(n, 256), 256, 0, stream>>>((const float4*)x, (const float4*)dy, (float4*)dx,
-                                                                accumulate, B, H, W, Ho, Wo, C / 4);
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
-}
-
-int depth_space2(const float* src, float* dst, int B, int H, int W, int C, int to_depth, cudaStream_t stream) {
-  FPD_REQUIRE(C % 4 == 0 && C > 0, "depth_space2: C=%d must be a positive multiple of 4", C);
-  const int64_t n = (int64_t)B * H * W * 4 * (C / 4);
-  depth_space2_kernel<<<grid_for(n, 256), 256, 0, stream>>>((const float4*)src, (float4*)dst, B, H, W, C / 4,
-                                                            to_depth ? 1 : 0);
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
-}
-
-int deconv_weight_map(const float* src, float* dst, int Cin, int Cout, int k, int pad, int to_deconv,
-                      cudaStream_t stream) {
-  FPD_REQUIRE((k == 4 && pad == 1) || (k == 3 && pad == 1) || (k == 2 && pad == 0),
-              "deconv_weight_map: (kernel, padding) = (%d, %d) is not one of pose_resnet's (4,1) (3,1) (2,0)", k, pad);
-  FPD_REQUIRE(src && dst && Cin > 0 && Cout > 0, "deconv_weight_map: bad argument");
-  const int64_t n = to_deconv ? (int64_t)Cin * Cout * k * k : (int64_t)4 * Cout * Cin * 9;
-  deconv_weight_map_kernel<<<grid_for(n, 256), 256, 0, stream>>>(src, dst, Cin, Cout, k, pad, to_deconv ? 1 : 0);
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
-}
-
-int nchw_to_nhwc(const float* x, float* y, int B, int C, int H, int W, cudaStream_t stream) {
-  // per image: [C][HW] -> [HW][C]
-  dim3 grid((H * W + 31) / 32, (C + 31) / 32, B), block(32, 8);
-  transpose_cs_kernel<<<grid, block, 0, stream>>>(x, y, C, H * W, 0);
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
-}
-
-int nchw_to_nhwc_flipw(const float* x, float* y, int B, int C, int H, int W, cudaStream_t stream) {
-  dim3 grid((H * W + 31) / 32, (C + 31) / 32, B), block(32, 8);
-  transpose_cs_kernel<<<grid, block, 0, stream>>>(x, y, C, H * W, W);
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
-}
-
-int nhwc_to_nchw(const float* x, float* y, int B, int C, int H, int W, cudaStream_t stream) {
-  dim3 grid((C + 31) / 32, (H * W + 31) / 32, B), block(32, 8);
-  transpose_cs_kernel<<<grid, block, 0, stream>>>(x, y, H * W, C, 0);
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
-}
-
-int add_tensors(const float* a, const float* b, float* out, int64_t n, cudaStream_t stream) {
-  FPD_REQUIRE(n % 4 == 0, "add_tensors: n must be a multiple of 4");
-  add_kernel<<<grid_for(n / 4, 256), 256, 0, stream>>>((const float4*)a, (const float4*)b, (float4*)out, n / 4);
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
-}
-
-size_t channel_reduce_workspace_bytes(int64_t P, int C) {
-  RedGeom g = red_geom(P, C);
-  return (size_t)g.nblocks * 2 * C * sizeof(double) + (size_t)g.nblocks * sizeof(float);   // + block maxima (fused form)
-}
-
+// =================================================================================================
+// launch helpers shared by several entry points
+// =================================================================================================
 template <int NV, class F>
 static int run_channel_reduce_fused(F f, int64_t P, int C, float scale, float* out, float* amax_scale, void* workspace,
                                     size_t ws_bytes, unsigned int* counter, cudaStream_t stream) {
@@ -1426,8 +1220,284 @@ __global__ void channel_sum_generic_kernel(const float* __restrict__ dy, int64_t
   }
 }
 
-int channel_sum(const float* dy, int64_t P, int C, float scale, float* out, void* workspace, size_t ws_bytes,
-                cudaStream_t stream) {
+template <typename T>
+static int fuse_sum_t(const void* const* terms, const int* shifts, int n, int relu, T* out, int B, int H, int W, int C,
+                      cudaStream_t stream) {
+  FPD_REQUIRE(n >= 1 && n <= 4, "fuse_sum: 1..4 terms, got %d", n);
+  FPD_REQUIRE(C % 4 == 0, "fuse_sum: C=%d must be a multiple of 4", C);
+  FuseTerms ft{};
+  ft.n = n;
+  for (int j = 0; j < n; ++j) {
+    FPD_REQUIRE(shifts[j] >= 0 && (H % (1 << shifts[j])) == 0 && (W % (1 << shifts[j])) == 0,
+                "fuse_sum: term %d upsampling factor does not divide the output size", j);
+    ft.t[j] = terms[j];
+    ft.shift[j] = shifts[j];
+  }
+  const int64_t n4 = (int64_t)B * H * W * (C / 4);
+  fuse_sum_kernel<<<grid_for(n4, 256), 256, 0, stream>>>(ft, relu, out, B, H, W, C / 4);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+// fp16-in / fp16-out affine_act, and affine_add_act where residual is not NULL
+static int affine_act_f16(const void* x, const float* mean, const float* scale, const float* shift,
+                          const void* residual, int relu, void* y, int64_t P, int C, cudaStream_t stream) {
+  FPD_REQUIRE(C % 4 == 0, "affine_act_f16: C=%d must be a multiple of 4", C);
+  FPD_REQUIRE((scale == nullptr) == (shift == nullptr), "affine_act_f16: scale/shift must come in pairs");
+  const int64_t n4 = P * C / 4;
+  affine_act_f16_kernel<<<grid_for(n4, 256), 256, 0, stream>>>((const __half*)x, mean, scale, shift, relu,
+                                                               (const __half*)residual, (__half*)y, n4, C / 4);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+}  // namespace fpd
+
+using namespace fpd;
+
+// =================================================================================================
+// entry points
+// =================================================================================================
+extern "C" {
+
+size_t fpd_bn_stats_workspace_bytes(int64_t P, int C) {
+  RedGeom g = red_geom(P, C);
+  return (size_t)g.nblocks * C * 2 * sizeof(double);
+}
+
+int fpd_bn_stats(const float* x, int64_t P, int C, float* mean, float* var_biased, void* workspace, size_t ws_bytes,
+                 fpd_stream_t stream) {
+  FPD_REQUIRE(C % 4 == 0 && C >= 4 && C <= 4096, "bn_stats: C=%d must be a multiple of 4 in [4,4096]", C);
+  FPD_REQUIRE(P > 0, "bn_stats: empty tensor");
+  RedGeom g = red_geom(P, C);
+  FPD_REQUIRE(ws_bytes >= (size_t)g.nblocks * C * 2 * sizeof(double), "bn_stats: workspace too small");
+  const size_t smem = ((size_t)g.R * C * 2 + g.R) * sizeof(double);
+  static bool attr = false;
+  if (!attr) {
+    FPD_CUDA_CHECK(cudaFuncSetAttribute(bn_stats_partial_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        160 * 1024));
+    FPD_CUDA_CHECK(cudaFuncSetAttribute(bn_stats_partial_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        160 * 1024));
+    attr = true;
+  }
+  if (C > 4 * kRedThreads)
+    bn_stats_partial_kernel<true><<<g.nblocks, kRedThreads, smem, stream>>>(x, P, C, g.L, g.R, g.rows_per_block,
+                                                                            (double*)workspace);
+  else
+    bn_stats_partial_kernel<false><<<g.nblocks, kRedThreads, smem, stream>>>(x, P, C, g.L, g.R, g.rows_per_block,
+                                                                             (double*)workspace);
+  FPD_LAUNCH_CHECK();
+  bn_stats_final_kernel<<<(C * 32 + 127) / 128, 128, 0, stream>>>((const double*)workspace, g.nblocks,
+                                                             g.rows_per_block, P, C, mean, var_biased);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int fpd_bn_finalize(const float* mean, const float* var_biased, const float* gamma, const float* beta, float eps,
+                    int64_t count, float* scale, float* shift, float* invstd, float* running_mean, float* running_var,
+                    float momentum, int C, fpd_stream_t stream) {
+  FPD_REQUIRE((running_mean == nullptr) == (running_var == nullptr), "bn_finalize: running stats must come in pairs");
+  bn_finalize_kernel<<<(C + 127) / 128, 128, 0, stream>>>(mean, var_biased, gamma, beta, eps, count, scale, shift,
+                                                          invstd, running_mean, running_var, momentum, C);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int fpd_affine_act_split(const float* x, const float* mean, const float* scale, const float* shift, int relu,
+                         float* a_hi, float* a_lo, int64_t P, int C, fpd_stream_t stream) {
+  FPD_REQUIRE(C % 4 == 0, "affine_act_split: C=%d must be a multiple of 4", C);
+  FPD_REQUIRE((scale == nullptr) == (shift == nullptr), "affine_act_split: scale/shift must come in pairs");
+  const int64_t n4 = P * C / 4;
+  affine_act_split_kernel<<<grid_for(n4, 256), 256, 0, stream>>>((const float4*)x, mean, scale, shift, relu,
+                                                                 (float4*)a_hi, (float4*)a_lo, n4, C / 4, 1);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int fpd_affine_act(const float* x, const float* mean, const float* scale, const float* shift, int relu, float* y,
+                   int64_t P, int C, fpd_stream_t stream) {
+  FPD_REQUIRE(C % 4 == 0, "affine_act: C=%d must be a multiple of 4", C);
+  FPD_REQUIRE((scale == nullptr) == (shift == nullptr), "affine_act: scale/shift must come in pairs");
+  const int64_t n4 = P * C / 4;
+  affine_act_split_kernel<<<grid_for(n4, 256), 256, 0, stream>>>((const float4*)x, mean, scale, shift, relu,
+                                                                 (float4*)y, nullptr, n4, C / 4, 0);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int fpd_affine_act_f16(const void* x, const float* mean, const float* scale, const float* shift, int relu, void* y,
+                       int64_t P, int C, fpd_stream_t stream) {
+  return affine_act_f16(x, mean, scale, shift, nullptr, relu, y, P, C, stream);
+}
+
+int fpd_affine_add_act_f16(const void* x, const float* mean, const float* scale, const float* shift,
+                           const void* residual, int relu, void* y, int64_t P, int C, fpd_stream_t stream) {
+  FPD_REQUIRE(residual, "fpd_affine_add_act_f16: NULL residual");
+  return affine_act_f16(x, mean, scale, shift, residual, relu, y, P, C, stream);
+}
+
+int fpd_half_to_float(const void* x, float* y, int64_t n, fpd_stream_t stream) {
+  FPD_REQUIRE(n % 4 == 0, "half_to_float: n=%lld must be a multiple of 4", (long long)n);
+  half_to_float_kernel<<<grid_for(n / 4, 256), 256, 0, stream>>>((const __half*)x, y, n / 4);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int fpd_maxpool2x2_fwd(const float* x, float* y, int B, int H, int W, int C, fpd_stream_t stream) {
+  FPD_REQUIRE(C % 4 == 0 && H % 2 == 0 && W % 2 == 0, "maxpool2x2: bad shape H=%d W=%d C=%d", H, W, C);
+  const int64_t n = (int64_t)B * (H / 2) * (W / 2) * (C / 4);
+  maxpool2x2_fwd_kernel<<<grid_for(n, 256), 256, 0, stream>>>(x, y, B, H / 2, W / 2, C / 4);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int fpd_maxpool2x2_fwd_f16(const void* x, void* y, int B, int H, int W, int C, fpd_stream_t stream) {
+  FPD_REQUIRE(C % 4 == 0 && H % 2 == 0 && W % 2 == 0, "maxpool2x2_f16: bad shape H=%d W=%d C=%d", H, W, C);
+  const int64_t n = (int64_t)B * (H / 2) * (W / 2) * (C / 4);
+  maxpool2x2_fwd_kernel<<<grid_for(n, 256), 256, 0, stream>>>((const __half*)x, (__half*)y, B, H / 2, W / 2, C / 4);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int fpd_maxpool2x2_bwd(const float* x, const float* dy, float* dx, int accumulate, int B, int H, int W, int C,
+                       fpd_stream_t stream) {
+  FPD_REQUIRE(C % 4 == 0 && H % 2 == 0 && W % 2 == 0, "maxpool2x2_bwd: bad shape H=%d W=%d C=%d", H, W, C);
+  const int64_t n = (int64_t)B * (H / 2) * (W / 2) * (C / 4);
+  maxpool2x2_bwd_kernel<<<grid_for(n, 256), 256, 0, stream>>>((const float4*)x, (const float4*)dy, (float4*)dx,
+                                                              accumulate, B, H / 2, W / 2, C / 4);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int fpd_upsample2x_add(const float* up1, const float* low, float* out, int B, int H, int W, int C,
+                       fpd_stream_t stream) {
+  FPD_REQUIRE(C % 4 == 0 && H % 2 == 0 && W % 2 == 0, "upsample2x_add: bad shape H=%d W=%d C=%d", H, W, C);
+  const int64_t n = (int64_t)B * H * W * (C / 4);
+  upsample2x_add_kernel<<<grid_for(n, 256), 256, 0, stream>>>(up1, low, out, B, H, W, C / 4);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int fpd_upsample2x_add_f16(const void* up1, const void* low, void* out, int B, int H, int W, int C,
+                           fpd_stream_t stream) {
+  FPD_REQUIRE(C % 4 == 0 && H % 2 == 0 && W % 2 == 0, "upsample2x_add_f16: bad shape H=%d W=%d C=%d", H, W, C);
+  const int64_t n = (int64_t)B * H * W * (C / 4);
+  upsample2x_add_kernel<<<grid_for(n, 256), 256, 0, stream>>>((const __half*)up1, (const __half*)low, (__half*)out, B,
+                                                              H, W, C / 4);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int fpd_upsample2x_bwd(const float* dout, float* dlow, int B, int H, int W, int C, fpd_stream_t stream) {
+  FPD_REQUIRE(C % 4 == 0 && H % 2 == 0 && W % 2 == 0, "upsample2x_bwd: bad shape H=%d W=%d C=%d", H, W, C);
+  const int64_t n = (int64_t)B * (H / 2) * (W / 2) * (C / 4);
+  upsample2x_bwd_kernel<<<grid_for(n, 256), 256, 0, stream>>>((const float4*)dout, (float4*)dlow, B, H / 2, W / 2,
+                                                              C / 4);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int fpd_subsample2(const float* x, float* y, int B, int H, int W, int C, fpd_stream_t stream) {
+  FPD_REQUIRE(C % 4 == 0 && H % 2 == 0 && W % 2 == 0, "subsample2: need C %% 4 == 0 and even H, W (C=%d H=%d W=%d)", C, H, W);
+  const int64_t n = (int64_t)B * (H / 2) * (W / 2) * (C / 4);
+  subsample2_kernel<<<grid_for(n, 256), 256, 0, stream>>>(x, y, B, H / 2, W / 2, C / 4);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int fpd_subsample2_f16(const void* x, void* y, int B, int H, int W, int C, fpd_stream_t stream) {
+  FPD_REQUIRE(C % 4 == 0 && H % 2 == 0 && W % 2 == 0, "subsample2_f16: need C %% 4 == 0 and even H, W (C=%d H=%d W=%d)",
+              C, H, W);
+  const int64_t n = (int64_t)B * (H / 2) * (W / 2) * (C / 4);
+  subsample2_kernel<<<grid_for(n, 256), 256, 0, stream>>>((const __half*)x, (__half*)y, B, H / 2, W / 2, C / 4);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int fpd_upsample_zero2(const float* dy, float* dx, int B, int Ho, int Wo, int C, fpd_stream_t stream) {
+  FPD_REQUIRE(C % 4 == 0, "upsample_zero2: C=%d must be a multiple of 4", C);
+  const int64_t n = (int64_t)B * (2 * Ho) * (2 * Wo) * (C / 4);
+  upsample_zero2_kernel<<<grid_for(n, 256), 256, 0, stream>>>((const float4*)dy, (float4*)dx, B, Ho, Wo, C / 4);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int fpd_maxpool3x3s2_fwd(const float* x, float* y, int B, int H, int W, int C, fpd_stream_t stream) {
+  FPD_REQUIRE(C % 4 == 0 && H >= 1 && W >= 1, "maxpool3x3s2: bad shape H=%d W=%d C=%d", H, W, C);
+  const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
+  const int64_t n = (int64_t)B * Ho * Wo * (C / 4);
+  maxpool3x3s2_fwd_kernel<<<grid_for(n, 256), 256, 0, stream>>>((const float4*)x, (float4*)y, B, H, W, Ho, Wo, C / 4);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int fpd_maxpool3x3s2_bwd(const float* x, const float* dy, float* dx, int accumulate, int B, int H, int W, int C,
+                         fpd_stream_t stream) {
+  FPD_REQUIRE(C % 4 == 0 && H >= 1 && W >= 1, "maxpool3x3s2_bwd: bad shape H=%d W=%d C=%d", H, W, C);
+  const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
+  const int64_t n = (int64_t)B * H * W * (C / 4);
+  maxpool3x3s2_bwd_kernel<<<grid_for(n, 256), 256, 0, stream>>>((const float4*)x, (const float4*)dy, (float4*)dx,
+                                                                accumulate, B, H, W, Ho, Wo, C / 4);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int fpd_depth_space2(const float* src, float* dst, int B, int H, int W, int C, int to_depth, fpd_stream_t stream) {
+  FPD_REQUIRE(C % 4 == 0 && C > 0, "depth_space2: C=%d must be a positive multiple of 4", C);
+  const int64_t n = (int64_t)B * H * W * 4 * (C / 4);
+  depth_space2_kernel<<<grid_for(n, 256), 256, 0, stream>>>((const float4*)src, (float4*)dst, B, H, W, C / 4,
+                                                            to_depth ? 1 : 0);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int fpd_deconv_weight_map(const float* src, float* dst, int Cin, int Cout, int k, int pad, int to_deconv,
+                          fpd_stream_t stream) {
+  FPD_REQUIRE((k == 4 && pad == 1) || (k == 3 && pad == 1) || (k == 2 && pad == 0),
+              "deconv_weight_map: (kernel, padding) = (%d, %d) is not one of pose_resnet's (4,1) (3,1) (2,0)", k, pad);
+  FPD_REQUIRE(src && dst && Cin > 0 && Cout > 0, "deconv_weight_map: bad argument");
+  const int64_t n = to_deconv ? (int64_t)Cin * Cout * k * k : (int64_t)4 * Cout * Cin * 9;
+  deconv_weight_map_kernel<<<grid_for(n, 256), 256, 0, stream>>>(src, dst, Cin, Cout, k, pad, to_deconv ? 1 : 0);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int fpd_nchw_to_nhwc(const float* x, float* y, int B, int C, int H, int W, fpd_stream_t stream) {
+  // per image: [C][HW] -> [HW][C]
+  dim3 grid((H * W + 31) / 32, (C + 31) / 32, B), block(32, 8);
+  transpose_cs_kernel<<<grid, block, 0, stream>>>(x, y, C, H * W, 0);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int fpd_nchw_to_nhwc_flipw(const float* x, float* y, int B, int C, int H, int W, fpd_stream_t stream) {
+  dim3 grid((H * W + 31) / 32, (C + 31) / 32, B), block(32, 8);
+  transpose_cs_kernel<<<grid, block, 0, stream>>>(x, y, C, H * W, W);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int fpd_nhwc_to_nchw(const float* x, float* y, int B, int C, int H, int W, fpd_stream_t stream) {
+  dim3 grid((C + 31) / 32, (H * W + 31) / 32, B), block(32, 8);
+  transpose_cs_kernel<<<grid, block, 0, stream>>>(x, y, H * W, C, 0);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int fpd_add(const float* a, const float* b, float* out, int64_t n, fpd_stream_t stream) {
+  FPD_REQUIRE(n % 4 == 0, "add_tensors: n must be a multiple of 4");
+  add_kernel<<<grid_for(n / 4, 256), 256, 0, stream>>>((const float4*)a, (const float4*)b, (float4*)out, n / 4);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+size_t fpd_channel_reduce_workspace_bytes(int64_t P, int C) {
+  RedGeom g = red_geom(P, C);
+  return (size_t)g.nblocks * 2 * C * sizeof(double) + (size_t)g.nblocks * sizeof(float);   // + block maxima (fused form)
+}
+
+int fpd_channel_sum(const float* dy, int64_t P, int C, float scale, float* out, void* workspace, size_t ws_bytes,
+                    fpd_stream_t stream) {
   if (C % 4 != 0) {
     channel_sum_generic_kernel<<<C, 256, 0, stream>>>(dy, P, C, scale, out);
     FPD_LAUNCH_CHECK();
@@ -1437,22 +1507,22 @@ int channel_sum(const float* dy, int64_t P, int C, float scale, float* out, void
   return run_channel_reduce<1>(f, P, C, scale, out, workspace, ws_bytes, stream);
 }
 
-int channel_sum_fused(const float* dy, int64_t P, int C, float scale, float* out, float* amax_scale, void* workspace,
-                      size_t ws_bytes, unsigned int* counter, cudaStream_t stream) {
+int fpd_channel_sum_fused(const float* dy, int64_t P, int C, float scale, float* out, float* amax_scale,
+                          void* workspace, size_t ws_bytes, unsigned int* counter, fpd_stream_t stream) {
   SumFunctor f{dy, C};
   return run_channel_reduce_fused<1>(f, P, C, scale, out, amax_scale, workspace, ws_bytes, counter, stream);
 }
 
-int bn_bwd_reduce_fused(const float* da, const float* x, const float* mean, const float* invstd, const float* scale,
-                        const float* shift, int relu, int64_t P, int C, float* sums, void* workspace, size_t ws_bytes,
-                        unsigned int* counter, cudaStream_t stream) {
+int fpd_bn_bwd_reduce_fused(const float* da, const float* x, const float* mean, const float* invstd, const float* scale,
+                            const float* shift, int relu, int64_t P, int C, float* sums, void* workspace,
+                            size_t ws_bytes, unsigned int* counter, fpd_stream_t stream) {
   BnBwdFunctor f{da, x, mean, invstd, scale, shift, relu, C};
   return run_channel_reduce_fused<2>(f, P, C, 1.f, sums, nullptr, workspace, ws_bytes, counter, stream);
 }
 
-int bn_stats_fused(const float* x, int64_t P, int C, const float* gamma, const float* beta, float eps, float momentum,
-                   float* rmean, float* rvar, float* mean, float* var, float* scale, float* shift, float* invstd,
-                   void* workspace, size_t ws_bytes, unsigned int* counter, cudaStream_t stream) {
+int fpd_bn_stats_fused(const float* x, int64_t P, int C, const float* gamma, const float* beta, float eps,
+                       float momentum, float* rmean, float* rvar, float* mean, float* var, float* scale, float* shift,
+                       float* invstd, void* workspace, size_t ws_bytes, unsigned int* counter, fpd_stream_t stream) {
   (void)counter;   // see run_channel_reduce_fused: two launches (partial + final/finalize) instead of three
   FPD_REQUIRE(C % 4 == 0 && C >= 4 && C <= 4096, "bn_stats_fused: C=%d must be a multiple of 4 in [4,4096]", C);
   FPD_REQUIRE(P > 0 && mean && var && scale && shift, "bn_stats_fused: bad argument");
@@ -1482,9 +1552,9 @@ int bn_stats_fused(const float* x, int64_t P, int C, const float* gamma, const f
   return FPD_OK;
 }
 
-int bn_finalize_sums(const double* part, int nblocks, const float* pivot, int64_t P, int C, const float* gamma,
-                     const float* beta, float eps, float momentum, float* rmean, float* rvar, float* mean, float* var,
-                     float* scale, float* shift, float* invstd, cudaStream_t stream) {
+int fpd_bn_finalize_sums(const double* part, int nblocks, const float* pivot, int64_t P, int C, const float* gamma,
+                         const float* beta, float eps, float momentum, float* rmean, float* rvar, float* mean,
+                         float* var, float* scale, float* shift, float* invstd, fpd_stream_t stream) {
   FPD_REQUIRE(part && nblocks > 0 && P > 0 && C > 0 && mean && var && scale && shift, "bn_finalize_sums: bad argument");
   FPD_REQUIRE((rmean == nullptr) == (rvar == nullptr), "bn_finalize_sums: running stats come in pairs");
   BnFinalize fz{gamma, beta, eps, momentum, mean, var, scale, shift, invstd, rmean, rvar};
@@ -1493,16 +1563,16 @@ int bn_finalize_sums(const double* part, int nblocks, const float* pivot, int64_
   return FPD_OK;
 }
 
-int bn_bwd_reduce(const float* da, const float* x, const float* mean, const float* invstd, const float* scale,
-                  const float* shift, int relu, int64_t P, int C, float* sums, void* workspace, size_t ws_bytes,
-                  cudaStream_t stream) {
+int fpd_bn_bwd_reduce(const float* da, const float* x, const float* mean, const float* invstd, const float* scale,
+                      const float* shift, int relu, int64_t P, int C, float* sums, void* workspace, size_t ws_bytes,
+                      fpd_stream_t stream) {
   BnBwdFunctor f{da, x, mean, invstd, scale, shift, relu, C};
   return run_channel_reduce<2>(f, P, C, 1.f, sums, workspace, ws_bytes, stream);
 }
 
-int bn_bwd_apply(const float* da, const float* x, const float* mean, const float* invstd, const float* scale,
-                 const float* shift, const float* gamma, int relu, const float* sums, int accumulate, float* dx,
-                 int64_t P, int C, cudaStream_t stream) {
+int fpd_bn_bwd_apply(const float* da, const float* x, const float* mean, const float* invstd, const float* scale,
+                     const float* shift, const float* gamma, int relu, const float* sums, int accumulate, float* dx,
+                     int64_t P, int C, fpd_stream_t stream) {
   FPD_REQUIRE(C % 4 == 0, "bn_bwd_apply: C=%d must be a multiple of 4", C);
   const int64_t n4 = P * C / 4;
   bn_bwd_apply_kernel<<<grid_for(n4, 256), 256, 0, stream>>>((const float4*)da, (const float4*)x, mean, invstd,
@@ -1512,16 +1582,16 @@ int bn_bwd_apply(const float* da, const float* x, const float* mean, const float
   return FPD_OK;
 }
 
-int bn_bwd_apply_sum(const float* da, const float* x, const float* mean, const float* invstd, const float* scale,
-                     const float* shift, const float* gamma, int relu, const float* sums, float* dx, float* dx_sum,
-                     float* amax_scale, int64_t P, int C, void* workspace, size_t ws_bytes, cudaStream_t stream) {
+int fpd_bn_bwd_apply_sum(const float* da, const float* x, const float* mean, const float* invstd, const float* scale,
+                         const float* shift, const float* gamma, int relu, const float* sums, float* dx, float* dx_sum,
+                         float* amax_scale, int64_t P, int C, void* workspace, size_t ws_bytes, fpd_stream_t stream) {
   FPD_REQUIRE(da && x && mean && invstd && scale && shift && sums && dx && dx_sum, "bn_bwd_apply_sum: null pointer");
   BnBwdApplySumFunctor f{da, x, mean, invstd, scale, shift, gamma, sums, dx, relu, C, 1.f / (float)P};
   return run_channel_reduce_fused<1>(f, P, C, 1.f, dx_sum, amax_scale, workspace, ws_bytes, nullptr, stream);
 }
 
-int affine_act_bwd(const float* da, const float* x, const float* mean, const float* scale, const float* shift,
-                   int relu, int accumulate, float* dx, int64_t P, int C, cudaStream_t stream) {
+int fpd_affine_act_bwd(const float* da, const float* x, const float* mean, const float* scale, const float* shift,
+                       int relu, int accumulate, float* dx, int64_t P, int C, fpd_stream_t stream) {
   FPD_REQUIRE(C % 4 == 0, "affine_act_bwd: C=%d must be a multiple of 4", C);
   const int64_t n4 = P * C / 4;
   affine_act_bwd_kernel<<<grid_for(n4, 256), 256, 0, stream>>>((const float4*)da, (const float4*)x, mean, scale,
@@ -1530,16 +1600,16 @@ int affine_act_bwd(const float* da, const float* x, const float* mean, const flo
   return FPD_OK;
 }
 
-int weight_prep(const float* w_oihw, float* w_hi, float* w_lo, int O, int I, int k, int for_dgrad,
-                cudaStream_t stream) {
+int fpd_weight_prep(const float* w_oihw, float* w_hi, float* w_lo, int O, int I, int k, int for_dgrad,
+                    fpd_stream_t stream) {
   const int64_t n = (int64_t)O * I * k * k;
   weight_prep_kernel<<<grid_for(n, 256), 256, 0, stream>>>(w_oihw, w_hi, w_lo, O, I, k, for_dgrad);
   FPD_LAUNCH_CHECK();
   return FPD_OK;
 }
 
-int weight_prep_f16(const float* w_oihw, void* w_hi, void* w_lo, int O, int I, int k, int for_dgrad,
-                    cudaStream_t stream) {
+int fpd_weight_prep_f16(const float* w_oihw, void* w_hi, void* w_lo, int O, int I, int k, int for_dgrad,
+                        fpd_stream_t stream) {
   const int64_t n = (int64_t)O * I * k * k;
   weight_prep_f16_kernel<<<grid_for(n, 256), 256, 0, stream>>>(w_oihw, (__half*)w_hi, (__half*)w_lo, O, I, k, for_dgrad,
                                                                (float)(1 << kF16WeightScaleLog2));
@@ -1547,8 +1617,8 @@ int weight_prep_f16(const float* w_oihw, void* w_hi, void* w_lo, int O, int I, i
   return FPD_OK;
 }
 
-int weight_prep_f16_both(const float* w_oihw, void* f_hi, void* f_lo, void* d_hi, void* d_lo, int O, int I, int k,
-                         cudaStream_t stream) {
+int fpd_weight_prep_f16_both(const float* w_oihw, void* f_hi, void* f_lo, void* d_hi, void* d_lo, int O, int I, int k,
+                             fpd_stream_t stream) {
   FPD_REQUIRE(w_oihw && f_hi && d_hi, "weight_prep_f16_both: null operand");
   FPD_REQUIRE((f_lo == nullptr) == (d_lo == nullptr), "weight_prep_f16_both: f_lo and d_lo are both set or both NULL");
   const int64_t n = (int64_t)O * I * k * k;
@@ -1559,8 +1629,8 @@ int weight_prep_f16_both(const float* w_oihw, void* f_hi, void* f_lo, void* d_hi
   return FPD_OK;
 }
 
-int affine_add_act(const float* x, const float* mean, const float* scale, const float* shift, const float* residual,
-                   int relu, float* y, int64_t P, int C, cudaStream_t stream) {
+int fpd_affine_add_act(const float* x, const float* mean, const float* scale, const float* shift, const float* residual,
+                       int relu, float* y, int64_t P, int C, fpd_stream_t stream) {
   FPD_REQUIRE(C % 4 == 0, "affine_add_act: C=%d must be a multiple of 4", C);
   FPD_REQUIRE((scale == nullptr) == (shift == nullptr), "affine_add_act: scale/shift must come in pairs");
   const int64_t n4 = P * C / 4;
@@ -1571,36 +1641,19 @@ int affine_add_act(const float* x, const float* mean, const float* scale, const 
   return FPD_OK;
 }
 
-template <typename T>
-static int fuse_sum_t(const void* const* terms, const int* shifts, int n, int relu, T* out, int B, int H, int W, int C,
-                      cudaStream_t stream) {
-  FPD_REQUIRE(n >= 1 && n <= 4, "fuse_sum: 1..4 terms, got %d", n);
-  FPD_REQUIRE(C % 4 == 0, "fuse_sum: C=%d must be a multiple of 4", C);
-  FuseTerms ft{};
-  ft.n = n;
-  for (int j = 0; j < n; ++j) {
-    FPD_REQUIRE(shifts[j] >= 0 && (H % (1 << shifts[j])) == 0 && (W % (1 << shifts[j])) == 0,
-                "fuse_sum: term %d upsampling factor does not divide the output size", j);
-    ft.t[j] = terms[j];
-    ft.shift[j] = shifts[j];
-  }
-  const int64_t n4 = (int64_t)B * H * W * (C / 4);
-  fuse_sum_kernel<<<grid_for(n4, 256), 256, 0, stream>>>(ft, relu, out, B, H, W, C / 4);
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
-}
-
-int fuse_sum(const float* const* terms, const int* shifts, int n, int relu, float* out, int B, int H, int W, int C,
-             cudaStream_t stream) {
+int fpd_fuse_sum(const float* const* terms, const int* shifts, int n, int relu, float* out, int B, int H, int W, int C,
+                 fpd_stream_t stream) {
+  FPD_REQUIRE(terms && shifts, "fpd_fuse_sum: NULL term table");
   return fuse_sum_t(reinterpret_cast<const void* const*>(terms), shifts, n, relu, out, B, H, W, C, stream);
 }
 
-int fuse_sum_f16(const void* const* terms, const int* shifts, int n, int relu, void* out, int B, int H, int W, int C,
-                 cudaStream_t stream) {
+int fpd_fuse_sum_f16(const void* const* terms, const int* shifts, int n, int relu, void* out, int B, int H, int W,
+                     int C, fpd_stream_t stream) {
+  FPD_REQUIRE(terms && shifts, "fpd_fuse_sum_f16: NULL term table");
   return fuse_sum_t(terms, shifts, n, relu, (__half*)out, B, H, W, C, stream);
 }
 
-int upsample_bwd(const float* dout, float* dlow, int shift, int B, int H, int W, int C, cudaStream_t stream) {
+int fpd_upsample_bwd(const float* dout, float* dlow, int shift, int B, int H, int W, int C, fpd_stream_t stream) {
   FPD_REQUIRE(C % 4 == 0 && shift >= 0 && H % (1 << shift) == 0 && W % (1 << shift) == 0,
               "upsample_bwd: bad shape H=%d W=%d C=%d shift=%d", H, W, C, shift);
   const int Ho = H >> shift, Wo = W >> shift;
@@ -1610,8 +1663,8 @@ int upsample_bwd(const float* dout, float* dlow, int shift, int B, int H, int W,
   return FPD_OK;
 }
 
-int im2col(const float* x, float* cols, int B, int H, int W, int Cin, int k, int stride, int pad, int Kpad,
-           cudaStream_t stream) {
+int fpd_im2col(const float* x, float* cols, int B, int H, int W, int Cin, int k, int stride, int pad, int Kpad,
+               fpd_stream_t stream) {
   FPD_REQUIRE(Kpad % 4 == 0 && Kpad >= k * k * Cin, "im2col: Kpad=%d must be a multiple of 4 and >= k*k*Cin", Kpad);
   const int Ho = (H + 2 * pad - k) / stride + 1, Wo = (W + 2 * pad - k) / stride + 1;
   const int64_t n = (int64_t)B * Ho * Wo * (Kpad / 4);
@@ -1625,14 +1678,9 @@ int im2col(const float* x, float* cols, int B, int H, int W, int Cin, int k, int
   return FPD_OK;
 }
 
-int device_sm_count() {
-  static int n = 0;
-  if (n == 0) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return kNumSMs;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = kNumSMs;
-  }
-  return n;
-}
+const char* fpd_last_error(void) { return g_err; }
+int fpd_version(void) { return 100; }
+int fpd_sm_count(void) { return device_sm_count(); }
+long long fpd_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
 
-}  // namespace fpd
+}  // extern "C"

@@ -12,7 +12,6 @@
 // Layouts: student / teacher heat-maps are the network-internal NHWC [B,h,w,J]; `target` is the caller's
 // NCHW [B,J,h,w] tensor (lib/dataset/JointsDataset.py target layout), staged through shared memory.
 #include "common.cuh"
-#include "kernels.h"
 
 namespace fpd {
 namespace {
@@ -120,6 +119,11 @@ joints_mse_kernel(const float* __restrict__ out, const float* __restrict__ targe
 }
 
 }  // namespace
+}  // namespace fpd
+
+using namespace fpd;
+
+extern "C" {
 
 size_t fpd_loss_workspace_bytes(int B, int J, int h, int w) {
   const int64_t hw = (int64_t)h * w;
@@ -128,9 +132,10 @@ size_t fpd_loss_workspace_bytes(int B, int J, int h, int w) {
   return (size_t)nblocks * 2 * sizeof(double);
 }
 
-int fpd_loss(const float* const* outs, int S, const float* target_nchw, const float* teacher_nhwc, const float* tw,
-             float alpha, float* const* grads, float grad_scale, float* losses, int B, int J, int h, int w,
-             void* workspace, size_t ws_bytes, cudaStream_t stream) {
+int fpd_loss_fused(const float* const* outs, int S, const float* target_nchw, const float* teacher_nhwc, const float* tw,
+                   float alpha, float* const* grads, float grad_scale, float* losses, int B, int J, int h, int w,
+                   void* workspace, size_t ws_bytes, fpd_stream_t stream) {
+  FPD_REQUIRE(outs != nullptr, "fpd_loss_fused: outs_host is NULL");
   const int hw = h * w;
   FPD_REQUIRE(S >= 1 && S <= kMaxStacks, "fpd_loss: S=%d out of range [1,%d]", S, kMaxStacks);
   FPD_REQUIRE(hw % kPix == 0, "fpd_loss: h*w=%d must be a multiple of %d", hw, kPix);
@@ -153,8 +158,8 @@ int fpd_loss(const float* const* outs, int S, const float* target_nchw, const fl
   return FPD_OK;
 }
 
-int joints_mse(const float* out_nchw, const float* target_nchw, const float* tw, float* loss, float* grad_out,
-               float, int B, int J, int hw, void* workspace, size_t ws_bytes, cudaStream_t stream) {
+int fpd_joints_mse(const float* out_nchw, const float* target_nchw, const float* tw, float* loss, float* grad_out, int B,
+                   int J, int hw, void* workspace, size_t ws_bytes, fpd_stream_t stream) {
   const int64_t n = (int64_t)B * J * hw;
   int nblocks = (int)((n + kThreads * 8 - 1) / (kThreads * 8));
   if (nblocks > 2048) nblocks = 2048;
@@ -168,6 +173,8 @@ int joints_mse(const float* out_nchw, const float* target_nchw, const float* tw,
   FPD_LAUNCH_CHECK();
   return FPD_OK;
 }
+
+}  // extern "C"
 
 // ---------------------------------------------------------------------------------------------------------------
 // Online hard keypoint mining (reference lib/core/loss.py:42-87, JointsOHKMMSELoss):
@@ -183,6 +190,7 @@ int joints_mse(const float* out_nchw, const float* target_nchw, const float* tw,
 //
 // Workspace: part double [B][nch][S][2][J] | contrib double [B][S][2] | coef float [B][S][2][J]
 // (nch = 64-pixel chunks per sample on the fused NHWC form, 1 on the NCHW module form).
+namespace fpd {
 namespace {
 
 constexpr int kMaxJ = 64;
@@ -437,6 +445,9 @@ OhkmWs ohkm_ws_split(void* ws, int64_t B, int64_t nch, int64_t S, int64_t J) {
 }
 
 }  // namespace
+}  // namespace fpd
+
+extern "C" {
 
 size_t fpd_loss_ohkm_workspace_bytes(int S, int B, int J, int h, int w) {
   const int64_t hw = (int64_t)h * w;
@@ -444,14 +455,16 @@ size_t fpd_loss_ohkm_workspace_bytes(int S, int B, int J, int h, int w) {
   return ohkm_ws_bytes(B, (hw + kPix - 1) / kPix, S, J);
 }
 
-size_t joints_ohkm_workspace_bytes(int B, int J) {
+size_t fpd_joints_ohkm_workspace_bytes(int B, int J) {
   if (B < 1 || J < 1) return 0;
   return ohkm_ws_bytes(B, 1, 1, J);
 }
 
-int fpd_loss_ohkm(const float* const* outs, int S, const float* target_nchw, const float* teacher_nhwc, const float* tw,
-                  float alpha, float* const* grads, float grad_scale, float* losses, int B, int J, int h, int w,
-                  int pose_topk, int kd_topk, void* workspace, size_t ws_bytes, cudaStream_t stream) {
+int fpd_loss_ohkm_fused(const float* const* outs, int S, const float* target_nchw, const float* teacher_nhwc,
+                        const float* tw, float alpha, float* const* grads, float grad_scale, float* losses, int B, int J,
+                        int h, int w, int pose_topk, int kd_topk, void* workspace, size_t ws_bytes,
+                        fpd_stream_t stream) {
+  FPD_REQUIRE(outs != nullptr, "fpd_loss_ohkm_fused: outs_host is NULL");
   FPD_REQUIRE(S >= 1 && S <= kMaxStacks, "fpd_loss_ohkm: S=%d out of range [1,%d]", S, kMaxStacks);
   FPD_REQUIRE(B >= 1, "fpd_loss_ohkm: B=%d (an empty batch has no loss)", B);
   FPD_REQUIRE(h >= 1 && w >= 1, "fpd_loss_ohkm: empty heat-map %dx%d", h, w);
@@ -494,8 +507,8 @@ int fpd_loss_ohkm(const float* const* outs, int S, const float* target_nchw, con
   return FPD_OK;
 }
 
-int joints_ohkm(const float* out_nchw, const float* target_nchw, const float* tw, int topk, float* loss3,
-                float* grad_out, int B, int J, int hw, void* workspace, size_t ws_bytes, cudaStream_t stream) {
+int fpd_joints_ohkm(const float* out_nchw, const float* target_nchw, const float* tw, int topk, float* loss3,
+                    float* grad_out, int B, int J, int hw, void* workspace, size_t ws_bytes, fpd_stream_t stream) {
   FPD_REQUIRE(out_nchw != nullptr && target_nchw != nullptr && loss3 != nullptr,
               "joints_ohkm: out, target or loss3 is NULL");
   FPD_REQUIRE(B >= 1, "joints_ohkm: B=%d (an empty batch has no loss)", B);
@@ -519,4 +532,4 @@ int joints_ohkm(const float* out_nchw, const float* target_nchw, const float* tw
   return FPD_OK;
 }
 
-}  // namespace fpd
+}  // extern "C"

@@ -14,8 +14,9 @@
 //    time: the 64 diagonal words are staged to shared memory, one thread resolves the chunk with register
 //    bit-ops, then the whole CTA ORs the kept rows into the running "removed" bitmap (coalesced reads).
 //    Only the keep list (<= n ints) and its length ever cross PCIe.
+#include <mutex>
+
 #include "common.cuh"
-#include "kernels.h"
 
 namespace fpd {
 namespace {
@@ -220,44 +221,17 @@ gaussian_target_kernel(const float* __restrict__ joints, const float* __restrict
   if (threadIdx.x == 0) target_weight[nj] = joints_weight ? v * joints_weight[j] : v;
 }
 
-}  // namespace
-
-size_t nms_workspace_bytes(int n) {
-  const size_t col_blocks = (size_t)(n + kT - 1) / kT;
-  return (size_t)n * col_blocks * sizeof(unsigned long long) + 256;
-}
-
-int nms_device(const float* boxes_sorted_dev, int n, int box_dim, float thresh, int* keep_dev, int* num_keep_dev,
-               void* workspace, size_t ws_bytes, cudaStream_t stream) {
-  FPD_REQUIRE(box_dim >= 4, "nms: box_dim=%d must be >= 4 (x1,y1,x2,y2[,score])", box_dim);
-  if (n <= 0) {
-    FPD_CUDA_CHECK(cudaMemsetAsync(num_keep_dev, 0, sizeof(int), stream));
-    return FPD_OK;
-  }
-  FPD_REQUIRE(ws_bytes >= nms_workspace_bytes(n), "nms: workspace too small");
-  const int col_blocks = (n + kT - 1) / kT;
-  FPD_REQUIRE(col_blocks <= 4096, "nms: n=%d too large", n);
-  unsigned long long* mask = (unsigned long long*)workspace;
-  const int tri = col_blocks * (col_blocks + 1) / 2;
-  nms_mask_kernel<<<tri, kT, 0, stream>>>(boxes_sorted_dev, n, box_dim, thresh, col_blocks, mask);
-  FPD_LAUNCH_CHECK();
-  const size_t smem = (size_t)(col_blocks + kT) * sizeof(unsigned long long);
-  nms_sweep_kernel<<<1, 1024, smem, stream>>>(mask, n, col_blocks, keep_dev, num_keep_dev);
-  FPD_LAUNCH_CHECK();
-  return FPD_OK;
-}
-
 template <typename T>
-static int oks_nms_device_t(const T* kpts, const double* areas, const double* vars_, int n, int J, double thresh, int use_vis,
-                            double in_vis_thre, int* keep_dev, int* num_keep_dev, void* workspace, size_t ws_bytes,
-                            cudaStream_t stream) {
+int oks_nms_device_t(const T* kpts, const double* areas, const double* vars_, int n, int J, double thresh, int use_vis,
+                     double in_vis_thre, int* keep_dev, int* num_keep_dev, void* workspace, size_t ws_bytes,
+                     cudaStream_t stream) {
   FPD_REQUIRE(J >= 1 && J <= kMaxJ, "oks_nms: J=%d must be in [1, %d]", J, kMaxJ);
   if (n <= 0) {
     FPD_CUDA_CHECK(cudaMemsetAsync(num_keep_dev, 0, sizeof(int), stream));
     return FPD_OK;
   }
   FPD_REQUIRE(kpts && areas && vars_, "oks_nms: null input");
-  FPD_REQUIRE(ws_bytes >= nms_workspace_bytes(n), "oks_nms: workspace too small");
+  FPD_REQUIRE(ws_bytes >= fpd_nms_workspace_bytes(n), "oks_nms: workspace too small");
   const int col_blocks = (n + kT - 1) / kT;
   FPD_REQUIRE(col_blocks <= 4096, "oks_nms: n=%d too large", n);
   unsigned long long* mask = (unsigned long long*)workspace;
@@ -270,17 +244,49 @@ static int oks_nms_device_t(const T* kpts, const double* areas, const double* va
   return FPD_OK;
 }
 
-int oks_nms_device(const void* kpts_sorted, int kpt_f64, const double* areas_sorted, const double* vars_, int n, int J,
-                   double thresh, int use_vis, double in_vis_thre, int* keep_dev, int* num_keep_dev, void* workspace,
-                   size_t ws_bytes, cudaStream_t stream) {
+}  // namespace
+}  // namespace fpd
+
+using namespace fpd;
+
+extern "C" {
+
+size_t fpd_nms_workspace_bytes(int n) {
+  const size_t col_blocks = (size_t)(n + kT - 1) / kT;
+  return (size_t)n * col_blocks * sizeof(unsigned long long) + 256;
+}
+
+int fpd_nms_device(const float* boxes_sorted_dev, int n, int box_dim, float thresh, int* keep_dev, int* num_keep_dev,
+                   void* workspace, size_t ws_bytes, fpd_stream_t stream) {
+  FPD_REQUIRE(box_dim >= 4, "nms: box_dim=%d must be >= 4 (x1,y1,x2,y2[,score])", box_dim);
+  if (n <= 0) {
+    FPD_CUDA_CHECK(cudaMemsetAsync(num_keep_dev, 0, sizeof(int), stream));
+    return FPD_OK;
+  }
+  FPD_REQUIRE(ws_bytes >= fpd_nms_workspace_bytes(n), "nms: workspace too small");
+  const int col_blocks = (n + kT - 1) / kT;
+  FPD_REQUIRE(col_blocks <= 4096, "nms: n=%d too large", n);
+  unsigned long long* mask = (unsigned long long*)workspace;
+  const int tri = col_blocks * (col_blocks + 1) / 2;
+  nms_mask_kernel<<<tri, kT, 0, stream>>>(boxes_sorted_dev, n, box_dim, thresh, col_blocks, mask);
+  FPD_LAUNCH_CHECK();
+  const size_t smem = (size_t)(col_blocks + kT) * sizeof(unsigned long long);
+  nms_sweep_kernel<<<1, 1024, smem, stream>>>(mask, n, col_blocks, keep_dev, num_keep_dev);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int fpd_oks_nms_device(const void* kpts_sorted, int kpt_f64, const double* areas_sorted, const double* vars_, int n,
+                       int J, double thresh, int use_vis, double in_vis_thre, int* keep_dev, int* num_keep_dev,
+                       void* workspace, size_t ws_bytes, fpd_stream_t stream) {
   return kpt_f64 ? oks_nms_device_t<double>((const double*)kpts_sorted, areas_sorted, vars_, n, J, thresh, use_vis,
                                             in_vis_thre, keep_dev, num_keep_dev, workspace, ws_bytes, stream)
                  : oks_nms_device_t<float>((const float*)kpts_sorted, areas_sorted, vars_, n, J, thresh, use_vis,
                                            in_vis_thre, keep_dev, num_keep_dev, workspace, ws_bytes, stream);
 }
 
-int oks_rescore(const void* kpts, int kpt_f64, const double* box_score, int n, int J, double in_vis_thre, double* out,
-                cudaStream_t stream) {
+int fpd_oks_rescore(const void* kpts, int kpt_f64, const double* box_score, int n, int J, double in_vis_thre,
+                    double* out, fpd_stream_t stream) {
   if (n <= 0) return FPD_OK;
   FPD_REQUIRE(kpts && box_score && out && J >= 1, "oks_rescore: bad arguments");
   if (kpt_f64) oks_rescore_kernel<double><<<(n + 127) / 128, 128, 0, stream>>>((const double*)kpts, box_score, n, J, in_vis_thre, out);
@@ -289,9 +295,9 @@ int oks_rescore(const void* kpts, int kpt_f64, const double* box_score, int n, i
   return FPD_OK;
 }
 
-int gaussian_targets(const float* joints, const float* joints_vis, const float* joints_weight, const float* gauss_table,
-                     float* target, float* target_weight, int N, int J, int H, int W, int image_w, int image_h, int sigma,
-                     cudaStream_t stream) {
+int fpd_gaussian_targets(const float* joints, const float* joints_vis, const float* joints_weight,
+                         const float* gauss_table, float* target, float* target_weight, int N, int J, int H, int W,
+                         int image_w, int image_h, int sigma, fpd_stream_t stream) {
   FPD_REQUIRE(joints && joints_vis && gauss_table && target && target_weight, "gaussian_targets: null pointer");
   FPD_REQUIRE(N >= 0 && J >= 1 && H >= 1 && W >= 1 && sigma >= 1, "gaussian_targets: bad sizes");
   if (N == 0) return FPD_OK;
@@ -301,4 +307,60 @@ int gaussian_targets(const float* joints, const float* joints_vis, const float* 
   return FPD_OK;
 }
 
-}  // namespace fpd
+int fpd_nms_host(int* keep_out, int* num_out, const float* boxes_host, int boxes_num, int boxes_dim, float thresh,
+                 int device_id) {
+  FPD_REQUIRE(keep_out && num_out, "fpd_nms_host: NULL output pointer");
+  if (boxes_num <= 0) {
+    *num_out = 0;
+    return FPD_OK;
+  }
+  FPD_REQUIRE(boxes_host != nullptr, "fpd_nms_host: boxes_host is NULL");
+  int cur = -1;
+  FPD_CUDA_CHECK(cudaGetDevice(&cur));
+  if (cur != device_id) FPD_CUDA_CHECK(cudaSetDevice(device_id));
+  // grow-only scratch (the reference signature has no workspace argument)
+  static std::mutex mu;
+  static void* scratch = nullptr;
+  static size_t scratch_bytes = 0;
+  static int scratch_dev = -1;
+  std::lock_guard<std::mutex> lock(mu);
+  const size_t boxes_bytes = (size_t)boxes_num * boxes_dim * sizeof(float);
+  const size_t boxes_pad = (boxes_bytes + 255) / 256 * 256;
+  const size_t keep_pad = ((size_t)boxes_num * sizeof(int) + 255) / 256 * 256;
+  const size_t need = boxes_pad + keep_pad + 256 + fpd_nms_workspace_bytes(boxes_num);
+  if (need > scratch_bytes || scratch_dev != device_id) {
+    if (scratch) cudaFree(scratch);
+    scratch = nullptr;
+    scratch_bytes = 0;
+    FPD_CUDA_CHECK(cudaMalloc(&scratch, need));
+    scratch_bytes = need;
+    scratch_dev = device_id;
+  }
+  char* base = (char*)scratch;
+  float* boxes_dev = (float*)base;
+  int* keep_dev = (int*)(base + boxes_pad);
+  int* num_dev = (int*)(base + boxes_pad + keep_pad);
+  void* ws = base + boxes_pad + keep_pad + 256;
+  cudaStream_t st = 0;
+  FPD_CUDA_CHECK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+  int rc = FPD_OK;
+  do {
+    if (cudaMemcpyAsync(boxes_dev, boxes_host, boxes_bytes, cudaMemcpyHostToDevice, st) != cudaSuccess) { rc = FPD_ERR_CUDA; break; }
+    rc = fpd_nms_device(boxes_dev, boxes_num, boxes_dim, thresh, keep_dev, num_dev, ws,
+                        fpd_nms_workspace_bytes(boxes_num), st);
+    if (rc) break;
+    if (cudaMemcpyAsync(num_out, num_dev, sizeof(int), cudaMemcpyDeviceToHost, st) != cudaSuccess) { rc = FPD_ERR_CUDA; break; }
+    if (cudaStreamSynchronize(st) != cudaSuccess) { rc = FPD_ERR_CUDA; break; }
+    if (*num_out > 0 &&
+        cudaMemcpy(keep_out, keep_dev, (size_t)(*num_out) * sizeof(int), cudaMemcpyDeviceToHost) != cudaSuccess) {
+      rc = FPD_ERR_CUDA;
+      break;
+    }
+  } while (0);
+  if (rc == FPD_ERR_CUDA) set_last_error("fpd_nms_host: CUDA failure: %s", cudaGetErrorString(cudaGetLastError()));
+  cudaStreamDestroy(st);
+  if (cur != device_id && cur >= 0) cudaSetDevice(cur);
+  return rc;
+}
+
+}  // extern "C"

@@ -99,7 +99,8 @@ int fpd_conv2d_tc_f16x1(const float* x, const float* pre_mean, const float* pre_
  * operand scale); stat_part (device double[stat_blocks][Cout][2] or NULL) and stat_pivot as fpd_conv2d_tc_h_stats.
  * fpd_conv2d_tc_f16x1_train_plan (host only, no device needed) returns the kernel a launch with (stats != 0) or
  * without statistics runs on, coded as fpd_conv2d_tc_f16x1_kernel (0: unsupported, including statistics with
- * Cout > 256), and writes to *stat_blocks (nullable) the number of partial blocks a statistics launch writes. */
+ * Cout > 256), and writes to *stat_blocks (nullable) the number of partial blocks a statistics launch writes (0 without
+ * statistics or when unsupported). */
 int fpd_conv2d_tc_f16x1_train_plan(int B, int H, int W, int Cin, int Cout, int ksize, int stats, int* stat_blocks);
 int fpd_conv2d_tc_f16x1_train(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
                               int pre_relu, const void* w, const float* bias, const float* residual,
@@ -132,7 +133,8 @@ int fpd_weight_prep_f16(const float* w_oihw, void* w_hi, void* w_lo, int O, int 
  * over the tensor that nn.BatchNorm2d (lib/models/hourglass.py:18-26) implies disappears. Arguments as fpd_conv2d_tc_h
  * (no relu_mask / in_scale: forward only); stat_part: device double[fpd_conv2d_tc_h_stats_blocks(...)][Cout][2];
  * stat_pivot: device float[Cout] or NULL, any per-channel value near the expected mean (improves conditioning only). */
-int fpd_conv2d_tc_h_stats_blocks(int B, int H, int W, int Cin, int Cout, int ksize, int f16);   /* 0 = shape not supported */
+/* 0: the shape cannot carry the statistics (unsupported, or e.g. Cout > 256) */
+int fpd_conv2d_tc_h_stats_blocks(int B, int H, int W, int Cin, int Cout, int ksize, int f16);
 int fpd_conv2d_tc_h_stats(const float* x, const float* pre_mean, const float* pre_scale, const float* pre_shift,
                           int pre_relu, const void* w_hi, const void* w_lo, int f16, const float* bias,
                           const float* residual, float* y, float out_scale, int B, int H, int W, int Cin, int Cout,
@@ -180,7 +182,9 @@ int fpd_conv2d_wgrad_tc_fused(const float* x, const float* pre_mean, const float
 /* 1 if fpd_conv2d_wgrad_tc_fused takes this 3x3 shape in one launch (the same rule as fpd_conv2d_wgrad_tc_supported). */
 int fpd_conv2d_wgrad_tc3_supported(int H, int W, int Cin, int Cout, int ksize);
 
-/* Generic fp32 CUDA-core convolution (any k/stride/pad): x NHWC [B,H,W,Cin], w OIHW. */
+/* Generic fp32 CUDA-core convolution (any k/stride/pad): x NHWC [B,H,W,Cin], w OIHW. Used for the shapes the tensor-core
+ * kernels do not take (7x7 stem, 16-channel score convs) and as the on-device cross-check in tests. In the data gradient
+ * H, W are the input size: dx [B,H,W,Cin]. */
 int fpd_conv2d_simt_fwd(const float* x, const float* w_oihw, const float* bias, const float* residual, float* y,
                         int B, int H, int W, int Cin, int Cout, int k, int stride, int pad, fpd_stream_t stream);
 int fpd_conv2d_simt_dgrad(const float* dy, const float* w_oihw, float* dx, int B, int H, int W, int Cin, int Cout,
@@ -200,7 +204,7 @@ int fpd_weight_prep(const float* w_oihw, float* w_hi, float* w_lo, int O, int I,
  * nn.Upsample(scale_factor=2) + add: lib/models/hourglass.py:18-28,34-50,60,82-91,117-124.
  * ------------------------------------------------------------------------------------------------- */
 size_t fpd_bn_stats_workspace_bytes(int64_t P, int C);
-/* per-channel batch mean and biased variance of x[P,C] */
+/* per-channel batch mean and biased variance of x[P,C] (per-chunk shifted sums, Chan merge in fp64) */
 int fpd_bn_stats(const float* x, int64_t P, int C, float* mean, float* var_biased, void* workspace,
                  size_t workspace_bytes, fpd_stream_t stream);
 /* Centred affine form used by every consumer: y = (x - mean) * scale + shift with
@@ -232,6 +236,7 @@ int fpd_upsample_bwd(const float* dout, float* dlow, int shift, int B, int H, in
 int fpd_im2col(const float* x, float* cols, int B, int H, int W, int Cin, int k, int stride, int pad, int Kpad,
                fpd_stream_t stream);
 size_t fpd_channel_reduce_workspace_bytes(int64_t P, int C);
+/* out[C] = scale * (sum over the P pixels of dy[P,C]) */
 int fpd_channel_sum(const float* dy, int64_t P, int C, float scale, float* out, void* workspace,
                     size_t workspace_bytes, fpd_stream_t stream);
 /* BN(+ReLU) backward: phase 1 reduces sums[0:C]=sum dz, sums[C:2C]=sum dz*xhat; phase 2 writes
@@ -249,6 +254,7 @@ int fpd_bn_bwd_apply_sum(const float* da, const float* x, const float* mean, con
 int fpd_bn_bwd_apply(const float* da, const float* x, const float* mean, const float* invstd, const float* scale,
                      const float* shift, const float* gamma, int relu, const float* sums, int accumulate, float* dx,
                      int64_t P, int C, fpd_stream_t stream);
+/* eval-mode (no batch statistics) BatchNorm(+ReLU) backward: dx (= or +=) da * relu mask * scale */
 int fpd_affine_act_bwd(const float* da, const float* x, const float* mean, const float* scale, const float* shift,
                        int relu, int accumulate, float* dx, int64_t P, int C, fpd_stream_t stream);
 int fpd_maxpool2x2_fwd(const float* x, float* y, int B, int H, int W, int C, fpd_stream_t stream);
@@ -301,6 +307,7 @@ int fpd_nchw_to_nhwc(const float* x, float* y, int B, int C, int H, int W, fpd_s
  * np.flip(input, 3)), so the second forward needs no separate flip pass. */
 int fpd_nchw_to_nhwc_flipw(const float* x_nchw, float* y_nhwc, int B, int C, int H, int W, fpd_stream_t stream);
 int fpd_nhwc_to_nchw(const float* x, float* y, int B, int C, int H, int W, fpd_stream_t stream);
+/* out = a + b over n floats (n % 4 == 0) */
 int fpd_add(const float* a, const float* b, float* out, int64_t n, fpd_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------
