@@ -108,6 +108,7 @@ _SIGNATURES = {
     "fpd_flip_merge_argmax": (c_int, [P, P, P, c_int, P, P, P, c_int, c_int, c_int, c_int, P]),
     "fpd_argmax_nchw": (c_int, [P, P, P, c_int, c_int, P]),
     "fpd_final_preds": (c_int, [P, P, P, P, c_int, P, c_int, c_int, c_int, c_int, P]),
+    "fpd_final_preds_dark": (c_int, [P, P, P, P, c_int, P, c_int, c_int, c_int, c_int, P]),
     "fpd_pck_counts": (c_int, [P, P, P, P, P, c_int, c_int, c_int, c_int, P]),
     "fpd_nms_workspace_bytes": (c_size_t, [c_int]),
     "fpd_nms_device": (c_int, [P, c_int, c_int, c_float, P, P, P, c_size_t, P]),
@@ -116,6 +117,7 @@ _SIGNATURES = {
                                    P]),
     "fpd_oks_rescore": (c_int, [P, c_int, P, c_int, c_int, ctypes.c_double, P, P]),
     "fpd_gaussian_targets": (c_int, [P, P, P, P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, P]),
+    "fpd_gaussian_targets_unbiased": (c_int, [P, P, P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, P]),
     "fpd_crop_affine_normalize": (c_int, [P, c_size_t, P, P, P, P, P, P, c_int, c_int, c_int, P]),
     "fpd_adam_flat": (c_int, [P, P, P, P, c_int64, c_float, c_float, c_float, c_float, c_float, c_int, c_float, P]),
 }

@@ -211,13 +211,15 @@ class DeviceCropLoader:
     """Iterates a DataLoader of raw_collate batches and yields (input [N,3,h,w], target [N,J,hh,hw], target_weight [N,J,1],
     meta): input and targets on the device, meta on the CPU -- the tuple function.train / fpd_train / validate expect.
     Per batch: the H2D copies, one crop launch and one TargetGenerator call. heatmap_size = (w, h) and sigma as
-    cfg.MODEL.HEATMAP_SIZE / SIGMA; joints_weight as the dataset's when LOSS.USE_DIFFERENT_JOINTS_WEIGHT."""
+    cfg.MODEL.HEATMAP_SIZE / SIGMA; joints_weight as the dataset's when LOSS.USE_DIFFERENT_JOINTS_WEIGHT; unbiased=True
+    builds DARK's unbiased targets (TargetGenerator)."""
 
-    def __init__(self, loader, heatmap_size, sigma, joints_weight=None, device=None):
+    def __init__(self, loader, heatmap_size, sigma, joints_weight=None, device=None, unbiased=False):
         self.loader = loader
         self.heatmap_size = (int(heatmap_size[0]), int(heatmap_size[1]))
         self.sigma = int(sigma)
         self.joints_weight = joints_weight
+        self.unbiased = bool(unbiased)
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         self._targets = {}
 
@@ -243,7 +245,7 @@ class DeviceCropLoader:
         gen = self._targets.get(out_size)
         if gen is None:
             gen = self._targets[out_size] = TargetGenerator(out_size, self.heatmap_size, self.sigma, self.joints_weight,
-                                                            self.device)
+                                                            self.device, unbiased=self.unbiased)
         target, target_weight = gen(dev['joints'], dev['joints_vis'])
         return inp, target, target_weight
 

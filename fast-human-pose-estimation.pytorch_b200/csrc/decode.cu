@@ -12,6 +12,8 @@
 //   lib/core/evaluate.py:16-71   accuracy: PCK@0.5 against the arg-max of the target heat-maps
 // Every floating-point step is an explicitly rounded intrinsic in the order the host (numpy / torch) evaluates it, so
 // the results are bit-identical to lib/core/inference.py::get_final_preds and lib/core/evaluate.py::accuracy.
+// final_preds_dark is the opt-in alternative to the quarter-pixel nudge: DARK's Taylor step on the log of the blurred
+// map (Zhang et al., "Distribution-Aware Coordinate Representation for Human Pose Estimation", CVPR 2020).
 #include "common.cuh"
 
 namespace fpd {
@@ -115,6 +117,18 @@ __device__ __forceinline__ void coords_from_argmax(int idx, float maxval, int w,
 // torch.sign: NaN -> 0
 __device__ __forceinline__ float sign_of(float d) { return (float)((0.f < d) - (d < 0.f)); }
 
+// preds[t] = (x, y) mapped by the heat-map -> image matrix T, and maxval.
+// transform_preds evaluates coords @ t[:, :2].T + t[:, 2] through numpy's matmul, whose OpenBLAS dgemm rounds x*t0,
+// adds y*t1 in one fused multiply-add, then adds t2. Plain multiply-then-add differs in the last double bit, and
+// now and then in the float32 result.
+__device__ __forceinline__ void store_pred(float* __restrict__ preds, int t, const double* __restrict__ T, float x,
+                                           float y, float mv) {
+  const double xd = x, yd = y;
+  preds[(int64_t)t * 3 + 0] = (float)__dadd_rn(__fma_rn(yd, T[1], __dmul_rn(xd, T[0])), T[2]);
+  preds[(int64_t)t * 3 + 1] = (float)__dadd_rn(__fma_rn(yd, T[4], __dmul_rn(xd, T[3])), T[5]);
+  preds[(int64_t)t * 3 + 2] = mv;
+}
+
 // get_final_preds: one thread per (b,j)
 __global__ void final_preds_kernel(const float* __restrict__ avg_nhwc, const int* __restrict__ idx,
                                    const float* __restrict__ maxval, const double* __restrict__ inv, int post_process,
@@ -137,14 +151,143 @@ __global__ void final_preds_kernel(const float* __restrict__ avg_nhwc, const int
     x = __fadd_rn(x, __fmul_rn(__fmul_rn(dx, ok), 0.25f));
     y = __fadd_rn(y, __fmul_rn(__fmul_rn(dy, ok), 0.25f));
   }
-  // transform_preds evaluates coords @ t[:, :2].T + t[:, 2] through numpy's matmul, whose OpenBLAS dgemm rounds x*t0,
-  // adds y*t1 in one fused multiply-add, then adds t2. Plain multiply-then-add differs in the last double bit, and
-  // now and then in the float32 result.
-  const double* T = inv + (int64_t)b * 6;
-  const double xd = x, yd = y;
-  preds[(int64_t)t * 3 + 0] = (float)__dadd_rn(__fma_rn(yd, T[1], __dmul_rn(xd, T[0])), T[2]);
-  preds[(int64_t)t * 3 + 1] = (float)__dadd_rn(__fma_rn(yd, T[4], __dmul_rn(xd, T[3])), T[5]);
-  preds[(int64_t)t * 3 + 2] = mv;
+  store_pred(preds, t, inv + (int64_t)b * 6, x, y, mv);
+}
+
+// ---- DARK decode (distribution-aware coordinates, Zhang et al., CVPR 2020): a second-order Taylor step on the log of
+// the Gaussian-blurred map at the arg-max. One CTA per (b,j) map, which it holds in shared memory with its blur along x.
+constexpr int kDarkThreads = 256;
+constexpr int kDarkMaxKernel = 15;
+// dynamic shared memory per block: sm_90's 227 KB opt-in less room for the kernel's static arrays (352 bytes), which
+// count against the same limit
+constexpr size_t kDarkSmemLimit = 226 * 1024;
+
+// np.max semantics (a NaN anywhere makes the result NaN); exact, so the reduction order cannot change the result
+__device__ __forceinline__ float nan_max(float m, float v) { return (v > m || v != v) ? v : m; }
+
+__device__ float block_nan_max(float v, float* red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = nan_max(v, __shfl_xor_sync(0xffffffffu, v, o));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float r = red[0];
+  for (int i = 1; i < kDarkThreads / 32; ++i) r = nan_max(r, red[i]);
+  return r;
+}
+
+// The 13 cells the derivatives read, as (dx, dy) around the arg-max, each offset + 2 in 3 bits:
+// 0 (0,0), 1 (+1,0), 2 (-1,0), 3 (+2,0), 4 (-2,0), 5 (0,+1), 6 (0,-1), 7 (0,+2), 8 (0,-2),
+// 9 (+1,+1), 10 (+1,-1), 11 (-1,+1), 12 (-1,-1)
+constexpr uint64_t kDarkCellX = 01133222204132ull;   // octal digits, cell 0 last
+constexpr uint64_t kDarkCellY = 01313041322222ull;
+
+__global__ void __launch_bounds__(kDarkThreads)
+final_preds_dark_kernel(const float* __restrict__ avg_nhwc, const int* __restrict__ idx, const float* __restrict__ maxval,
+                        const double* __restrict__ inv, int ksize, float* __restrict__ preds, int J, int h, int w) {
+  extern __shared__ float dark_sm[];
+  float* m = dark_sm;               // [h*w] the map
+  float* hb = dark_sm + h * w;      // [h*w] the map blurred along x
+  __shared__ double wk64[kDarkMaxKernel];
+  __shared__ float wk32[kDarkMaxKernel];
+  __shared__ float red[2][kDarkThreads / 32];
+  __shared__ double gwin[13];
+  const int t = blockIdx.x;
+  const int b = t / J, j = t - b * J;
+  const int hw = h * w, r = ksize / 2;
+  const float* src = avg_nhwc + (int64_t)b * hw * J + j;
+  float mmax = -INFINITY;
+  for (int p = threadIdx.x; p < hw; p += kDarkThreads) {
+    const float v = __ldg(src + (int64_t)p * J);
+    m[p] = v;
+    mmax = nan_max(mmax, v);
+  }
+  if (threadIdx.x == 0) {
+    // sigma_b = 0.3 ((k - 1) / 2 - 1) + 0.8, weights normalised to sum to 1
+    const double sigma = 0.3 * ((ksize - 1) * 0.5 - 1.0) + 0.8;
+    double sum = 0.0;
+    for (int i = 0; i < ksize; ++i) {
+      const double d = i - r;
+      wk64[i] = exp(-(d * d) / (2.0 * sigma * sigma));
+      sum += wk64[i];
+    }
+    for (int i = 0; i < ksize; ++i) {
+      wk64[i] /= sum;
+      wk32[i] = (float)wk64[i];
+    }
+  }
+  __syncthreads();
+  // max G over the whole map enters only through the 1e-10 clamp: fp32 is enough there
+  for (int p = threadIdx.x; p < hw; p += kDarkThreads) {
+    const int y = p / w, x = p - y * w;
+    float a = 0.f;
+    for (int i = 0; i < ksize; ++i) {
+      const int xx = x + i - r;
+      if (xx >= 0 && xx < w) a = fmaf(wk32[i], m[y * w + xx], a);
+    }
+    hb[p] = a;
+  }
+  __syncthreads();
+  float gmax = -INFINITY;
+  for (int p = threadIdx.x; p < hw; p += kDarkThreads) {
+    const int y = p / w, x = p - y * w;
+    float a = 0.f;
+    for (int i = 0; i < ksize; ++i) {
+      const int yy = y + i - r;
+      if (yy >= 0 && yy < h) a = fmaf(wk32[i], hb[yy * w + x], a);
+    }
+    gmax = nan_max(gmax, a);
+  }
+  mmax = block_nan_max(mmax, red[0]);
+  gmax = block_nan_max(gmax, red[1]);
+
+  const float mv = maxval[t];
+  float x, y;
+  coords_from_argmax(idx[t], mv, w, x, y);
+  const int x0 = (int)x, y0 = (int)y;
+  if (!(x0 >= 2 && x0 <= w - 3 && y0 >= 2 && y0 <= h - 3)) {
+    if (threadIdx.x == 0) store_pred(preds, t, inv + (int64_t)b * 6, x, y, mv);
+    return;
+  }
+  // G at the 13 cells in fp64, straight from the map (zero outside it), in a fixed order
+  if (threadIdx.x < 13) {
+    const int px = x0 + (int)((kDarkCellX >> (3 * threadIdx.x)) & 7) - 2;
+    const int py = y0 + (int)((kDarkCellY >> (3 * threadIdx.x)) & 7) - 2;
+    double g = 0.0;
+    for (int u = 0; u < ksize; ++u) {
+      const int yy = py + u - r;
+      if (yy < 0 || yy >= h) continue;
+      double row = 0.0;
+      for (int v = 0; v < ksize; ++v) {
+        const int xx = px + v - r;
+        if (xx >= 0 && xx < w) row = fma(wk64[v], (double)m[yy * w + xx], row);
+      }
+      g = fma(wk64[u], row, g);
+    }
+    gwin[threadIdx.x] = g;
+  }
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  // G *= max(M) / max(G) when max(G) > 0; L = log(max(G, 1e-10)), a NaN staying NaN
+  const double scale = gmax > 0.f ? (double)mmax / (double)gmax : 1.0;
+  double L[13];
+#pragma unroll
+  for (int i = 0; i < 13; ++i) {
+    const double g = gwin[i] * scale;
+    L[i] = log(g > 1e-10 || g != g ? g : 1e-10);
+  }
+  const double dx = 0.5 * (L[1] - L[2]), dy = 0.5 * (L[5] - L[6]);
+  const double dxx = 0.25 * (L[3] - 2.0 * L[0] + L[4]), dyy = 0.25 * (L[7] - 2.0 * L[0] + L[8]);
+  const double dxy = 0.25 * (L[9] - L[10] - L[11] + L[12]);
+  const double det = dxx * dyy - dxy * dxy;
+  if (det != 0.0) {
+    // offset = -H^-1 (dx, dy), H = [[dxx, dxy], [dxy, dyy]]
+    const double ox = -(dyy * dx - dxy * dy) / det, oy = -(dxx * dy - dxy * dx) / det;
+    if (isfinite(ox) && isfinite(oy)) {
+      x = (float)(x0 + ox);
+      y = (float)(y0 + oy);
+    }
+  }
+  store_pred(preds, t, inv + (int64_t)b * 6, x, y, mv);
 }
 
 // accuracy(): one warp per (b,j) takes the target's arg-max, lane 0 compares it with the prediction's and adds the
@@ -211,6 +354,24 @@ int fpd_final_preds(const float* avg_nhwc, const int* idx, const float* maxval, 
   const int BJ = B * J, threads = 128;
   final_preds_kernel<<<(BJ + threads - 1) / threads, threads, 0, stream>>>(avg_nhwc, idx, maxval, inv, post_process,
                                                                            preds, BJ, J, h, w);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int fpd_final_preds_dark(const float* avg_nhwc, const int* idx, const float* maxval, const double* inv, int blur_kernel,
+                         float* preds, int B, int J, int h, int w, fpd_stream_t stream) {
+  FPD_REQUIRE(B >= 0 && J >= 1 && J <= 64, "final_preds_dark: B=%d J=%d out of range", B, J);
+  FPD_REQUIRE(h >= 5 && w >= 5, "final_preds_dark: needs a heat-map of at least 5x5, got %dx%d", h, w);
+  FPD_REQUIRE(blur_kernel >= 3 && blur_kernel <= kDarkMaxKernel && blur_kernel % 2 == 1,
+              "final_preds_dark: blur_kernel=%d must be odd and in [3, %d]", blur_kernel, kDarkMaxKernel);
+  FPD_REQUIRE(avg_nhwc && idx && maxval && inv && preds, "final_preds_dark: null pointer");
+  const size_t smem = (size_t)2 * h * w * sizeof(float);
+  FPD_REQUIRE(smem <= kDarkSmemLimit, "final_preds_dark: a %dx%d heat-map does not fit in shared memory", h, w);
+  if (B == 0) return FPD_OK;
+  if (smem > 48 * 1024)
+    FPD_CUDA_CHECK(cudaFuncSetAttribute(final_preds_dark_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        (int)kDarkSmemLimit));
+  final_preds_dark_kernel<<<B * J, kDarkThreads, smem, stream>>>(avg_nhwc, idx, maxval, inv, blur_kernel, preds, J, h, w);
   FPD_LAUNCH_CHECK();
   return FPD_OK;
 }

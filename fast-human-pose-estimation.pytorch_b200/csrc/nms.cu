@@ -221,6 +221,36 @@ gaussian_target_kernel(const float* __restrict__ joints, const float* __restrict
   if (threadIdx.x == 0) target_weight[nj] = joints_weight ? v * joints_weight[j] : v;
 }
 
+// Unbiased targets (DARK, Zhang et al., CVPR 2020): the Gaussian on the sub-pixel centre mu = joint * (W / image_w,
+// H / image_h), evaluated in double at every pixel of the map. Visibility as gaussian_target_kernel, on the unrounded
+// window ul = mu - 3 sigma, br = mu + 3 sigma + 1.
+__global__ void __launch_bounds__(256)
+gaussian_target_unbiased_kernel(const float* __restrict__ joints, const float* __restrict__ joints_vis,
+                                const float* __restrict__ joints_weight, float* __restrict__ target,
+                                float* __restrict__ target_weight, int J, int H, int W, double scale_x, double scale_y,
+                                double sigma) {
+  const int nj = blockIdx.x;
+  const int j = nj % J;
+  const float* jt = joints + (size_t)nj * 3;
+  const double mu_x = (double)jt[0] * scale_x, mu_y = (double)jt[1] * scale_y;
+  const double rad = 3.0 * sigma, den = 2.0 * sigma * sigma;
+  float v = joints_vis[(size_t)nj * 3];
+  const bool oob = mu_x - rad >= W || mu_y - rad >= H || mu_x + rad + 1.0 < 0.0 || mu_y + rad + 1.0 < 0.0;
+  if (oob) v = 0.f;
+  const bool stamp = !oob && v > 0.5f;
+  float* tg = target + (size_t)nj * H * W;
+  for (int p = threadIdx.x; p < H * W; p += blockDim.x) {
+    const int y = p / W, x = p - y * W;
+    float o = 0.f;
+    if (stamp) {
+      const double dx = x - mu_x, dy = y - mu_y;
+      o = (float)exp(-(dx * dx + dy * dy) / den);
+    }
+    tg[p] = o;
+  }
+  if (threadIdx.x == 0) target_weight[nj] = joints_weight ? v * joints_weight[j] : v;
+}
+
 template <typename T>
 int oks_nms_device_t(const T* kpts, const double* areas, const double* vars_, int n, int J, double thresh, int use_vis,
                      double in_vis_thre, int* keep_dev, int* num_keep_dev, void* workspace, size_t ws_bytes,
@@ -303,6 +333,20 @@ int fpd_gaussian_targets(const float* joints, const float* joints_vis, const flo
   if (N == 0) return FPD_OK;
   gaussian_target_kernel<<<N * J, 256, 0, stream>>>(joints, joints_vis, joints_weight, gauss_table, target, target_weight, J,
                                                     H, W, (double)image_w / W, (double)image_h / H, sigma * 3);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int fpd_gaussian_targets_unbiased(const float* joints, const float* joints_vis, const float* joints_weight, float* target,
+                                  float* target_weight, int N, int J, int H, int W, int image_w, int image_h, int sigma,
+                                  fpd_stream_t stream) {
+  FPD_REQUIRE(joints && joints_vis && target && target_weight, "gaussian_targets_unbiased: null pointer");
+  FPD_REQUIRE(N >= 0 && J >= 1 && H >= 1 && W >= 1 && image_w >= 1 && image_h >= 1 && sigma >= 1,
+              "gaussian_targets_unbiased: bad sizes");
+  if (N == 0) return FPD_OK;
+  gaussian_target_unbiased_kernel<<<N * J, 256, 0, stream>>>(joints, joints_vis, joints_weight, target, target_weight, J,
+                                                             H, W, (double)W / image_w, (double)H / image_h,
+                                                             (double)sigma);
   FPD_LAUNCH_CHECK();
   return FPD_OK;
 }

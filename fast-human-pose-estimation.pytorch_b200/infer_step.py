@@ -9,14 +9,23 @@ one pixel, average, D2H of the merged heat-maps, numpy arg-max. Here, per batch:
                    fused flip_back + shift + average + arg-max -> idx[B,J], maxval[B,J] (+ merged heat-maps)
                    [optional box NMS of the detector boxes that produced the crops: lib/nms, csrc/nms.cu]
                    [decode=True: merged map -> NCHW -> JointsMSELoss or JointsOHKMMSELoss (loss3), get_final_preds
-                    (preds), accuracy() counts (pck), all on the device, bit-identical to lib/core/function.py's eager
-                    route] }
+                    (preds; DARK's decode with post_process="dark"), accuracy() counts (pck), all on the device,
+                    bit-identical to lib/core/function.py's eager route] }
 
 Only [B,J] indices and maxima (or [B,J,3] predictions, 3 loss floats and [J,2] counts) need to cross PCIe. The module must be one of fpd_b200.lib.models (hourglass / pose_hrnet).
 """
 import torch
 
 from . import ops
+
+
+def _post_process(post_process):
+    """The decode a post_process argument selects: "dark", or a bool (the quarter-pixel nudge or none)."""
+    if isinstance(post_process, str):
+        if post_process != "dark":
+            raise ValueError("post_process must be a bool or 'dark', got %r" % (post_process,))
+        return post_process
+    return bool(post_process)
 
 
 class FlipTestInference:
@@ -85,12 +94,15 @@ class FlipTestInference:
                 res["loss3"], _ = ops.joints_ohkm_mse(out_nchw, extra["target"], tw, extra["topk"], want_grad=False)
             else:
                 res["loss3"], _ = ops.joints_mse(out_nchw, extra["target"], tw, want_grad=False)
-            res["preds"] = ops.final_preds(avg, idx, maxval, extra["inv"], extra["post_process"])
+            if extra["post_process"] == "dark":
+                res["preds"] = ops.final_preds_dark(avg, idx, maxval, extra["inv"], extra["blur_kernel"])
+            else:
+                res["preds"] = ops.final_preds(avg, idx, maxval, extra["inv"], extra["post_process"])
             res["pck"], _ = ops.pck_counts(idx, maxval, extra["target"])
         self._keep = (ctx, ctx_f, nhwc, out_nchw)      # every intermediate stays referenced: the graph pool never recycles them
         return res
 
-    def _extra(self, inv, target, target_weight, use_target_weight, post_process, topk, static):
+    def _extra(self, inv, target, target_weight, use_target_weight, post_process, topk, blur_kernel, static):
         """The decode stage's inputs on the device: fresh copies, or refills of the graph's static buffers."""
         if not self.decode:
             return None
@@ -104,8 +116,8 @@ class FlipTestInference:
                 return torch.empty(tuple(t.shape), dtype=dtype, device=dev).copy_(t)
             return {"inv": own(inv, torch.float64), "target": own(target, torch.float32),
                     "target_weight": own(target_weight, torch.float32),
-                    "use_target_weight": bool(use_target_weight), "post_process": bool(post_process),
-                    "topk": int(topk)}
+                    "use_target_weight": bool(use_target_weight), "post_process": _post_process(post_process),
+                    "topk": int(topk), "blur_kernel": int(blur_kernel)}
         static["inv"].copy_(inv, non_blocking=True)
         static["target"].copy_(target, non_blocking=True)
         static["target_weight"].copy_(target_weight, non_blocking=True)
@@ -137,12 +149,13 @@ class FlipTestInference:
         self._staged_for = next_x
 
     def __call__(self, x, boxes_sorted=None, nms_thresh=0.6, next_x=None, inv=None, target=None, target_weight=None,
-                 use_target_weight=True, post_process=True, topk=0):
+                 use_target_weight=True, post_process=True, topk=0, blur_kernel=11):
         """x: [B,3,H,W] fp32, CUDA or pinned host. boxes_sorted: optional device [n,5] detector boxes sorted by score.
         next_x: optional pinned host tensor = the NEXT batch (its H2D copy overlaps this batch; pass it as `x` next time).
         With decode=True: inv host float64 [B,6] heat-map -> image matrices (lib.core.inference.inverse_affines of the
         batch's centres / scales), target [B,J,h,w] and target_weight [B,J,1] (host or device), use_target_weight (the
-        criterion's), post_process (config.TEST.POST_PROCESS) and topk (the JointsOHKMMSELoss criterion's topk; 0 for
+        criterion's), post_process (config.TEST.POST_PROCESS; "dark" decodes with ops.final_preds_dark and a
+        blur_kernel-tap blur instead of the quarter-pixel nudge) and topk (the JointsOHKMMSELoss criterion's topk; 0 for
         JointsMSELoss).
         Returns a dict of DEVICE tensors (static across calls in graph mode): idx int32 [B,J] (flat arg-max, first maximum),
         maxval [B,J], avg_nhwc [B,h,w,J] merged heat-maps, nms_keep / nms_num; with decode=True also preds [B,J,3]
@@ -152,18 +165,19 @@ class FlipTestInference:
         if not self.use_graph:
             xd = x.cuda(non_blocking=True).float().contiguous()
             return self._body(xd, boxes_sorted, self._extra(inv, target, target_weight, use_target_weight, post_process,
-                                                            topk, None))
+                                                            topk, blur_kernel, None))
         shape = (tuple(x.shape), None if boxes_sorted is None else tuple(boxes_sorted.shape), self.nms_thresh)
         if self.decode:
-            shape += (tuple(target.shape), tuple(target_weight.shape), bool(use_target_weight), bool(post_process),
-                      int(topk))
+            shape += (tuple(target.shape), tuple(target_weight.shape), bool(use_target_weight),
+                      _post_process(post_process), int(topk), int(blur_kernel))
         gen = self.net.engine().generation
         if self.graph is None or shape != self._shape or gen != self._gen:
             xd = x.cuda(non_blocking=True).float().contiguous()
             self.static_x = torch.empty_like(xd)
             self.static_x.copy_(xd)
             self.static_boxes = None if boxes_sorted is None else boxes_sorted.clone()
-            self.static_extra = self._extra(inv, target, target_weight, use_target_weight, post_process, topk, None)
+            self.static_extra = self._extra(inv, target, target_weight, use_target_weight, post_process, topk, blur_kernel,
+                                            None)
             side = torch.cuda.Stream()
             side.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(side):
@@ -181,7 +195,7 @@ class FlipTestInference:
         self._stage(x)
         if boxes_sorted is not None:
             self.static_boxes.copy_(boxes_sorted, non_blocking=True)
-        self._extra(inv, target, target_weight, use_target_weight, post_process, topk, self.static_extra)
+        self._extra(inv, target, target_weight, use_target_weight, post_process, topk, blur_kernel, self.static_extra)
         self.graph.replay()
         self._prefetch(next_x)
         return self.result

@@ -88,13 +88,32 @@ def transform_preds(coords, center, scale, output_size):
     return out
 
 
+def use_dark(config):
+    """config.TEST.DARK: DARK's decode (ops.final_preds_dark) replaces the quarter-pixel nudge where POST_PROCESS is on."""
+    return bool(config.TEST.POST_PROCESS) and bool(getattr(config.TEST, "DARK", False))
+
+
+def blur_kernel(config):
+    """config.TEST.BLUR_KERNEL: the size of DARK's Gaussian blur (odd, 3..15)."""
+    return int(getattr(config.TEST, "BLUR_KERNEL", 11))
+
+
 def get_final_preds(config, batch_heatmaps, center, scale):
-    """inference.py:49-79: arg-max, optional quarter-pixel nudge toward the higher neighbour, map back to
-    image coordinates. batch_heatmaps: CUDA tensor or numpy [B,J,h,w]."""
+    """inference.py:49-79: arg-max, optional quarter-pixel nudge toward the higher neighbour (or, with
+    config.TEST.DARK, DARK's Taylor step), map back to image coordinates. batch_heatmaps: CUDA tensor or numpy
+    [B,J,h,w]."""
     if isinstance(batch_heatmaps, np.ndarray):
         batch_heatmaps = torch.from_numpy(np.ascontiguousarray(batch_heatmaps)).cuda()
     hm = batch_heatmaps.contiguous().float()
     B, J, H, W = hm.shape
+    if use_dark(config):
+        # the kernel validate()'s graph route runs, on the same map: both routes give the same bits
+        from fpd_b200 import ops
+        nhwc = ops.nchw_to_nhwc(hm)
+        _, idx, maxvals = ops.flip_merge_argmax(nhwc, want_avg=False)
+        inv = torch.from_numpy(inverse_affines(center, scale, [W, H])).to(hm.device)
+        preds = ops.final_preds_dark(nhwc, idx, maxvals, inv, blur_kernel(config)).cpu().numpy()
+        return preds[..., :2].copy(), preds[..., 2:].copy()
     idx, maxvals = _device_argmax(hm)
     coords, maxvals_np = preds_from_argmax(idx.cpu().numpy(), maxvals.cpu().numpy(), W)
     if config.TEST.POST_PROCESS:

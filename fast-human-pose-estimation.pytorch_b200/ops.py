@@ -858,6 +858,20 @@ def final_preds(avg_nhwc, idx, maxval, inv, post_process, out=None):
     return preds
 
 
+def final_preds_dark(avg_nhwc, idx, maxval, inv, blur_kernel=11, out=None):
+    """final_preds with DARK's sub-pixel decode (csrc/decode.cu) in place of the quarter-pixel nudge: a Taylor step on
+    the log of the map blurred by a blur_kernel-tap Gaussian (odd, 3..15). Same arguments otherwise; returns preds
+    [B,J,3] = (x, y, maxval) in image coordinates."""
+    _chk(avg_nhwc, "avg_nhwc")
+    B, h, w, J = avg_nhwc.shape
+    if not (inv.is_cuda and inv.dtype == torch.float64 and inv.is_contiguous() and tuple(inv.shape) == (B, 6)):
+        raise ValueError("inv must be a contiguous float64 CUDA tensor of shape (%d, 6)" % B)
+    preds = out if out is not None else torch.empty((B, J, 3), dtype=torch.float32, device=avg_nhwc.device)
+    N.check(N.lib().fpd_final_preds_dark(_p(avg_nhwc), _p(idx), _p(maxval), _p(inv), int(blur_kernel), _p(preds), B, J,
+                                         h, w, _stream()), "final_preds_dark")
+    return preds
+
+
 def pck_counts(idx, maxval, target_nchw, want_pred_hm=False, out=None):
     """accuracy() counts on the device (csrc/decode.cu): int32 [J,2] = {valid, hit} per joint, plus the prediction in
     heat-map coordinates [B,J,2] when want_pred_hm (else None). lib.core.evaluate.pck_from_counts turns the counts into
@@ -952,6 +966,23 @@ def gaussian_targets(joints, joints_vis, heatmap_size, image_size, sigma=2, join
     jw = None if joints_weight is None else joints_weight.to(dev).float().contiguous().reshape(-1)
     N.check(N.lib().fpd_gaussian_targets(_p(joints), _p(joints_vis), _p(jw), _p(gauss_table), _p(target), _p(tw), n, J, H, W,
                                          int(image_size[0]), int(image_size[1]), int(sigma), _stream()), "gaussian_targets")
+    return target, tw
+
+
+def gaussian_targets_unbiased(joints, joints_vis, heatmap_size, image_size, sigma=2, joints_weight=None):
+    """gaussian_targets with DARK's unbiased encoding: the Gaussian on the sub-pixel joint joint * heatmap_size /
+    image_size rather than on the rounded one, over the whole map. Same arguments (no table) and results."""
+    _chk(joints, "joints")
+    _chk(joints_vis, "joints_vis")
+    n, J = joints.shape[0], joints.shape[1]
+    W, H = int(heatmap_size[0]), int(heatmap_size[1])
+    dev = joints.device
+    target = torch.empty((n, J, H, W), dtype=torch.float32, device=dev)
+    tw = torch.empty((n, J, 1), dtype=torch.float32, device=dev)
+    jw = None if joints_weight is None else joints_weight.to(dev).float().contiguous().reshape(-1)
+    N.check(N.lib().fpd_gaussian_targets_unbiased(_p(joints), _p(joints_vis), _p(jw), _p(target), _p(tw), n, J, H, W,
+                                                  int(image_size[0]), int(image_size[1]), int(sigma), _stream()),
+            "gaussian_targets_unbiased")
     return target, tw
 
 

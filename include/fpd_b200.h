@@ -365,6 +365,14 @@ int fpd_argmax_nchw(const float* hm_nchw, int* idx, float* maxval, int BJ, int h
  * maxval). J <= 64. */
 int fpd_final_preds(const float* avg_nhwc, const int* idx, const float* maxval, const double* inv, int post_process,
                     float* preds, int B, int J, int h, int w, fpd_stream_t stream);
+/* fpd_final_preds with DARK's sub-pixel decode (Zhang et al., CVPR 2020) in place of the quarter-pixel nudge: each map is
+ * blurred by a normalised blur_kernel-tap separable Gaussian (sigma = 0.3 ((blur_kernel - 1) / 2 - 1) + 0.8, zeros
+ * outside the map), rescaled to the map's maximum, and at an arg-max at least 2 cells inside every border the coordinate
+ * moves by -H^-1 grad of log(max(G, 1e-10)) (central differences, computed in double; no move when det H = 0 or the
+ * offset is not finite). blur_kernel: odd, in [3, 15]. h, w >= 5, 2 h w floats must fit in shared memory; J <= 64.
+ * preds[..., 2] = maxval. Deterministic: no atomics. */
+int fpd_final_preds_dark(const float* avg_nhwc, const int* idx, const float* maxval, const double* inv, int blur_kernel,
+                         float* preds, int B, int J, int h, int w, fpd_stream_t stream);
 /* accuracy(), lib/core/evaluate.py:16-71, as per-joint counts: the arg-max of each target map target_nchw [B,J,h,w]
  * against the prediction's idx / maxval [B,J]. counts: device int32[J,2] = {joints whose target lies at x > 1 and
  * y > 1, those of them within 0.5 of the target after normalising x by h/10 and y by w/10}; zeroed by the call.
@@ -408,6 +416,13 @@ int fpd_oks_rescore(const void* kpts, int kpt_f64, const double* box_score, int 
 int fpd_gaussian_targets(const float* joints, const float* joints_vis, const float* joints_weight, const float* gauss_table,
                          float* target, float* target_weight, int N, int J, int H, int W, int image_w, int image_h,
                          int sigma, fpd_stream_t stream);
+/* Unbiased targets (DARK, Zhang et al., CVPR 2020), same arguments without the table: the Gaussian
+ * exp(-|p - mu|^2 / (2 sigma^2)) on the unrounded centre mu = joint * (W / image_w, H / image_h), at every pixel of the
+ * map. A joint whose window mu - 3 sigma .. mu + 3 sigma + 1 lies outside the map gets weight 0 and an all-zero map;
+ * joints_vis and joints_weight act as in fpd_gaussian_targets. */
+int fpd_gaussian_targets_unbiased(const float* joints, const float* joints_vis, const float* joints_weight, float* target,
+                                  float* target_weight, int N, int J, int H, int W, int image_w, int image_h, int sigma,
+                                  fpd_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------
  * Input crop. Replaces the per-sample cv2.warpAffine(INTER_LINEAR) + ToTensor + Normalize of
