@@ -118,6 +118,7 @@ _SIGNATURES = {
     "fpd_oks_rescore": (c_int, [P, c_int, P, c_int, c_int, ctypes.c_double, P, P]),
     "fpd_gaussian_targets": (c_int, [P, P, P, P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, P]),
     "fpd_gaussian_targets_unbiased": (c_int, [P, P, P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, P]),
+    "fpd_gaussian_targets_udp": (c_int, [P, P, P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, P]),
     "fpd_crop_affine_normalize": (c_int, [P, c_size_t, P, P, P, P, P, P, c_int, c_int, c_int, P]),
     "fpd_adam_flat": (c_int, [P, P, P, P, c_int64, c_float, c_float, c_float, c_float, c_float, c_int, c_float, P]),
 }

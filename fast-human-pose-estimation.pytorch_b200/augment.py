@@ -51,6 +51,23 @@ def crop_matrix(center, scale, rot, output_size):
     return cv2.getAffineTransform(np.float32(src), np.float32(dst))
 
 
+def udp_crop_matrix(center, scale, rot, output_size):
+    """The forward 2x3 crop matrix of UDP (unbiased data processing, Huang et al., CVPR 2020), in float64 and closed
+    form. Sizes are pixel spacings and positions pixel centres: rotate about `center` by `rot` degrees, in crop_matrix's
+    direction; scale each axis by (output_size - 1) / (scale * 200); move `center` to ((w - 1) / 2, (h - 1) / 2). The
+    box edges then land on the first and last output pixel centres, and mirroring the image (x -> width - 1 - x, the
+    centre with it) mirrors the crop (x -> w - 1 - x) when rot = 0."""
+    box = np.broadcast_to(np.asarray(scale, np.float64).reshape(-1), (2,)) * 200.0
+    kx, ky = (output_size[0] - 1.0) / box[0], (output_size[1] - 1.0) / box[1]
+    rot_rad = np.pi * rot / 180
+    sn, cs = np.sin(rot_rad), np.cos(rot_rad)
+    m = np.array([[kx * cs, kx * sn, 0.0], [-ky * sn, ky * cs, 0.0]])
+    cx, cy = float(center[0]), float(center[1])
+    m[0, 2] = (output_size[0] - 1.0) * 0.5 - (m[0, 0] * cx + m[0, 1] * cy)
+    m[1, 2] = (output_size[1] - 1.0) * 0.5 - (m[1, 0] * cx + m[1, 1] * cy)
+    return m
+
+
 def invert_affine(m):
     """cv2.invertAffineTransform of a float64 2x3 matrix, in the same operation order (and so the same bits); it is also
     the inversion warpAffine applies internally."""
@@ -116,10 +133,14 @@ class RawJointsDataset(torch.utils.data.Dataset):
         inv         float64 [2, 3]: output -> image coordinates
         joints, joints_vis: float64 [J, 3], transformed as the reference transforms them
         meta        the reference's meta dict
+
+    udp=True crops with udp_crop_matrix instead of the reference's matrix, for UDP training and validation; pair it with
+    DeviceCropLoader(..., udp=True) and, for validation, TEST.UDP.
     """
 
-    def __init__(self, base):
+    def __init__(self, base, udp=False):
         self.base = base
+        self.udp = bool(udp)
         self.mean, self.std = _normalize_of(base.transform)
         self.image_size = (int(base.image_size[0]), int(base.image_size[1]))
 
@@ -160,7 +181,7 @@ class RawJointsDataset(torch.utils.data.Dataset):
                 flipped = True
                 joints, joints_vis = _flip_joints(joints, joints_vis, img.shape[1], b.flip_pairs)
                 c[0] = img.shape[1] - c[0] - 1
-        trans = crop_matrix(c, s, r, b.image_size)
+        trans = (udp_crop_matrix if self.udp else crop_matrix)(c, s, r, b.image_size)
         inv = invert_affine(trans)
         img_h, img_w = img.shape[:2]
         x0, y0, x1, y1 = source_window(inv, self.image_size, img_w, img_h)
@@ -212,14 +233,18 @@ class DeviceCropLoader:
     meta): input and targets on the device, meta on the CPU -- the tuple function.train / fpd_train / validate expect.
     Per batch: the H2D copies, one crop launch and one TargetGenerator call. heatmap_size = (w, h) and sigma as
     cfg.MODEL.HEATMAP_SIZE / SIGMA; joints_weight as the dataset's when LOSS.USE_DIFFERENT_JOINTS_WEIGHT; unbiased=True
-    builds DARK's unbiased targets (TargetGenerator)."""
+    builds DARK's unbiased targets, udp=True UDP's targets for a RawJointsDataset(udp=True) loader (TargetGenerator;
+    not both)."""
 
-    def __init__(self, loader, heatmap_size, sigma, joints_weight=None, device=None, unbiased=False):
+    def __init__(self, loader, heatmap_size, sigma, joints_weight=None, device=None, unbiased=False, udp=False):
+        if unbiased and udp:
+            raise ValueError("DeviceCropLoader: unbiased (DARK) and udp are two different target encodings; pick one")
         self.loader = loader
         self.heatmap_size = (int(heatmap_size[0]), int(heatmap_size[1]))
         self.sigma = int(sigma)
         self.joints_weight = joints_weight
         self.unbiased = bool(unbiased)
+        self.udp = bool(udp)
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         self._targets = {}
 
@@ -245,7 +270,7 @@ class DeviceCropLoader:
         gen = self._targets.get(out_size)
         if gen is None:
             gen = self._targets[out_size] = TargetGenerator(out_size, self.heatmap_size, self.sigma, self.joints_weight,
-                                                            self.device, unbiased=self.unbiased)
+                                                            self.device, unbiased=self.unbiased, udp=self.udp)
         target, target_weight = gen(dev['joints'], dev['joints_vis'])
         return inp, target, target_weight
 

@@ -251,6 +251,39 @@ gaussian_target_unbiased_kernel(const float* __restrict__ joints, const float* _
   if (threadIdx.x == 0) target_weight[nj] = joints_weight ? v * joints_weight[j] : v;
 }
 
+// UDP targets (unbiased data processing, Huang et al., CVPR 2020). Sizes are pixel spacings, so the stride is
+// (image - 1) / (map - 1) per axis and the centre mu = joint / stride is not rounded. The window and the visibility
+// rule are gaussian_target_kernel's, around the rounded centre int(mu + 0.5); inside the window the Gaussian on the
+// unrounded centre is evaluated in double.
+__global__ void __launch_bounds__(256)
+gaussian_target_udp_kernel(const float* __restrict__ joints, const float* __restrict__ joints_vis,
+                           const float* __restrict__ joints_weight, float* __restrict__ target,
+                           float* __restrict__ target_weight, int J, int H, int W, double stride_x, double stride_y,
+                           int tmp, double sigma) {
+  const int nj = blockIdx.x;
+  const int j = nj % J;
+  const float* jt = joints + (size_t)nj * 3;
+  const double mu_x = (double)jt[0] / stride_x, mu_y = (double)jt[1] / stride_y;
+  const int cx = (int)(mu_x + 0.5), cy = (int)(mu_y + 0.5);
+  const int ulx = cx - tmp, uly = cy - tmp, brx = cx + tmp + 1, bry = cy + tmp + 1;
+  const double den = 2.0 * sigma * sigma;
+  float v = joints_vis[(size_t)nj * 3];
+  const bool oob = ulx >= W || uly >= H || brx < 0 || bry < 0;
+  if (oob) v = 0.f;
+  const bool stamp = !oob && v > 0.5f;
+  float* tg = target + (size_t)nj * H * W;
+  for (int p = threadIdx.x; p < H * W; p += blockDim.x) {
+    const int y = p / W, x = p - y * W;
+    float o = 0.f;
+    if (stamp && x >= ulx && x < brx && y >= uly && y < bry) {
+      const double dx = x - mu_x, dy = y - mu_y;
+      o = (float)exp(-(dx * dx + dy * dy) / den);
+    }
+    tg[p] = o;
+  }
+  if (threadIdx.x == 0) target_weight[nj] = joints_weight ? v * joints_weight[j] : v;
+}
+
 template <typename T>
 int oks_nms_device_t(const T* kpts, const double* areas, const double* vars_, int n, int J, double thresh, int use_vis,
                      double in_vis_thre, int* keep_dev, int* num_keep_dev, void* workspace, size_t ws_bytes,
@@ -347,6 +380,20 @@ int fpd_gaussian_targets_unbiased(const float* joints, const float* joints_vis, 
   gaussian_target_unbiased_kernel<<<N * J, 256, 0, stream>>>(joints, joints_vis, joints_weight, target, target_weight, J,
                                                              H, W, (double)W / image_w, (double)H / image_h,
                                                              (double)sigma);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int fpd_gaussian_targets_udp(const float* joints, const float* joints_vis, const float* joints_weight, float* target,
+                             float* target_weight, int N, int J, int H, int W, int image_w, int image_h, int sigma,
+                             fpd_stream_t stream) {
+  FPD_REQUIRE(joints && joints_vis && target && target_weight, "gaussian_targets_udp: null pointer");
+  FPD_REQUIRE(N >= 0 && J >= 1 && H >= 2 && W >= 2 && image_w >= 2 && image_h >= 2 && sigma >= 1,
+              "gaussian_targets_udp: bad sizes");
+  if (N == 0) return FPD_OK;
+  gaussian_target_udp_kernel<<<N * J, 256, 0, stream>>>(joints, joints_vis, joints_weight, target, target_weight, J, H,
+                                                        W, (image_w - 1.0) / (W - 1), (image_h - 1.0) / (H - 1),
+                                                        sigma * 3, (double)sigma);
   FPD_LAUNCH_CHECK();
   return FPD_OK;
 }

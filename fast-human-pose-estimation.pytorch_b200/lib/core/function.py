@@ -27,7 +27,7 @@ import numpy as np
 import torch
 
 from .evaluate import accuracy, pck_from_counts, pck_from_preds
-from .inference import blur_kernel, get_final_preds, inverse_affines, preds_from_argmax, use_dark
+from .inference import blur_kernel, get_final_preds, inverse_affines, preds_from_argmax, use_dark, use_udp
 
 logger = logging.getLogger(__name__)
 
@@ -424,6 +424,7 @@ class _GraphValidation:
         self.topk = _criterion_topk(criterion)
         self.post_process = "dark" if use_dark(config) else bool(config.TEST.POST_PROCESS)
         self.blur_kernel = blur_kernel(config)
+        self.udp = use_udp(config)
         self.preds = torch.empty((num_samples, J, 3), dtype=torch.float32, pin_memory=True)
         self.loss = torch.empty(num_batches, dtype=torch.float32, pin_memory=True)
         self.counts = torch.empty((num_batches, J, 2), dtype=torch.int32, pin_memory=True)
@@ -433,9 +434,9 @@ class _GraphValidation:
 
     def run(self, i, input, target, target_weight, c, s, idx):
         B, _, h, w = target.shape
-        r = self.runner(input, inv=inverse_affines(c, s, [w, h]), target=target, target_weight=target_weight,
-                        use_target_weight=self.use_tw, post_process=self.post_process, topk=self.topk,
-                        blur_kernel=self.blur_kernel)
+        r = self.runner(input, inv=inverse_affines(c, s, [w, h], udp=self.udp), target=target,
+                        target_weight=target_weight, use_target_weight=self.use_tw, post_process=self.post_process,
+                        topk=self.topk, blur_kernel=self.blur_kernel)
         self.preds[idx:idx + B].copy_(r["preds"], non_blocking=True)
         self.loss[i:i + 1].copy_(r["loss3"][:1], non_blocking=True)
         self.counts[i].copy_(r["pck"], non_blocking=True)

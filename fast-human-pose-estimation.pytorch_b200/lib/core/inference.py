@@ -54,10 +54,26 @@ def _inverse_affine(center, scale, output_size):
     return np.linalg.solve(a, src.astype(np.float64)).T          # maps heat-map (dst) coordinates to image (src)
 
 
-def inverse_affines(center, scale, output_size):
+def _udp_inverse_affines(center, scale, output_size):
+    """UDP's heat-map -> image matrices (Huang et al., CVPR 2020), the inverse of augment.udp_crop_matrix at rot = 0
+    composed with the heat-map stride: x = x_hm * s * 200 / (w - 1) + c - s * 200 / 2 per axis, in float64."""
+    c = np.asarray(center, np.float64).reshape(-1, 2)
+    box = np.asarray(scale, np.float64).reshape(-1, 2) * 200.0
+    t = np.zeros((c.shape[0], 6))
+    t[:, 0] = box[:, 0] / (output_size[0] - 1.0)
+    t[:, 4] = box[:, 1] / (output_size[1] - 1.0)
+    t[:, 2] = c[:, 0] - box[:, 0] * 0.5
+    t[:, 5] = c[:, 1] - box[:, 1] * 0.5
+    return t
+
+
+def inverse_affines(center, scale, output_size, udp=False):
     """_inverse_affine for a whole batch: center, scale [B,2] -> float64 [B,6], row b the row-major 2x3 matrix of sample
     b, equal bit for bit to _inverse_affine(center[b], scale[b], output_size) (the same float32 point arithmetic, the
-    same LAPACK solve per sample). This is the `inv` that ops.final_preds takes."""
+    same LAPACK solve per sample). This is the `inv` that ops.final_preds takes. udp=True gives UDP's matrices instead,
+    for maps of crops made by augment.udp_crop_matrix (config.TEST.UDP)."""
+    if udp:
+        return _udp_inverse_affines(center, scale, output_size)
     c = np.asarray(center, np.float32).reshape(-1, 2)
     src_w = np.asarray(scale, np.float32).reshape(-1, 2)[:, 0] * np.float32(200.0)
     B = c.shape[0]
@@ -79,18 +95,28 @@ def inverse_affines(center, scale, output_size):
     return np.ascontiguousarray(t.transpose(0, 2, 1).reshape(B, 6))
 
 
-def transform_preds(coords, center, scale, output_size):
-    """lib/utils/transforms.py:49-54 for the whole [J,2] array at once (rot = 0 is the only call the hot path makes)."""
+def _apply_affine(coords, t):
+    """coords [J,2] mapped by the 2x3 matrix t, in float64."""
     coords = np.asarray(coords, dtype=np.float64)
-    t = _inverse_affine(center, scale, output_size)
     out = np.zeros(coords.shape)
     out[:, 0:2] = coords[:, 0:2] @ t[:, :2].T + t[:, 2]
     return out
 
 
+def transform_preds(coords, center, scale, output_size):
+    """lib/utils/transforms.py:49-54 for the whole [J,2] array at once (rot = 0 is the only call the hot path makes)."""
+    return _apply_affine(coords, _inverse_affine(center, scale, output_size))
+
+
 def use_dark(config):
     """config.TEST.DARK: DARK's decode (ops.final_preds_dark) replaces the quarter-pixel nudge where POST_PROCESS is on."""
     return bool(config.TEST.POST_PROCESS) and bool(getattr(config.TEST, "DARK", False))
+
+
+def use_udp(config):
+    """config.TEST.UDP: map heat-map coordinates to the image with UDP's matrices (inverse_affines(..., udp=True)), for
+    models trained and validated on RawJointsDataset(udp=True) crops. Either decode runs on them unchanged."""
+    return bool(getattr(config.TEST, "UDP", False))
 
 
 def blur_kernel(config):
@@ -100,8 +126,8 @@ def blur_kernel(config):
 
 def get_final_preds(config, batch_heatmaps, center, scale):
     """inference.py:49-79: arg-max, optional quarter-pixel nudge toward the higher neighbour (or, with
-    config.TEST.DARK, DARK's Taylor step), map back to image coordinates. batch_heatmaps: CUDA tensor or numpy
-    [B,J,h,w]."""
+    config.TEST.DARK, DARK's Taylor step), map back to image coordinates (with config.TEST.UDP, by UDP's matrices).
+    batch_heatmaps: CUDA tensor or numpy [B,J,h,w]."""
     if isinstance(batch_heatmaps, np.ndarray):
         batch_heatmaps = torch.from_numpy(np.ascontiguousarray(batch_heatmaps)).cuda()
     hm = batch_heatmaps.contiguous().float()
@@ -111,7 +137,7 @@ def get_final_preds(config, batch_heatmaps, center, scale):
         from fpd_b200 import ops
         nhwc = ops.nchw_to_nhwc(hm)
         _, idx, maxvals = ops.flip_merge_argmax(nhwc, want_avg=False)
-        inv = torch.from_numpy(inverse_affines(center, scale, [W, H])).to(hm.device)
+        inv = torch.from_numpy(inverse_affines(center, scale, [W, H], udp=use_udp(config))).to(hm.device)
         preds = ops.final_preds_dark(nhwc, idx, maxvals, inv, blur_kernel(config)).cpu().numpy()
         return preds[..., :2].copy(), preds[..., 2:].copy()
     idx, maxvals = _device_argmax(hm)
@@ -131,6 +157,11 @@ def get_final_preds(config, batch_heatmaps, center, scale):
         coords[..., 0] += dx.cpu().numpy() * .25
         coords[..., 1] += dy.cpu().numpy() * .25
     preds = coords.copy()
+    if use_udp(config):
+        inv = inverse_affines(center, scale, [W, H], udp=True).reshape(B, 2, 3)
+        for i in range(B):
+            preds[i] = _apply_affine(coords[i], inv[i])
+        return preds, maxvals_np
     for i in range(B):
         preds[i] = transform_preds(coords[i], center[i], scale[i], [W, H])
     return preds, maxvals_np

@@ -969,9 +969,8 @@ def gaussian_targets(joints, joints_vis, heatmap_size, image_size, sigma=2, join
     return target, tw
 
 
-def gaussian_targets_unbiased(joints, joints_vis, heatmap_size, image_size, sigma=2, joints_weight=None):
-    """gaussian_targets with DARK's unbiased encoding: the Gaussian on the sub-pixel joint joint * heatmap_size /
-    image_size rather than on the rounded one, over the whole map. Same arguments (no table) and results."""
+def _sub_pixel_targets(name, joints, joints_vis, heatmap_size, image_size, sigma, joints_weight):
+    """Calls fpd_<name>, a target entry point with gaussian_targets' arguments less the table."""
     _chk(joints, "joints")
     _chk(joints_vis, "joints_vis")
     n, J = joints.shape[0], joints.shape[1]
@@ -980,10 +979,24 @@ def gaussian_targets_unbiased(joints, joints_vis, heatmap_size, image_size, sigm
     target = torch.empty((n, J, H, W), dtype=torch.float32, device=dev)
     tw = torch.empty((n, J, 1), dtype=torch.float32, device=dev)
     jw = None if joints_weight is None else joints_weight.to(dev).float().contiguous().reshape(-1)
-    N.check(N.lib().fpd_gaussian_targets_unbiased(_p(joints), _p(joints_vis), _p(jw), _p(target), _p(tw), n, J, H, W,
-                                                  int(image_size[0]), int(image_size[1]), int(sigma), _stream()),
-            "gaussian_targets_unbiased")
+    N.check(getattr(N.lib(), "fpd_" + name)(_p(joints), _p(joints_vis), _p(jw), _p(target), _p(tw), n, J, H, W,
+                                            int(image_size[0]), int(image_size[1]), int(sigma), _stream()), name)
     return target, tw
+
+
+def gaussian_targets_unbiased(joints, joints_vis, heatmap_size, image_size, sigma=2, joints_weight=None):
+    """gaussian_targets with DARK's unbiased encoding: the Gaussian on the sub-pixel joint joint * heatmap_size /
+    image_size rather than on the rounded one, over the whole map. Same arguments (no table) and results."""
+    return _sub_pixel_targets("gaussian_targets_unbiased", joints, joints_vis, heatmap_size, image_size, sigma,
+                              joints_weight)
+
+
+def gaussian_targets_udp(joints, joints_vis, heatmap_size, image_size, sigma=2, joints_weight=None):
+    """gaussian_targets with UDP's encoding (Huang et al., CVPR 2020), for joints cropped by augment.udp_crop_matrix:
+    stride (image_size - 1) / (heatmap_size - 1), the Gaussian on the unrounded centre joint / stride, within the
+    default 3 sigma window around the rounded one. Same arguments (no table) and results."""
+    return _sub_pixel_targets("gaussian_targets_udp", joints, joints_vis, heatmap_size, image_size, sigma,
+                              joints_weight)
 
 
 CROP_DESC_LEN = 7   # desc columns: byte offset, region x, y, w, h, image w, h (include/fpd_b200.h)

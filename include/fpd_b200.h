@@ -423,6 +423,15 @@ int fpd_gaussian_targets(const float* joints, const float* joints_vis, const flo
 int fpd_gaussian_targets_unbiased(const float* joints, const float* joints_vis, const float* joints_weight, float* target,
                                   float* target_weight, int N, int J, int H, int W, int image_w, int image_h, int sigma,
                                   fpd_stream_t stream);
+/* UDP targets (unbiased data processing, Huang et al., CVPR 2020), same arguments as fpd_gaussian_targets_unbiased.
+ * Sizes are pixel spacings: stride = ((image_w - 1) / (W - 1), (image_h - 1) / (H - 1)) and the centre
+ * mu = joint / stride is not rounded. Inside fpd_gaussian_targets' window, the 3 sigma square around int(mu + 0.5), the
+ * map holds exp(-|p - mu|^2 / (2 sigma^2)) evaluated in double; it is zero elsewhere. A joint whose window lies outside
+ * the map gets weight 0; joints_vis and joints_weight act as in fpd_gaussian_targets. H, W, image_w, image_h >= 2.
+ * Deterministic: no atomics. */
+int fpd_gaussian_targets_udp(const float* joints, const float* joints_vis, const float* joints_weight, float* target,
+                             float* target_weight, int N, int J, int H, int W, int image_w, int image_h, int sigma,
+                             fpd_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------
  * Input crop. Replaces the per-sample cv2.warpAffine(INTER_LINEAR) + ToTensor + Normalize of
