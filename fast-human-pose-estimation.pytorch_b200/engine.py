@@ -774,6 +774,20 @@ class Engine:
             self._branch_streams[key] = st
         return st
 
+    def check_input_size(self, H, W):
+        """Raises RuntimeError for an input of H x W the hourglass cannot run, before anything is launched: each of its
+        2x2 max-pools (the stem's and the four of every hourglass) needs an even height and width, or its up-sampled
+        output no longer matches the skip branch (the reference fails at that add). A 384x288 input reaches the
+        innermost level at 12x9."""
+        c = self.convs["conv1"]
+        h, w = (H + 2 * c.pad - c.k) // c.stride + 1, (W + 2 * c.pad - c.k) // c.stride + 1
+        for where in ("the stem's max-pool", "hourglass level 4", "hourglass level 3", "hourglass level 2",
+                      "hourglass level 1"):
+            if h % 2 or w % 2:
+                raise RuntimeError("hourglass: a %dx%d input reaches %s at %dx%d; its 2x2 max-pool needs an even height "
+                                   "and width" % (H, W, where, h, w))
+            h, w = h // 2, w // 2
+
     def hourglass_net(self, ctx, img_nchw):
         """HourglassNet.forward, reference hourglass.py:170-192. Returns the per-stack heat-map Vars (NHWC)."""
         net = self.net
@@ -806,6 +820,7 @@ class Engine:
     def prepare_stem(self, img_nchw, shared_stem):
         """Fills shared_stem with the NHWC image and (when the stem conv runs as im2col + tensor-core GEMM) its columns,
         on the current stream, so that several networks consuming this batch can share them."""
+        self.check_input_size(*img_nchw.shape[2:])
         if not (img_nchw.is_contiguous() and img_nchw.dtype == torch.float32):
             return
         c = self.convs.get("conv1")
@@ -826,6 +841,7 @@ class Engine:
         student + frozen teacher). The first forward stores the NHWC image and the stem's im2col columns in it, later
         ones reuse them (the caller orders the streams: the producer's forward must have been enqueued first and the
         consumer's stream must wait on it)."""
+        self.check_input_size(*img_nchw.shape[2:])
         ctx = _Ctx()
         ctx.shared_stem = shared_stem
         ctx.training = training

@@ -18,6 +18,9 @@ class HRNetEngine(Engine):
         super().__init__(net)
         self.force_apply_sum = True     # bias-free convolutions: dY's 3xFP16 operand scale comes from the BN-backward pass
 
+    def check_input_size(self, H, W):
+        """Every size runs: the strided convolutions round odd sizes up, like the reference's."""
+
     # ------------------------------------------------------------------ extra building blocks
     def bn_add_act(self, ctx, x, bn_name, residual, relu=True):
         aff = self._bn_affine(ctx, x, bn_name)

@@ -161,6 +161,7 @@ class FlipTestInference:
         maxval [B,J], avg_nhwc [B,h,w,J] merged heat-maps, nms_keep / nms_num; with decode=True also preds [B,J,3]
         (get_final_preds: x, y, maxval), loss3 [3] (loss3[0] = the criterion's value) and pck int32 [J,2] (per joint:
         valid, hit; lib.core.evaluate.pck_from_counts gives accuracy()'s acc / avg_acc / cnt)."""
+        self.net.engine().check_input_size(*x.shape[2:])     # before any copy, launch or capture
         self.nms_thresh = float(nms_thresh)
         if not self.use_graph:
             xd = x.cuda(non_blocking=True).float().contiguous()

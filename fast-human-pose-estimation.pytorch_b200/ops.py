@@ -390,9 +390,18 @@ def maxpool2x2_f16(x, out=None):
     return y
 
 
+def _chk_low(up1, low, name):
+    """up1 + upsample2x(low) needs low of (B, H / 2, W / 2, C): the kernel reads low's shape from up1's."""
+    B, H, W, C = up1.shape
+    if tuple(low.shape) != (B, H // 2, W // 2, C):
+        raise ValueError("%s: low must be %s for up1 of %s, got %s" % (
+            name, (B, H // 2, W // 2, C), tuple(up1.shape), tuple(low.shape)))
+
+
 def upsample2x_add_f16(up1, low, out=None):
     _chk_f16(up1, "up1")
     _chk_f16(low, "low")
+    _chk_low(up1, low, "upsample2x_add_f16")
     B, H, W, C = up1.shape
     y = out if out is not None else torch.empty_like(up1)
     N.check(N.lib().fpd_upsample2x_add_f16(_p(up1), _p(low), _p(y), B, H, W, C, _stream()), "upsample2x_add_f16")
@@ -645,6 +654,7 @@ def maxpool2x2_bwd(x, dy, accumulate_into=None):
 
 
 def upsample2x_add(up1, low, out=None):
+    _chk_low(up1, low, "upsample2x_add")
     B, H, W, C = up1.shape
     y = out if out is not None else torch.empty_like(up1)
     N.check(N.lib().fpd_upsample2x_add(_p(up1), _p(low), _p(y), B, H, W, C, _stream()), "upsample2x_add")
