@@ -533,3 +533,462 @@ int fpd_joints_ohkm(const float* out_nchw, const float* target_nchw, const float
 }
 
 }  // extern "C"
+
+// ---------------------------------------------------------------------------------------------------------------
+// Channel-wise distillation (Shu et al., ICCV 2021) per joint heat-map, JointsKLDLoss: each (b, j) map is a
+// distribution over its P = h*w pixels at temperature T,
+//   p = softmax(r / T) (reference: target or teacher),  q = softmax(o / T) (student),  KL = sum_p p (log p - log q)
+//   L = T^2 / (B*J) * sum_{b,j} w[b,j] KL[b,j]          dL/do = T * w * (q - p) / (B*J)
+// With m = max r, S = sum exp((r - m)/T) and C = sum exp((r - m)/T) (r - o) (and m', S' for o):
+//   KL = C / (T S) + (m' - m) / T + log(S' / S)
+// Three passes, like the hard keypoint mining above: (1) per (sample, 64-pixel chunk) block, each map's chunk maximum,
+// then the chunk's exp-sums and cross sums relative to it (fp32 within a thread, lanes added in fp64); (2) one block
+// per sample merges the chunks in fp64 (rescaling by exp((m_c - m)/T)), forms KL (or the sums of squares of an MSE /
+// OHKM term, with the same selection), the sample's share of each term and the gradient constants; (3) one pass writes
+// every gradient element. The reference's statistics are computed once and shared by all stacks. Student and reference
+// probabilities come out of the same arithmetic, so a student equal to its reference gives exactly zero loss and
+// gradient. No floating-point atomics: deterministic and graph-capturable.
+//
+// The module form (NCHW student) runs the same three kernels with S = 1 and the reference in the pose slot, chunk by
+// chunk; for h*w % 64 == 0 it therefore gives the fused form's bits term by term.
+//
+// Workspace: part double [B][nch][S+1][2][J][3] (slot S: the reference; {max, exp-sum, cross sum} or {-, sum of
+// squares, -}) | contrib double [B][S][2] | coef float4 [B][S+1][2][J] ({coefficient, max, 1/exp-sum, -}).
+namespace fpd {
+namespace {
+
+enum { kKindSq = 0, kKindKl = 1 };
+
+struct KlTerms {
+  int kind[2];      // pose, kd: kKindSq (MSE / OHKM) or kKindKl
+  float t[2];       // T of a KL term
+  float inv_t[2];   // its 1/T, the scale every exponent uses
+};
+
+// exp((x - m) / T): the one expression both the student's and the reference's statistics and probabilities use
+__device__ __forceinline__ float kl_exp(float x, float m, float inv_t) {
+  return expf(__fmul_rn(__fsub_rn(x, m), inv_t));
+}
+
+// (1) one block per (sample, 64-pixel chunk); thread (pl, j) owns joint j and pixels pl, pl + L, ... of the chunk.
+// NCHW_OUT: the student is NCHW (module form; the chunk may be partial), else NHWC with h*w % 64 == 0.
+template <bool NCHW_OUT>
+__global__ void __launch_bounds__(kThreads, 1)
+kl_stats_kernel(StackPtrs sp, int S, const float* __restrict__ target, const float* __restrict__ teacher, int J, int hw,
+                KlTerms tm, double* __restrict__ part) {
+  extern __shared__ float sm[];
+  float* tgt = sm;                          // [J][kPix+1]
+  float* red = sm + J * (kPix + 1);         // [max(S+2, 4)][L*J] lane partials
+  float* cmax = red + (S + 2 > 4 ? S + 2 : 4) * kThreads;   // [S+2][J] chunk maxima: stacks, target, teacher
+  const int nch = (hw + kPix - 1) / kPix;
+  const int b = blockIdx.x / nch;
+  const int p0 = (blockIdx.x % nch) * kPix;
+  const int np = min(kPix, hw - p0);
+  for (int i = threadIdx.x; i < J * kPix; i += kThreads) {
+    const int j = i / kPix, px = i % kPix;
+    if (px < np) tgt[j * (kPix + 1) + px] = __ldg(target + ((int64_t)b * J + j) * hw + p0 + px);
+  }
+  __syncthreads();
+  const int L = min(kPix, kThreads / J);
+  const int active = L * J;
+  const int j = threadIdx.x % J, pl = threadIdx.x / J;
+  const bool kl_p = tm.kind[0] == kKindKl, kl_k = tm.kind[1] == kKindKl;
+  const bool any_kl = kl_p || kl_k;
+  auto out_at = [&](int s, int px) -> float {
+    return NCHW_OUT ? __ldg(sp.out[s] + ((int64_t)b * J + j) * hw + p0 + px)
+                    : __ldg(sp.out[s] + ((int64_t)b * hw + p0 + px) * J + j);
+  };
+  auto teacher_at = [&](int px) -> float { return __ldg(teacher + ((int64_t)b * hw + p0 + px) * J + j); };
+  // chunk maxima (fmaxf passes a NaN over; the exp-sums below carry it into the loss)
+  if (any_kl) {
+    if (threadIdx.x < active) {
+      float mo[kMaxStacks], mg = -INFINITY, mt = -INFINITY;
+#pragma unroll
+      for (int s = 0; s < kMaxStacks; ++s) mo[s] = -INFINITY;
+      for (int px = pl; px < np; px += L) {
+        if (kl_p) mg = fmaxf(mg, tgt[j * (kPix + 1) + px]);
+        if (kl_k) mt = fmaxf(mt, teacher_at(px));
+#pragma unroll
+        for (int s = 0; s < kMaxStacks; ++s)
+          if (s < S) mo[s] = fmaxf(mo[s], out_at(s, px));
+      }
+#pragma unroll
+      for (int s = 0; s < kMaxStacks; ++s)
+        if (s < S) red[s * active + threadIdx.x] = mo[s];
+      red[S * active + threadIdx.x] = mg;
+      red[(S + 1) * active + threadIdx.x] = mt;
+    }
+    __syncthreads();
+    for (int q = threadIdx.x; q < (S + 2) * J; q += kThreads) {
+      const int slot = q / J, jj = q % J;
+      float m = -INFINITY;
+      for (int l = 0; l < L; ++l) m = fmaxf(m, red[slot * active + l * J + jj]);
+      cmax[q] = m;
+    }
+    __syncthreads();
+  }
+  // exp-sums, cross sums and sums of squares; per stack: {A_pose, C_pose, A_kd, C_kd}
+  float ap[kMaxStacks], cp[kMaxStacks], ak[kMaxStacks], ck[kMaxStacks], sg = 0.f, st = 0.f;
+#pragma unroll
+  for (int s = 0; s < kMaxStacks; ++s) ap[s] = cp[s] = ak[s] = ck[s] = 0.f;
+  if (threadIdx.x < active) {
+    const float mg = any_kl ? cmax[S * J + j] : 0.f, mt = any_kl ? cmax[(S + 1) * J + j] : 0.f;
+    for (int px = pl; px < np; px += L) {
+      const float g = tgt[j * (kPix + 1) + px];
+      const float t = teacher ? teacher_at(px) : 0.f;
+      const float eg = kl_p ? kl_exp(g, mg, tm.inv_t[0]) : 0.f;
+      const float et = kl_k ? kl_exp(t, mt, tm.inv_t[1]) : 0.f;
+      sg = __fadd_rn(sg, eg);
+      st = __fadd_rn(st, et);
+#pragma unroll
+      for (int s = 0; s < kMaxStacks; ++s) {
+        if (s < S) {
+          const float o = out_at(s, px);
+          const float mo = any_kl ? cmax[s * J + j] : 0.f;
+          if (kl_p) {
+            ap[s] = __fadd_rn(ap[s], kl_exp(o, mo, tm.inv_t[0]));
+            cp[s] = fmaf(eg, __fsub_rn(g, o), cp[s]);
+          } else {
+            const float d = o - g;
+            ap[s] = fmaf(d, d, ap[s]);
+          }
+          if (teacher) {
+            if (kl_k) {
+              ak[s] = __fadd_rn(ak[s], kl_exp(o, mo, tm.inv_t[1]));
+              ck[s] = fmaf(et, __fsub_rn(t, o), ck[s]);
+            } else {
+              const float d = o - t;
+              ak[s] = fmaf(d, d, ak[s]);
+            }
+          }
+        }
+      }
+    }
+  }
+  // lanes added in fp64 in lane order, one stack at a time (the shared buffer holds four slots)
+  const size_t J3 = (size_t)J * 3;
+  double* dst = part + (size_t)blockIdx.x * (S + 1) * 2 * J3;     // [S+1][2][J][3]
+  for (int s = 0; s <= S; ++s) {
+    __syncthreads();
+    if (threadIdx.x < active) {
+      float v[4] = {sg, 0.f, st, 0.f};       // slot S: the references
+#pragma unroll
+      for (int ss = 0; ss < kMaxStacks; ++ss)
+        if (ss == s && s < S) { v[0] = ap[ss]; v[1] = cp[ss]; v[2] = ak[ss]; v[3] = ck[ss]; }
+#pragma unroll
+      for (int k = 0; k < 4; ++k) red[k * active + threadIdx.x] = v[k];
+    }
+    __syncthreads();
+    for (int q = threadIdx.x; q < 2 * J; q += kThreads) {
+      const int term = q / J, jj = q % J;
+      double a = 0.0, c = 0.0;
+      for (int l = 0; l < L; ++l) {
+        a += (double)red[(2 * term) * active + l * J + jj];
+        c += (double)red[(2 * term + 1) * active + l * J + jj];
+      }
+      const int mslot = s < S ? s : S + term;       // the student's or this term's reference's maximum
+      double* r = dst + ((size_t)s * 2 + term) * J3 + (size_t)jj * 3;
+      r[0] = any_kl ? (double)cmax[mslot * J + jj] : 0.0;
+      r[1] = a;
+      r[2] = c;
+    }
+  }
+}
+
+// (2) one block per sample: merge the chunks, per-(s, term, j) losses, the sample's share of each term (losses as
+// ohkm_final_kernel sums them) and the gradient constants. For a KL term l = T^2 w KL and every joint counts (1/J).
+__global__ void __launch_bounds__(kThreads)
+kl_select_kernel(const double* __restrict__ part, int nch, int S, int J, int hw, int B, const float* __restrict__ tw,
+                 int has_teacher, int pose_topk, int kd_topk, KlTerms tm, float alpha, float grad_scale,
+                 double* __restrict__ contrib, float4* __restrict__ coef) {
+  __shared__ double ld[kMaxStacks * 2][kMaxJ];
+  __shared__ float lf[kMaxStacks * 2][kMaxJ];
+  __shared__ double rm[2][kMaxJ], rs[2][kMaxJ];
+  const int b = blockIdx.x;
+  const size_t rec = (size_t)(S + 1) * 2 * J * 3;        // one chunk's record
+  const double* pb = part + (size_t)b * nch * rec;
+  float4* cb = coef + (size_t)b * (S + 1) * 2 * J;
+  // the references' maxima and exp-sums
+  for (int q = threadIdx.x; q < 2 * J; q += kThreads) {
+    const int term = q / J, j = q % J;
+    if (tm.kind[term] != kKindKl || (term == 1 && !has_teacher)) continue;
+    const double it = (double)tm.inv_t[term];
+    const size_t off = ((size_t)S * 2 + term) * J * 3 + (size_t)j * 3;
+    double m = -INFINITY;
+    for (int c = 0; c < nch; ++c) m = fmax(m, pb[c * rec + off]);
+    double s = 0.0;
+    for (int c = 0; c < nch; ++c) s += pb[c * rec + off + 1] * exp((pb[c * rec + off] - m) * it);
+    rm[term][j] = m;
+    rs[term][j] = s;
+    cb[((size_t)S * 2 + term) * J + j] = make_float4(0.f, (float)m, (float)(1.0 / s), 0.f);
+  }
+  __syncthreads();
+  for (int q = threadIdx.x; q < S * 2 * J; q += kThreads) {
+    const int stt = q / J, j = q % J, term = stt & 1;
+    const double w = tw ? (double)__ldg(tw + (size_t)b * J + j) : 1.0;
+    const size_t off = (size_t)q * 3;
+    double l = 0.0;
+    if (term == 1 && !has_teacher) {
+      l = 0.0;
+    } else if (tm.kind[term] == kKindKl) {
+      const double it = (double)tm.inv_t[term];
+      const size_t roff = ((size_t)S * 2 + term) * J * 3 + (size_t)j * 3;
+      double m = -INFINITY;
+      for (int c = 0; c < nch; ++c) m = fmax(m, pb[c * rec + off]);
+      double a = 0.0, x = 0.0;
+      for (int c = 0; c < nch; ++c) {
+        a += pb[c * rec + off + 1] * exp((pb[c * rec + off] - m) * it);
+        x += pb[c * rec + off + 2] * exp((pb[c * rec + roff] - rm[term][j]) * it);
+      }
+      const double kl = x * it / rs[term][j] + (m - rm[term][j]) * it + log(a / rs[term][j]);
+      l = w * kl * (double)tm.t[term] * (double)tm.t[term];
+      cb[(size_t)q] = make_float4(0.f, (float)m, (float)(1.0 / a), 0.f);
+    } else {
+      double a = 0.0;
+      for (int c = 0; c < nch; ++c) a += pb[c * rec + off + 1];
+      l = 0.5 * (w * w) * a / (double)hw;
+    }
+    ld[stt][j] = l;
+    lf[stt][j] = (float)l;
+  }
+  __syncthreads();
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  for (int stt = wid; stt < S * 2; stt += kThreads / 32) {
+    const int s = stt >> 1, term = stt & 1;
+    float4* cf = cb + ((size_t)s * 2 + term) * J;
+    double* ct = contrib + ((size_t)b * S + s) * 2 + term;
+    if (term == 1 && !has_teacher) {
+      for (int j = lane; j < J; j += 32) cf[j].x = 0.f;
+      if (lane == 0) *ct = 0.0;
+      continue;
+    }
+    const bool kl = tm.kind[term] == kKindKl;
+    const int k = kl ? 0 : (term ? kd_topk : pose_topk);
+    const unsigned long long mask = k > 0 ? warp_topk_mask(lf[stt], J, k, lane)
+                                          : (J == 64 ? ~0ull : ((1ull << J) - 1ull));
+    const int cnt = k > 0 ? k : J;
+    const double factor = has_teacher ? (term ? (double)alpha : 1.0 - (double)alpha) : 1.0;
+    const double scale = kl ? (double)grad_scale * factor * (double)tm.t[term] / ((double)B * (double)J)
+                            : (double)grad_scale * factor / ((double)B * (double)cnt * (double)hw);
+    for (int j = lane; j < J; j += 32) {
+      const double w = tw ? (double)__ldg(tw + (size_t)b * J + j) : 1.0;
+      cf[j].x = ((mask >> j) & 1ull) ? (float)(kl ? scale * w : scale * w * w) : 0.f;
+    }
+    if (lane == 0) {
+      double sum = 0.0;
+      for (int j = 0; j < J; ++j)
+        if ((mask >> j) & 1ull) sum += ld[stt][j];
+      *ct = sum / (double)cnt;
+    }
+  }
+}
+
+// one term's gradient at one element: c (q - p) for KL, c (o - ref) otherwise; rounded on its own
+__device__ __forceinline__ float kl_term_grad(bool kl, float4 c, float o, float ref, float p, float inv_t) {
+  if (!kl) return __fmul_rn(c.x, o - ref);
+  const float q = __fmul_rn(kl_exp(o, c.y, inv_t), c.z);
+  return __fmul_rn(c.x, __fsub_rn(q, p));
+}
+
+// (3) fused form: grad_s = pose term + kd term for every element
+__global__ void __launch_bounds__(kThreads)
+kl_grad_nhwc_kernel(StackPtrs sp, int S, const float* __restrict__ target, const float* __restrict__ teacher,
+                    const float4* __restrict__ coef, int J, int hw, KlTerms tm) {
+  extern __shared__ float sm[];
+  float* tgt = sm;                                      // [J][kPix+1]
+  float4* cs = (float4*)(sm + ((J * (kPix + 1) + 3) & ~3));   // [S+1][2][J] of this sample
+  const int nch = hw / kPix;
+  const int b = blockIdx.x / nch;
+  const int p0 = (blockIdx.x % nch) * kPix;
+  for (int i = threadIdx.x; i < J * kPix; i += kThreads) {
+    const int j = i / kPix, px = i % kPix;
+    tgt[j * (kPix + 1) + px] = __ldg(target + ((int64_t)b * J + j) * hw + p0 + px);
+  }
+  const int n = (S + 1) * 2 * J;
+  for (int i = threadIdx.x; i < n; i += kThreads) cs[i] = __ldg(coef + (size_t)b * n + i);
+  __syncthreads();
+  const bool kl_p = tm.kind[0] == kKindKl, kl_k = tm.kind[1] == kKindKl;
+  const int64_t base = ((int64_t)b * hw + p0) * J;
+  for (int i = threadIdx.x; i < J * kPix; i += kThreads) {
+    const int px = i / J, j = i % J;
+    const float g = tgt[j * (kPix + 1) + px];
+    const float t = teacher ? __ldg(teacher + base + i) : 0.f;
+    float pg = 0.f, pt = 0.f;
+    if (kl_p) { const float4 r = cs[(S * 2) * J + j]; pg = __fmul_rn(kl_exp(g, r.y, tm.inv_t[0]), r.z); }
+    if (kl_k && teacher) { const float4 r = cs[(S * 2 + 1) * J + j]; pt = __fmul_rn(kl_exp(t, r.y, tm.inv_t[1]), r.z); }
+#pragma unroll
+    for (int s = 0; s < kMaxStacks; ++s) {
+      if (s < S) {
+        const float o = __ldg(sp.out[s] + base + i);
+        float gr = kl_term_grad(kl_p, cs[(2 * s) * J + j], o, g, pg, tm.inv_t[0]);
+        if (teacher) gr = __fadd_rn(gr, kl_term_grad(kl_k, cs[(2 * s + 1) * J + j], o, t, pt, tm.inv_t[1]));
+        sp.grad[s][base + i] = gr;
+      }
+    }
+  }
+}
+
+// (3) module form: one element per thread over the NCHW tensor
+__global__ void __launch_bounds__(kThreads)
+kl_grad_nchw_kernel(const float* __restrict__ out, const float* __restrict__ ref, const float4* __restrict__ coef,
+                    int J, int hw, float inv_t, int64_t n, float* __restrict__ grad) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t bj = i / hw;
+    const int b = (int)(bj / J), j = (int)(bj % J);
+    const float4* cb = coef + (size_t)b * 2 * 2 * J;      // [S+1 = 2][2][J]
+    const float4 rr = cb[2 * J + j];
+    const float r = __ldg(ref + i);
+    const float p = __fmul_rn(kl_exp(r, rr.y, inv_t), rr.z);
+    grad[i] = kl_term_grad(true, cb[j], __ldg(out + i), r, p, inv_t);
+  }
+}
+
+size_t kl_ws_bytes(int64_t B, int64_t nch, int64_t S, int64_t J) {
+  return (size_t)((B * nch * (S + 1) * 2 * J * 3 + B * S * 2) * (int64_t)sizeof(double) +
+                  B * (S + 1) * 2 * J * (int64_t)sizeof(float4));
+}
+
+struct KlWs {
+  double* part;
+  double* contrib;
+  float4* coef;
+};
+
+KlWs kl_ws_split(void* ws, int64_t B, int64_t nch, int64_t S, int64_t J) {
+  KlWs r;
+  r.part = (double*)ws;
+  r.contrib = r.part + B * nch * (S + 1) * 2 * J * 3;
+  r.coef = (float4*)(r.contrib + B * S * 2);     // an even number of doubles before it: 16-byte aligned
+  return r;
+}
+
+size_t kl_stats_smem(int S, int J) {
+  return ((size_t)J * (kPix + 1) + (size_t)(S + 2 > 4 ? S + 2 : 4) * kThreads + (size_t)(S + 2) * J) * sizeof(float);
+}
+
+// 0: not KL; else a finite T > 0
+bool kl_temperature_ok(float t) { return t == 0.f || (isfinite(t) && t > 0.f); }
+
+}  // namespace
+}  // namespace fpd
+
+extern "C" {
+
+size_t fpd_loss_kl_workspace_bytes(int S, int B, int J, int h, int w) {
+  const int64_t hw = (int64_t)h * w;
+  if (S < 1 || B < 1 || J < 1 || hw < 1) return 0;
+  return kl_ws_bytes(B, (hw + kPix - 1) / kPix, S, J) + 16;
+}
+
+size_t fpd_joints_kld_workspace_bytes(int B, int J, int hw) {
+  if (B < 1 || J < 1 || hw < 1) return 0;
+  return kl_ws_bytes(B, ((int64_t)hw + kPix - 1) / kPix, 1, J) + 16;
+}
+
+int fpd_loss_kl_fused(const float* const* outs, int S, const float* target_nchw, const float* teacher_nhwc,
+                      const float* tw, float alpha, float* const* grads, float grad_scale, float* losses, int B, int J,
+                      int h, int w, int pose_topk, int kd_topk, float pose_temperature, float kd_temperature,
+                      void* workspace, size_t ws_bytes, fpd_stream_t stream) {
+  FPD_REQUIRE(outs != nullptr, "fpd_loss_kl_fused: outs_host is NULL");
+  FPD_REQUIRE(S >= 1 && S <= kMaxStacks, "fpd_loss_kl: S=%d out of range [1,%d]", S, kMaxStacks);
+  FPD_REQUIRE(B >= 1, "fpd_loss_kl: B=%d (an empty batch has no loss)", B);
+  FPD_REQUIRE(h >= 1 && w >= 1, "fpd_loss_kl: empty heat-map %dx%d", h, w);
+  const int64_t hw64 = (int64_t)h * w;
+  FPD_REQUIRE(hw64 % kPix == 0 && hw64 <= (1 << 30), "fpd_loss_kl: h*w=%lld must be a multiple of %d",
+              (long long)hw64, kPix);
+  const int hw = (int)hw64;
+  FPD_REQUIRE(J >= 1 && J <= kMaxJ, "fpd_loss_kl: J=%d out of range [1,%d]", J, kMaxJ);
+  FPD_REQUIRE(kl_temperature_ok(pose_temperature), "fpd_loss_kl: pose_temperature=%g must be 0 (not KL) or finite > 0",
+              (double)pose_temperature);
+  FPD_REQUIRE(kl_temperature_ok(kd_temperature), "fpd_loss_kl: kd_temperature=%g must be 0 (not KL) or finite > 0",
+              (double)kd_temperature);
+  FPD_REQUIRE(pose_topk >= 0 && pose_topk <= J, "fpd_loss_kl: pose_topk=%d out of range [0,J=%d]", pose_topk, J);
+  FPD_REQUIRE(kd_topk >= 0 && kd_topk <= J, "fpd_loss_kl: kd_topk=%d out of range [0,J=%d]", kd_topk, J);
+  FPD_REQUIRE(!(pose_topk > 0 && pose_temperature > 0.f), "fpd_loss_kl: pose term has both topk=%d and temperature=%g",
+              pose_topk, (double)pose_temperature);
+  FPD_REQUIRE(!(kd_topk > 0 && kd_temperature > 0.f), "fpd_loss_kl: kd term has both topk=%d and temperature=%g",
+              kd_topk, (double)kd_temperature);
+  FPD_REQUIRE(teacher_nhwc != nullptr || (kd_topk == 0 && kd_temperature == 0.f),
+              "fpd_loss_kl: a kd topk or temperature without a teacher");
+  FPD_REQUIRE(target_nchw != nullptr && losses != nullptr, "fpd_loss_kl: target or losses is NULL");
+  FPD_REQUIRE(tw != nullptr, "fpd_loss_kl: target_weight is required (pass ones for use_target_weight=False)");
+  const int64_t nch = hw / kPix;
+  FPD_REQUIRE((int64_t)B * nch <= 0x7fffffff, "fpd_loss_kl: B * h*w/%d too large", kPix);
+  FPD_REQUIRE(workspace != nullptr && ws_bytes >= kl_ws_bytes(B, nch, S, J) + 16, "fpd_loss_kl: workspace too small");
+  StackPtrs sp{};
+  for (int s = 0; s < S; ++s) {
+    FPD_REQUIRE(outs[s] != nullptr, "fpd_loss_kl: outs[%d] is NULL", s);
+    sp.out[s] = outs[s];
+    sp.grad[s] = grads ? grads[s] : nullptr;
+    FPD_REQUIRE(grads == nullptr || grads[s] != nullptr, "fpd_loss_kl: grads[%d] is NULL", s);
+  }
+  KlTerms tm;
+  tm.kind[0] = pose_temperature > 0.f ? kKindKl : kKindSq;
+  tm.kind[1] = kd_temperature > 0.f ? kKindKl : kKindSq;
+  tm.t[0] = pose_temperature;
+  tm.t[1] = kd_temperature;
+  tm.inv_t[0] = pose_temperature > 0.f ? (float)(1.0 / (double)pose_temperature) : 0.f;
+  tm.inv_t[1] = kd_temperature > 0.f ? (float)(1.0 / (double)kd_temperature) : 0.f;
+  void* aligned = (void*)(((uintptr_t)workspace + 15) & ~(uintptr_t)15);
+  const KlWs ws = kl_ws_split(aligned, B, nch, S, J);
+  kl_stats_kernel<false><<<(int)(B * nch), kThreads, kl_stats_smem(S, J), stream>>>(sp, S, target_nchw, teacher_nhwc,
+                                                                                    J, hw, tm, ws.part);
+  FPD_LAUNCH_CHECK();
+  const int has_teacher = teacher_nhwc != nullptr;
+  kl_select_kernel<<<B, kThreads, 0, stream>>>(ws.part, (int)nch, S, J, hw, B, tw, has_teacher, pose_topk, kd_topk, tm,
+                                               alpha, grad_scale, ws.contrib, ws.coef);
+  FPD_LAUNCH_CHECK();
+  ohkm_final_kernel<<<1, 32, 0, stream>>>(ws.contrib, B, S, has_teacher, alpha, losses);
+  FPD_LAUNCH_CHECK();
+  if (grads) {
+    const size_t smem3 = ((size_t)((J * (kPix + 1) + 3) & ~3)) * sizeof(float) + (size_t)(S + 1) * 2 * J * sizeof(float4);
+    kl_grad_nhwc_kernel<<<(int)(B * nch), kThreads, smem3, stream>>>(sp, S, target_nchw, teacher_nhwc, ws.coef, J, hw,
+                                                                     tm);
+    FPD_LAUNCH_CHECK();
+  }
+  return FPD_OK;
+}
+
+int fpd_joints_kld(const float* out_nchw, const float* target_nchw, const float* tw, float temperature, float* loss3,
+                   float* grad_out, int B, int J, int hw, void* workspace, size_t ws_bytes, fpd_stream_t stream) {
+  FPD_REQUIRE(out_nchw != nullptr && target_nchw != nullptr && loss3 != nullptr,
+              "joints_kld: out, target or loss3 is NULL");
+  FPD_REQUIRE(B >= 1, "joints_kld: B=%d (an empty batch has no loss)", B);
+  FPD_REQUIRE(hw >= 1 && hw <= (1 << 30), "joints_kld: hw=%d out of range", hw);
+  FPD_REQUIRE(J >= 1 && J <= kMaxJ, "joints_kld: J=%d out of range [1,%d]", J, kMaxJ);
+  FPD_REQUIRE(isfinite(temperature) && temperature > 0.f, "joints_kld: temperature=%g must be finite and > 0",
+              (double)temperature);
+  const int64_t nch = ((int64_t)hw + kPix - 1) / kPix;
+  FPD_REQUIRE((int64_t)B * nch <= 0x7fffffff, "joints_kld: B * ceil(hw/%d) too large", kPix);
+  FPD_REQUIRE(workspace != nullptr && ws_bytes >= kl_ws_bytes(B, nch, 1, J) + 16, "joints_kld: workspace too small");
+  KlTerms tm;
+  tm.kind[0] = kKindKl;
+  tm.kind[1] = kKindSq;
+  tm.t[0] = temperature;
+  tm.t[1] = 0.f;
+  tm.inv_t[0] = (float)(1.0 / (double)temperature);
+  tm.inv_t[1] = 0.f;
+  void* aligned = (void*)(((uintptr_t)workspace + 15) & ~(uintptr_t)15);
+  const KlWs ws = kl_ws_split(aligned, B, nch, 1, J);
+  StackPtrs sp{};
+  sp.out[0] = out_nchw;
+  kl_stats_kernel<true><<<(int)(B * nch), kThreads, kl_stats_smem(1, J), stream>>>(sp, 1, target_nchw, nullptr, J, hw,
+                                                                                  tm, ws.part);
+  FPD_LAUNCH_CHECK();
+  kl_select_kernel<<<B, kThreads, 0, stream>>>(ws.part, (int)nch, 1, J, hw, B, tw, 0, 0, 0, tm, 0.f, 1.f, ws.contrib,
+                                               ws.coef);
+  FPD_LAUNCH_CHECK();
+  ohkm_final_kernel<<<1, 32, 0, stream>>>(ws.contrib, B, 1, 0, 0.f, loss3);
+  FPD_LAUNCH_CHECK();
+  if (grad_out) {
+    const int64_t n = (int64_t)B * J * hw;
+    int64_t nb = (n + kThreads - 1) / kThreads;
+    if (nb > 132 * 64) nb = 132 * 64;
+    kl_grad_nchw_kernel<<<(int)nb, kThreads, 0, stream>>>(out_nchw, target_nchw, ws.coef, J, hw, tm.inv_t[0], n,
+                                                          grad_out);
+    FPD_LAUNCH_CHECK();
+  }
+  return FPD_OK;
+}
+
+}  // extern "C"

@@ -8,7 +8,7 @@ one pixel, average, D2H of the merged heat-maps, numpy arg-max. Here, per batch:
                    forward (eval BN, cached 3xFP16 weights)      | second stream: forward of the mirrored image
                    fused flip_back + shift + average + arg-max -> idx[B,J], maxval[B,J] (+ merged heat-maps)
                    [optional box NMS of the detector boxes that produced the crops: lib/nms, csrc/nms.cu]
-                   [decode=True: merged map -> NCHW -> JointsMSELoss or JointsOHKMMSELoss (loss3), get_final_preds
+                   [decode=True: merged map -> NCHW -> JointsMSELoss, JointsOHKMMSELoss or JointsKLDLoss (loss3), get_final_preds
                     (preds; DARK's decode with post_process="dark"), accuracy() counts (pck), all on the device,
                     bit-identical to lib/core/function.py's eager route] }
 
@@ -26,6 +26,14 @@ def _post_process(post_process):
             raise ValueError("post_process must be a bool or 'dark', got %r" % (post_process,))
         return post_process
     return bool(post_process)
+
+
+def _temperature(topk, temperature):
+    """The decode stage's JointsKLDLoss temperature: 0 (another criterion) or finite and > 0, never with a topk."""
+    t = ops._check_temperature(temperature, "temperature", True)
+    if t and topk:
+        raise ValueError("the criterion is JointsOHKMMSELoss (topk) or JointsKLDLoss (temperature), not both")
+    return t
 
 
 class FlipTestInference:
@@ -90,7 +98,9 @@ class FlipTestInference:
             out_nchw = ops.nhwc_to_nchw(avg)
             B, J = idx.shape
             tw = extra["target_weight"].reshape(B, J) if extra["use_target_weight"] else None
-            if extra["topk"]:
+            if extra["temperature"]:
+                res["loss3"], _ = ops.joints_kld(out_nchw, extra["target"], tw, extra["temperature"], want_grad=False)
+            elif extra["topk"]:
                 res["loss3"], _ = ops.joints_ohkm_mse(out_nchw, extra["target"], tw, extra["topk"], want_grad=False)
             else:
                 res["loss3"], _ = ops.joints_mse(out_nchw, extra["target"], tw, want_grad=False)
@@ -102,7 +112,8 @@ class FlipTestInference:
         self._keep = (ctx, ctx_f, nhwc, out_nchw)      # every intermediate stays referenced: the graph pool never recycles them
         return res
 
-    def _extra(self, inv, target, target_weight, use_target_weight, post_process, topk, blur_kernel, static):
+    def _extra(self, inv, target, target_weight, use_target_weight, post_process, topk, blur_kernel, temperature,
+               static):
         """The decode stage's inputs on the device: fresh copies, or refills of the graph's static buffers."""
         if not self.decode:
             return None
@@ -117,7 +128,8 @@ class FlipTestInference:
             return {"inv": own(inv, torch.float64), "target": own(target, torch.float32),
                     "target_weight": own(target_weight, torch.float32),
                     "use_target_weight": bool(use_target_weight), "post_process": _post_process(post_process),
-                    "topk": int(topk), "blur_kernel": int(blur_kernel)}
+                    "topk": int(topk), "blur_kernel": int(blur_kernel),
+                    "temperature": _temperature(topk, temperature)}
         static["inv"].copy_(inv, non_blocking=True)
         static["target"].copy_(target, non_blocking=True)
         static["target_weight"].copy_(target_weight, non_blocking=True)
@@ -149,14 +161,14 @@ class FlipTestInference:
         self._staged_for = next_x
 
     def __call__(self, x, boxes_sorted=None, nms_thresh=0.6, next_x=None, inv=None, target=None, target_weight=None,
-                 use_target_weight=True, post_process=True, topk=0, blur_kernel=11):
+                 use_target_weight=True, post_process=True, topk=0, blur_kernel=11, temperature=0.0):
         """x: [B,3,H,W] fp32, CUDA or pinned host. boxes_sorted: optional device [n,5] detector boxes sorted by score.
         next_x: optional pinned host tensor = the NEXT batch (its H2D copy overlaps this batch; pass it as `x` next time).
         With decode=True: inv host float64 [B,6] heat-map -> image matrices (lib.core.inference.inverse_affines of the
         batch's centres / scales), target [B,J,h,w] and target_weight [B,J,1] (host or device), use_target_weight (the
         criterion's), post_process (config.TEST.POST_PROCESS; "dark" decodes with ops.final_preds_dark and a
-        blur_kernel-tap blur instead of the quarter-pixel nudge) and topk (the JointsOHKMMSELoss criterion's topk; 0 for
-        JointsMSELoss).
+        blur_kernel-tap blur instead of the quarter-pixel nudge), topk (the JointsOHKMMSELoss criterion's topk; 0 for
+        JointsMSELoss) and temperature (the JointsKLDLoss criterion's temperature; 0 for the other two).
         Returns a dict of DEVICE tensors (static across calls in graph mode): idx int32 [B,J] (flat arg-max, first maximum),
         maxval [B,J], avg_nhwc [B,h,w,J] merged heat-maps, nms_keep / nms_num; with decode=True also preds [B,J,3]
         (get_final_preds: x, y, maxval), loss3 [3] (loss3[0] = the criterion's value) and pck int32 [J,2] (per joint:
@@ -166,11 +178,11 @@ class FlipTestInference:
         if not self.use_graph:
             xd = x.cuda(non_blocking=True).float().contiguous()
             return self._body(xd, boxes_sorted, self._extra(inv, target, target_weight, use_target_weight, post_process,
-                                                            topk, blur_kernel, None))
+                                                            topk, blur_kernel, temperature, None))
         shape = (tuple(x.shape), None if boxes_sorted is None else tuple(boxes_sorted.shape), self.nms_thresh)
         if self.decode:
             shape += (tuple(target.shape), tuple(target_weight.shape), bool(use_target_weight),
-                      _post_process(post_process), int(topk), int(blur_kernel))
+                      _post_process(post_process), int(topk), int(blur_kernel), _temperature(topk, temperature))
         gen = self.net.engine().generation
         if self.graph is None or shape != self._shape or gen != self._gen:
             xd = x.cuda(non_blocking=True).float().contiguous()
@@ -178,7 +190,7 @@ class FlipTestInference:
             self.static_x.copy_(xd)
             self.static_boxes = None if boxes_sorted is None else boxes_sorted.clone()
             self.static_extra = self._extra(inv, target, target_weight, use_target_weight, post_process, topk, blur_kernel,
-                                            None)
+                                            temperature, None)
             side = torch.cuda.Stream()
             side.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(side):
@@ -196,7 +208,8 @@ class FlipTestInference:
         self._stage(x)
         if boxes_sorted is not None:
             self.static_boxes.copy_(boxes_sorted, non_blocking=True)
-        self._extra(inv, target, target_weight, use_target_weight, post_process, topk, blur_kernel, self.static_extra)
+        self._extra(inv, target, target_weight, use_target_weight, post_process, topk, blur_kernel, temperature,
+                    self.static_extra)
         self.graph.replay()
         self._prefetch(next_x)
         return self.result

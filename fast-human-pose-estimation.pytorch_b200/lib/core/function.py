@@ -7,7 +7,8 @@ What changes underneath:
     FPD loss+gradient kernel, the explicit backward tape -- and the gradients are handed to the caller's
     optimizer through .grad, so `optimizer.step()`, LR schedulers and checkpointing keep working. Any other
     model / criterion combination takes the generic autograd route, statement for statement like the reference.
-    The criteria may be JointsMSELoss or JointsOHKMMSELoss (online hard keypoint mining, any mix of the two under FPD).
+    The criteria may be JointsMSELoss, JointsOHKMMSELoss (online hard keypoint mining) or JointsKLDLoss (per-map
+    softmax KL distillation), any mix of the three under FPD with one use_target_weight.
   * per-iteration accuracy() and validate()'s flip test / decode run on the device; only [B,J] indices cross PCIe
     (the reference ships the full heat-maps to numpy every iteration: function.py:154-156, 218-240, 263).
   * train / fpd_train: on the fused route each batch of the epoch's batch shape is one CUDA graph replay (train_step.
@@ -15,7 +16,7 @@ What changes underneath:
     with the weight gradients on their own stream, PCK counts); the caller's optimizer then steps on the gradients. Losses
     and counts go to pinned host buffers asynchronously; the host waits only to log and at the end of the epoch. Other
     batch shapes (the short last batch) and config.DEBUG.DEBUG take the eager fused route, which gives the same bits.
-  * validate: for the fpd_b200 models with JointsMSELoss or JointsOHKMMSELoss, each batch is one CUDA graph replay (infer_step.
+  * validate: for the fpd_b200 models with JointsMSELoss, JointsOHKMMSELoss or JointsKLDLoss, each batch is one CUDA graph replay (infer_step.
     FlipTestInference with its decode stage: both forwards, flip merge, loss, keypoints, PCK counts); the results are
     copied to pinned host buffers asynchronously and the host waits only to log and at the end of the epoch.
 """
@@ -77,20 +78,25 @@ def _is_fpd_net(model):
 
 
 def _is_fpd_criterion(c):
-    from .loss import JointsMSELoss, JointsOHKMMSELoss
-    return isinstance(c, (JointsMSELoss, JointsOHKMMSELoss))
+    from .loss import JointsKLDLoss, JointsMSELoss, JointsOHKMMSELoss
+    return isinstance(c, (JointsMSELoss, JointsOHKMMSELoss, JointsKLDLoss))
 
 
-def _criterion_topk(c):
-    """The fused loss kernels' term selector: the criterion's topk for JointsOHKMMSELoss, 0 for JointsMSELoss."""
-    from .loss import JointsOHKMMSELoss
-    return c.topk if isinstance(c, JointsOHKMMSELoss) else 0
+def _criterion_term(c, term):
+    """The fused loss kernels' selector for one loss term (term "pose" or "kd"), as the keyword arguments of
+    ops.fpd_loss / FPDTrainStep that pick the criterion's kind: {term_topk: topk} for JointsOHKMMSELoss,
+    {term_temperature: temperature} for JointsKLDLoss, {term_topk: 0} for JointsMSELoss."""
+    from .loss import JointsKLDLoss, JointsOHKMMSELoss
+    if isinstance(c, JointsKLDLoss):
+        return {term + "_temperature": c.temperature}
+    return {term + "_topk": c.topk if isinstance(c, JointsOHKMMSELoss) else 0}
 
 
-def _fused_step(model, tmodel, input, target, target_weight, alpha, use_tw, graph=None, pose_topk=0, kd_topk=0):
+def _fused_step(model, tmodel, input, target, target_weight, alpha, use_tw, graph=None, **terms):
     """student fwd -> teacher fwd -> fused loss+grad -> backward tape; returns (losses[3] dev, last output NHWC).
-    graph: a _GraphTraining whose batch shape this batch has -- the same step is then one replay of its graph, and the
-    last output is None (the PCK counts come out of the graph instead)."""
+    terms: the criteria's _criterion_term selectors. graph: a _GraphTraining whose batch shape this batch has -- the
+    same step is then one replay of its graph, and the last output is None (the PCK counts come out of the graph
+    instead)."""
     if graph is not None:
         return graph.step(input, target, target_weight), None
     from fpd_b200 import ops
@@ -104,8 +110,7 @@ def _fused_step(model, tmodel, input, target, target_weight, alpha, use_tw, grap
         t_last = _unwrap(tmodel).forward_nhwc(x, training=False)[-1]
     B, _, _, J = outs[0].shape
     tw = target_weight.reshape(B, J) if use_tw else torch.ones(B, J, device=x.device)
-    losses, grads = ops.fpd_loss(outs, target.contiguous().float(), t_last, tw.contiguous().float(), alpha,
-                                 pose_topk=pose_topk, kd_topk=kd_topk)
+    losses, grads = ops.fpd_loss(outs, target.contiguous().float(), t_last, tw.contiguous().float(), alpha, **terms)
     pg = eng.backward(ctx, grads)
     params = [p for p in net.parameters() if p.requires_grad]      # frozen parameters keep whatever .grad they had
     glist = []
@@ -143,21 +148,22 @@ def _train_route(config, model, tmodel, criteria, target_shape):
 
 class _GraphTraining:
     """train()/fpd_train()'s per-batch work as replays of one FPDTrainStep(fused_adam=False, accuracy=True), which is
-    cached across calls keyed on the networks, the batch shapes, alpha and the topks. Losses and PCK counts go to pinned
-    host buffers with non-blocking copies; `flush` waits for them and applies the meter updates in batch order."""
+    cached across calls keyed on the networks, the batch shapes, alpha and the loss terms (topks and temperatures).
+    Losses and PCK counts go to pinned host buffers with non-blocking copies; `flush` waits for them and applies the
+    meter updates in batch order. terms: the criteria's _criterion_term selectors."""
 
-    def __init__(self, model, tmodel, alpha, use_tw, pose_topk, kd_topk, input, target, target_weight, num_batches):
+    def __init__(self, model, tmodel, alpha, use_tw, terms, input, target, target_weight, num_batches):
         from fpd_b200.train_step import FPDTrainStep
         net = _unwrap(model)
         tnet = _unwrap(tmodel) if tmodel is not None else None
         self.shapes = (tuple(input.shape), tuple(target.shape), tuple(target_weight.shape))
         alpha = float(alpha) if tnet is not None else 0.0
-        key = (id(net), id(tnet), self.shapes, alpha, pose_topk, kd_topk)
+        key = (id(net), id(tnet), self.shapes, alpha, tuple(sorted(terms.items())))
         step = _train_step_cache.get(key)
         if step is None:
             _train_step_cache.clear()          # one graph pool at a time
-            step = _train_step_cache[key] = FPDTrainStep(net, tnet, alpha=alpha, pose_topk=pose_topk, kd_topk=kd_topk,
-                                                         fused_adam=False, accuracy=True)
+            step = _train_step_cache[key] = FPDTrainStep(net, tnet, alpha=alpha, fused_adam=False, accuracy=True,
+                                                         **terms)
         self.train_step = step
         self.trainable = [(p, g) for p, g in zip(step.params, step.grad_views) if p.requires_grad]
         B, J = target.shape[0], target.shape[1]
@@ -247,6 +253,7 @@ def train(config, train_loader, model, criterion, optimizer, epoch, output_dir, 
     batch_time, data_time, losses, acc = AverageMeter(), AverageMeter(), AverageMeter(), AverageMeter()
     model.train()
     fused = _is_fpd_net(model) and _is_fpd_criterion(criterion)
+    terms = _criterion_term(criterion, "pose") if fused else None
     end = time.time()
     shape_checked = False
     graph = None
@@ -263,15 +270,15 @@ def train(config, train_loader, model, criterion, optimizer, epoch, output_dir, 
             fused = route != "generic"
             shape_checked = True
             if route == "graph":
-                graph = _GraphTraining(model, None, 0.0, criterion.use_target_weight, _criterion_topk(criterion), 0,
-                                       input, target, target_weight, len(train_loader))
+                graph = _GraphTraining(model, None, 0.0, criterion.use_target_weight, terms, input, target,
+                                       target_weight, len(train_loader))
         replay = graph if graph is not None and graph.accepts(input, target, target_weight) else None
         if graph is not None and replay is None:
             graph.flush(apply)          # meter updates stay in batch order
         if fused:
             optimizer.zero_grad()
             l3, out_nhwc = _fused_step(model, None, input, target, target_weight, 0.0, criterion.use_target_weight,
-                                       replay, pose_topk=_criterion_topk(criterion))
+                                       replay, **terms)
             optimizer.step()
             if replay is not None:
                 replay.record(i, l3, input.size(0))
@@ -323,6 +330,7 @@ def fpd_train(config, train_loader, model, tmodel, pose_criterion, kd_pose_crite
     fused = (_is_fpd_net(model) and _is_fpd_net(tmodel) and _is_fpd_criterion(pose_criterion)
              and _is_fpd_criterion(kd_pose_criterion)
              and pose_criterion.use_target_weight == kd_pose_criterion.use_target_weight)
+    terms = {**_criterion_term(pose_criterion, "pose"), **_criterion_term(kd_pose_criterion, "kd")} if fused else None
     end = time.time()
     shape_checked = False
     graph = None
@@ -343,17 +351,15 @@ def fpd_train(config, train_loader, model, tmodel, pose_criterion, kd_pose_crite
             fused = route != "generic"
             shape_checked = True
             if route == "graph":
-                graph = _GraphTraining(model, tmodel, alpha, pose_criterion.use_target_weight,
-                                       _criterion_topk(pose_criterion), _criterion_topk(kd_pose_criterion),
-                                       input, target, target_weight, len(train_loader))
+                graph = _GraphTraining(model, tmodel, alpha, pose_criterion.use_target_weight, terms, input, target,
+                                       target_weight, len(train_loader))
         replay = graph if graph is not None and graph.accepts(input, target, target_weight) else None
         if graph is not None and replay is None:
             graph.flush(apply)          # meter updates stay in batch order
         if fused:
             optimizer.zero_grad()
             l3, out_nhwc = _fused_step(model, tmodel, input, target, target_weight, alpha,
-                                       pose_criterion.use_target_weight, replay, pose_topk=_criterion_topk(pose_criterion),
-                                       kd_topk=_criterion_topk(kd_pose_criterion))
+                                       pose_criterion.use_target_weight, replay, **terms)
             optimizer.step()
             if replay is not None:
                 replay.record(i, l3, input.size(0))
@@ -421,7 +427,9 @@ class _GraphValidation:
         self.runner = FlipTestInference(net, val_dataset.flip_pairs, shift_heatmap=bool(config.TEST.SHIFT_HEATMAP),
                                         flip_test=bool(config.TEST.FLIP_TEST), decode=True)
         self.use_tw = criterion.use_target_weight
-        self.topk = _criterion_topk(criterion)
+        term = _criterion_term(criterion, "pose")
+        self.topk = term.get("pose_topk", 0)
+        self.temperature = term.get("pose_temperature", 0.0)
         self.post_process = "dark" if use_dark(config) else bool(config.TEST.POST_PROCESS)
         self.blur_kernel = blur_kernel(config)
         self.udp = use_udp(config)
@@ -436,7 +444,7 @@ class _GraphValidation:
         B, _, h, w = target.shape
         r = self.runner(input, inv=inverse_affines(c, s, [w, h], udp=self.udp), target=target,
                         target_weight=target_weight, use_target_weight=self.use_tw, post_process=self.post_process,
-                        topk=self.topk, blur_kernel=self.blur_kernel)
+                        topk=self.topk, temperature=self.temperature, blur_kernel=self.blur_kernel)
         self.preds[idx:idx + B].copy_(r["preds"], non_blocking=True)
         self.loss[i:i + 1].copy_(r["loss3"][:1], non_blocking=True)
         self.counts[i].copy_(r["pck"], non_blocking=True)

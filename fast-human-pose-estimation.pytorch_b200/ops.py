@@ -4,6 +4,8 @@ Every function takes contiguous fp32 CUDA tensors, enqueues on torch's current s
 (or fills) tensors. Activations are NHWC ([B,H,W,C]) unless a name says otherwise.
 """
 import ctypes
+import math
+import numbers
 import os
 
 import torch
@@ -768,10 +770,23 @@ def _check_topk(topk, J, lo, name):
     return int(topk)
 
 
+def _check_temperature(t, name, allow_zero):
+    """A JointsKLDLoss temperature: finite and > 0 (0 = "not KL" where allow_zero)."""
+    if isinstance(t, bool) or not isinstance(t, numbers.Real) or not (math.isfinite(t) and (t > 0 or (allow_zero and t == 0))):
+        raise ValueError("%s=%r must be a finite number > 0%s" % (name, t, " (or 0: not KL)" if allow_zero else ""))
+    return float(t)
+
+
 def fpd_loss(outs_nhwc, target_nchw, teacher_nhwc, target_weight, alpha, want_grads=True, grad_scale=1.0,
-             grads_out=None, losses_out=None, pose_topk=0, kd_topk=0):
+             grads_out=None, losses_out=None, pose_topk=0, kd_topk=0, pose_temperature=0, kd_temperature=0):
     """Fused FPD loss. outs_nhwc: list of [B,h,w,J]; returns (losses[3] device tensor, grads list or None).
-    pose_topk / kd_topk > 0 make that term JointsOHKMMSELoss(topk) instead of JointsMSELoss (fpd_loss_ohkm_fused)."""
+    pose_topk / kd_topk > 0 make that term JointsOHKMMSELoss(topk) instead of JointsMSELoss (fpd_loss_ohkm_fused);
+    pose_temperature / kd_temperature > 0 make it JointsKLDLoss(temperature) (fpd_loss_kl_fused, which takes any mix
+    of the three kinds). A term cannot have both a topk and a temperature."""
+    pose_temperature = _check_temperature(pose_temperature, "pose_temperature", True)
+    kd_temperature = _check_temperature(kd_temperature, "kd_temperature", True)
+    if (pose_topk and pose_temperature) or (kd_topk and kd_temperature):
+        raise ValueError("a loss term is JointsOHKMMSELoss (topk) or JointsKLDLoss (temperature), not both")
     S = len(outs_nhwc)
     B, h, w, J = outs_nhwc[0].shape
     dev = outs_nhwc[0].device
@@ -782,6 +797,17 @@ def fpd_loss(outs_nhwc, target_nchw, teacher_nhwc, target_weight, alpha, want_gr
         grads = grads_out if grads_out is not None else [torch.empty_like(o) for o in outs_nhwc]
     outs_arr = (ctypes.c_void_p * S)(*[o.data_ptr() for o in outs_nhwc])
     grads_arr = (ctypes.c_void_p * S)(*[g.data_ptr() for g in grads]) if grads is not None else None
+    if pose_temperature or kd_temperature:
+        pose_topk = _check_topk(pose_topk, J, 0, "pose_topk")
+        kd_topk = _check_topk(kd_topk, J, 0, "kd_topk")
+        for t in list(outs_nhwc) + [target_nchw, teacher_nhwc, tw]:
+            _chk(t, "fpd_loss argument")
+        ws = _ws.get(N.lib().fpd_loss_kl_workspace_bytes(S, B, J, h, w), dev)
+        N.check(N.lib().fpd_loss_kl_fused(outs_arr, S, _p(target_nchw), _p(teacher_nhwc), _p(tw), float(alpha),
+                                          grads_arr, float(grad_scale), _p(losses), B, J, h, w, pose_topk, kd_topk,
+                                          pose_temperature, kd_temperature, _p(ws), ws.numel(), _stream()),
+                "loss_kl_fused")
+        return losses, grads
     if pose_topk or kd_topk:
         pose_topk = _check_topk(pose_topk, J, 0, "pose_topk")
         kd_topk = _check_topk(kd_topk, J, 0, "kd_topk")
@@ -831,6 +857,29 @@ def joints_ohkm_mse(out_nchw, target_nchw, target_weight=None, topk=8, want_grad
     ws = _ws.get(N.lib().fpd_joints_ohkm_workspace_bytes(B, J), dev)
     N.check(N.lib().fpd_joints_ohkm(_p(out_nchw), _p(target_nchw), _p(tw), topk, _p(loss3), _p(grad), B, J, hw, _p(ws),
                                     ws.numel(), _stream()), "joints_ohkm")
+    return loss3, grad
+
+
+def joints_kld(out_nchw, ref_nchw, target_weight=None, temperature=1.0, want_grad=True):
+    """JointsKLDLoss on NCHW tensors: T^2/(B*J) * sum_{b,j} w[b,j] * KL(softmax(ref[b,j]/T) || softmax(out[b,j]/T)),
+    each map a distribution over its pixels; any h*w, J <= 64. Returns (loss3 device tensor, loss3[0] the value;
+    grad [B,J,h,w] or None)."""
+    temperature = _check_temperature(temperature, "temperature", False)
+    _chk(out_nchw, "out")
+    _chk(ref_nchw, "ref")
+    if out_nchw.dim() < 3 or out_nchw.shape[0] * out_nchw.shape[1] == 0 or ref_nchw.shape != out_nchw.shape:
+        raise ValueError("out / ref must be non-empty [B,J,...] tensors of one shape (got %s, %s)"
+                         % (tuple(out_nchw.shape), tuple(ref_nchw.shape)))
+    B, J = out_nchw.shape[:2]
+    hw = out_nchw.numel() // (B * J)
+    dev = out_nchw.device
+    loss3 = torch.empty(3, dtype=torch.float32, device=dev)
+    grad = torch.empty_like(out_nchw) if want_grad else None
+    tw = None if target_weight is None else target_weight.reshape(B, J).contiguous()
+    _chk(tw, "target_weight")
+    ws = _ws.get(N.lib().fpd_joints_kld_workspace_bytes(B, J, hw), dev)
+    N.check(N.lib().fpd_joints_kld(_p(out_nchw), _p(ref_nchw), _p(tw), temperature, _p(loss3), _p(grad), B, J, hw,
+                                   _p(ws), ws.numel(), _stream()), "joints_kld")
     return loss3, grad
 
 

@@ -11,8 +11,8 @@ eager ATen launches plus a DataParallel replicate/scatter/gather. Here the same 
 
 With fused_adam=False the step stops after the all-reduce: the parameters keep their own storage and the caller's
 optimizer (any torch.optim optimizer, its state dict, LR schedules) steps on the per-parameter views of the flat gradient
-buffer -- lib/core/function.py's train / fpd_train run this way. pose_topk / kd_topk select JointsOHKMMSELoss for a term;
-accuracy=True adds accuracy()'s PCK counts of the last stack to the graph.
+buffer -- lib/core/function.py's train / fpd_train run this way. pose_topk / kd_topk select JointsOHKMMSELoss for a term,
+pose_temperature / kd_temperature JointsKLDLoss; accuracy=True adds accuracy()'s PCK counts of the last stack to the graph.
 
 The teacher is forward-only (its gradients never influence the student update; the reference's teacher
 backward is wasted work). `plain=True` drops the teacher (function.train semantics,
@@ -72,8 +72,10 @@ def _check_topk(value, name):
 
 class FPDTrainStep:
     def __init__(self, student, teacher=None, alpha=0.5, lr=2.5e-4, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0,
-                 process_group=None, use_graph=True, pose_topk=0, kd_topk=0, fused_adam=True, accuracy=False):
+                 process_group=None, use_graph=True, pose_topk=0, kd_topk=0, fused_adam=True, accuracy=False,
+                 pose_temperature=0.0, kd_temperature=0.0):
         """pose_topk / kd_topk: > 0 makes that loss term JointsOHKMMSELoss(topk) instead of JointsMSELoss.
+        pose_temperature / kd_temperature: > 0 makes that term JointsKLDLoss(temperature) (not together with a topk).
         fused_adam=False (external-optimizer mode): step() stops once the gradients are in the flat gradient buffer
         (all-reduced, mean over ranks); the parameters keep their own storage and the caller's optimizer steps on
         `grad_views`. lr / betas / eps / weight_decay are then unused.
@@ -82,10 +84,17 @@ class FPDTrainStep:
         pose_topk, kd_topk = _check_topk(pose_topk, "pose_topk"), _check_topk(kd_topk, "kd_topk")
         if kd_topk and teacher is None:
             raise ValueError("kd_topk=%d needs a teacher" % kd_topk)
+        pose_temperature = ops._check_temperature(pose_temperature, "pose_temperature", True)
+        kd_temperature = ops._check_temperature(kd_temperature, "kd_temperature", True)
+        if kd_temperature and teacher is None:
+            raise ValueError("kd_temperature=%r needs a teacher" % kd_temperature)
+        if (pose_topk and pose_temperature) or (kd_topk and kd_temperature):
+            raise ValueError("a loss term is JointsOHKMMSELoss (topk) or JointsKLDLoss (temperature), not both")
         self.student, self.teacher = student, teacher
         self.alpha = float(alpha) if teacher is not None else 0.0
         self.lr, self.betas, self.eps, self.wd = lr, betas, eps, weight_decay
         self.pose_topk, self.kd_topk = pose_topk, kd_topk
+        self.pose_temperature, self.kd_temperature = pose_temperature, kd_temperature
         self.fused_adam = bool(fused_adam)
         self.want_accuracy = bool(accuracy)
         self.counts = None
@@ -192,7 +201,11 @@ class FPDTrainStep:
 
     def _loss(self, outs, target, t_last, tw):
         """The fused FPD loss and its gradients (+ the PCK counts of the last stack when accuracy=True)."""
-        if self.pose_topk or self.kd_topk:
+        if self.pose_temperature or self.kd_temperature:
+            losses, grads = ops.fpd_loss(outs, target, t_last, tw, self.alpha, losses_out=self.losses,
+                                         pose_topk=self.pose_topk, kd_topk=self.kd_topk,
+                                         pose_temperature=self.pose_temperature, kd_temperature=self.kd_temperature)
+        elif self.pose_topk or self.kd_topk:
             losses, grads = ops.fpd_loss(outs, target, t_last, tw, self.alpha, losses_out=self.losses,
                                          pose_topk=self.pose_topk, kd_topk=self.kd_topk)
         else:

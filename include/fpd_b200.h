@@ -348,6 +348,26 @@ int fpd_joints_ohkm(const float* out_nchw, const float* target_nchw, const float
                     float* loss3, float* grad, int B, int J, int hw, void* workspace, size_t workspace_bytes,
                     fpd_stream_t stream);
 
+/* JointsKLDLoss: channel-wise distillation per joint heat-map. With p = softmax(ref[b,j,:] / T) and
+ * q = softmax(out[b,j,:] / T) over the h*w pixels of each map,
+ *   L = T^2 / (B*J) * sum_{b,j} w[b,j] * KL(p || q),   dL/dout = T * w * (q - p) / (B*J).
+ * w = target_weight (enters linearly), or 1 when it is NULL. Deterministic (no atomics) and graph-capturable.
+ * Fused FPD form: the arguments of fpd_loss_ohkm_fused plus pose_temperature / kd_temperature. Each term is one of
+ * JointsMSELoss (topk 0, temperature 0), JointsOHKMMSELoss (topk > 0) or JointsKLDLoss (temperature > 0); a
+ * temperature must be 0 or finite and > 0, and a term may not have both. A kd topk or temperature needs a teacher.
+ * Same shape limits as fpd_loss_fused (h*w % 64 == 0, J <= 64, S <= 8). */
+size_t fpd_loss_kl_workspace_bytes(int S, int B, int J, int h, int w);
+int fpd_loss_kl_fused(const float* const* outs_host, int S, const float* target_nchw, const float* teacher_nhwc,
+                      const float* target_weight, float alpha, float* const* grads_host, float grad_scale,
+                      float* losses, int B, int J, int h, int w, int pose_topk, int kd_topk, float pose_temperature,
+                      float kd_temperature, void* workspace, size_t workspace_bytes, fpd_stream_t stream);
+/* Module form on NCHW tensors, any hw, J <= 64: temperature finite and > 0; loss3 (device, 3 floats, [0] is the
+ * loss); grad (optional) = dloss/dout, written everywhere; target_weight NULL = use_target_weight False. */
+size_t fpd_joints_kld_workspace_bytes(int B, int J, int hw);
+int fpd_joints_kld(const float* out_nchw, const float* target_nchw, const float* target_weight, float temperature,
+                   float* loss3, float* grad, int B, int J, int hw, void* workspace, size_t workspace_bytes,
+                   fpd_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------------------
  * Decode. Replaces the numpy round-trips of lib/core/function.py:218-240 (flip test),
  * lib/utils/transforms.py:15-29 (flip_back) and lib/core/inference.py:18-46 (get_max_preds).

@@ -1,13 +1,15 @@
 """Fused FPD loss time: fpd_loss_fused (both terms JointsMSELoss, one pass over the heat-maps) against
 fpd_loss_ohkm_fused (both terms JointsOHKMMSELoss, topk 8: sums, selection, gradient pass) at the two FPD bench
-shapes, value + gradient. Each variant is captured once in a CUDA graph of --launches calls and timed with CUDA events
+shapes, value + gradient. --kl adds fpd_loss_kl_fused (both terms JointsKLDLoss, T = 1: maxima and exp-sums, merge,
+gradient pass), and the time of one hg_fpd FPDTrainStep (bench.py's student, teacher and batch) with a JointsKLDLoss
+kd term against JointsMSELoss, the two steps alternating over --step-repeats windows of --step-iters replays. Each variant is captured once in a CUDA graph of --launches calls and timed with CUDA events
 over --repeats replays, the two variants alternating. Prints one JSON object with the card's name, power limit and the
 SM clock read after the timed windows.
 
-    python tools/bench_loss.py [--launches 200] [--repeats 7] [--out FILE]
+    python tools/bench_loss.py [--launches 200] [--repeats 7] [--kl] [--step-iters 20] [--step-repeats 5] [--out FILE]
 
 Bytes per call are what the kernels must move at least: every stack read once (MSE) or twice (OHKM), the target and
-the teacher read, every gradient written.
+the teacher read, every gradient written; KL reads every stack twice, like OHKM.
 """
 import argparse
 import json
@@ -31,10 +33,43 @@ def nvsmi(fields):
         return "unknown"
 
 
+def time_steps(args, dev):
+    """ms per hg_fpd FPDTrainStep (graph replay + fused Adam) with kd_temperature=1 against the MSE kd term."""
+    from bench import CONFIGS, build_models, synthetic_batch
+    from fpd_b200.train_step import FPDTrainStep
+    c = CONFIGS["hg_fpd"]
+    x, target, tw = (t.to(dev) for t in synthetic_batch(c["batch"], 1000, c["H"], c["W"], c["J"]))
+    steps = {}
+    for key, kw in (("mse", {}), ("kl_kd_T1", {"kd_temperature": 1.0})):
+        student, teacher = build_models("hg_fpd", dev)
+        steps[key] = FPDTrainStep(student, teacher, alpha=0.5, **kw)
+        for _ in range(3):
+            steps[key].step(x, target, tw)
+    torch.cuda.synchronize()
+    times = {k: [] for k in steps}
+    for _ in range(args.step_repeats):
+        for key, st in steps.items():
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            for _ in range(args.step_iters):
+                st.step(x, target, tw)
+            e1.record()
+            e1.synchronize()
+            times[key].append(e0.elapsed_time(e1) / args.step_iters)
+    out = {"iters_per_window": args.step_iters, "windows": args.step_repeats}
+    for key, ts in times.items():
+        ts = sorted(ts)
+        out[key] = {"ms_median": round(ts[len(ts) // 2], 3), "ms_min": round(ts[0], 3), "ms_max": round(ts[-1], 3)}
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--launches", type=int, default=200)
     ap.add_argument("--repeats", type=int, default=7)
+    ap.add_argument("--kl", action="store_true")
+    ap.add_argument("--step-iters", type=int, default=20)
+    ap.add_argument("--step-repeats", type=int, default=5)
     ap.add_argument("--out", default="")
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -53,6 +88,8 @@ def main():
         grads = [torch.empty_like(o) for o in outs]
         losses = torch.empty(3, device=dev)
         variants = {"mse": dict(), "ohkm_topk8": dict(pose_topk=8, kd_topk=8)}
+        if args.kl:
+            variants["kl_T1"] = dict(pose_temperature=1.0, kd_temperature=1.0)
         graphs = {}
         for key, kw in variants.items():
             side = torch.cuda.Stream()
@@ -80,6 +117,7 @@ def main():
         fmap = B * h * w * J * 4
         moved = {"mse": (S + 2 + S) * fmap if has_teacher else (S + 1 + S) * fmap,
                  "ohkm_topk8": (2 * S + 2 * (2 if has_teacher else 1) + S) * fmap}
+        moved["kl_T1"] = moved["ohkm_topk8"]
         entry = {"shape": name, "S": S, "B": B, "J": J, "hw": [h, w], "teacher": has_teacher}
         for key, ts in times.items():
             ts = sorted(ts)
@@ -87,7 +125,12 @@ def main():
                           "min_bytes": moved[key],
                           "GBps_at_median": round(moved[key] / (ts[len(ts) // 2] * 1e-6) / 1e9, 1)}
         entry["ohkm_over_mse"] = round(entry["ohkm_topk8"]["us_median"] / entry["mse"]["us_median"], 3)
+        if args.kl:
+            entry["kl_over_mse"] = round(entry["kl_T1"]["us_median"] / entry["mse"]["us_median"], 3)
+            entry["kl_over_ohkm"] = round(entry["kl_T1"]["us_median"] / entry["ohkm_topk8"]["us_median"], 3)
         result["shapes"].append(entry)
+    if args.kl:
+        result["hg_fpd_step"] = time_steps(args, dev)
     result["sm_clock_and_power_after"] = nvsmi("clocks.sm,power.draw")
     line = json.dumps(result)
     print(line)
