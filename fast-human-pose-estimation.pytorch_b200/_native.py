@@ -110,6 +110,9 @@ _SIGNATURES = {
                                   c_int, c_int, c_int, c_int, c_int, c_float, c_float, P, c_size_t, P]),
     "fpd_joints_kld_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "fpd_joints_kld": (c_int, [P, P, P, c_float, P, P, c_int, c_int, c_int, P, c_size_t, P]),
+    "fpd_kd_weights": (c_int, [P, P, c_float, P, c_int, c_int, c_int, c_int, P]),
+    "fpd_loss_kdw_fused": (c_int, [POINTER(c_void_p), c_int, P, P, P, P, c_float, POINTER(c_void_p), c_float, P, c_int,
+                                   c_int, c_int, c_int, c_int, c_int, c_float, c_float, P, c_size_t, P]),
     "fpd_flip_merge_argmax": (c_int, [P, P, P, c_int, P, P, P, c_int, c_int, c_int, c_int, P]),
     "fpd_argmax_nchw": (c_int, [P, P, P, c_int, c_int, P]),
     "fpd_final_preds": (c_int, [P, P, P, P, c_int, P, c_int, c_int, c_int, c_int, P]),

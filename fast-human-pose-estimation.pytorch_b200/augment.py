@@ -201,6 +201,33 @@ class RawJointsDataset(torch.utils.data.Dataset):
                 'out_size': self.image_size, 'mean': self.mean, 'std': self.std, 'meta': meta}
 
 
+def add_unlabeled_boxes(dataset, bbox_file, image_path=None, score_thre=0.0):
+    """Append the person boxes of a COCO-format detection list (the format of TEST.COCO_BBOX_FILE: a JSON list of
+    {"image_id", "category_id", "bbox": [x, y, w, h], "score"}) to dataset.db as unlabeled training records, for
+    distillation from unlabeled boxes (KD.UNLABELED). One record per box with category_id 1 and score >= score_thre:
+    centre and scale from dataset._box2cs(bbox), zero joints_3d and joints_3d_vis (so all-zero targets and target
+    weights), the detection score kept. image_path maps an image_id to a file (default: dataset.image_path_from_index).
+    Returns the number of records added. RawJointsDataset crops them as any record; with zero visibility there is no
+    half-body draw, as in the reference's __getitem__."""
+    import json
+    if image_path is None:
+        image_path = dataset.image_path_from_index
+    with open(bbox_file, 'r') as f:
+        boxes = json.load(f)
+    # the dataset's joint count; a dataset object without one takes it from its existing records
+    J = int(dataset.num_joints) if hasattr(dataset, 'num_joints') else len(dataset.db[0]['joints_3d'])
+    n = 0
+    for det in boxes:
+        if det['category_id'] != 1 or det['score'] < score_thre:
+            continue
+        center, scale = dataset._box2cs(det['bbox'])
+        dataset.db.append({'image': image_path(det['image_id']), 'center': center, 'scale': scale,
+                           'score': det['score'], 'joints_3d': np.zeros((J, 3), np.float64),
+                           'joints_3d_vis': np.zeros((J, 3), np.float64), 'filename': '', 'imgnum': 0})
+        n += 1
+    return n
+
+
 def raw_collate(items):
     """Batch of RawJointsDataset items -> dict of CPU tensors (pinned by the DataLoader's pin_memory):
     pixels uint8 [total bytes] (the regions back to back), desc int64 [N,7] (column 0 = byte offset), inv float64 [N,6],

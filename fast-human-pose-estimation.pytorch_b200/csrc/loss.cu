@@ -11,6 +11,8 @@
 //
 // Layouts: student / teacher heat-maps are the network-internal NHWC [B,h,w,J]; `target` is the caller's
 // NCHW [B,J,h,w] tensor (lib/dataset/JointsDataset.py target layout), staged through shared memory.
+#include <cooperative_groups.h>
+
 #include "common.cuh"
 
 namespace fpd {
@@ -25,10 +27,13 @@ struct StackPtrs {
   float* grad[kMaxStacks];
 };
 
+// KD_W: the kd term has its own weights kw (the pose term keeps tw). Where kw == tw the gradient is the expression of
+// the single-weight form, so equal weights give that form's bits.
+template <bool KD_W>
 __global__ void __launch_bounds__(kThreads)
 fpd_loss_kernel(StackPtrs sp, int S, const float* __restrict__ target, const float* __restrict__ teacher,
-                const float* __restrict__ tw, float alpha, float inv_norm, float grad_scale, int B, int J, int hw,
-                double* __restrict__ part /*[nblocks][2]*/) {
+                const float* __restrict__ tw, const float* __restrict__ kw, float alpha, float inv_norm,
+                float grad_scale, int B, int J, int hw, double* __restrict__ part /*[nblocks][2]*/) {
   extern __shared__ float tgt[];  // [J][kPix+1]
   const int blocks_per_img = hw / kPix;
   const int b = blockIdx.x / blocks_per_img;
@@ -44,6 +49,8 @@ fpd_loss_kernel(StackPtrs sp, int S, const float* __restrict__ target, const flo
     const int px = i / J, j = i % J;
     const float w = __ldg(tw + b * J + j);
     const float w2 = w * w;
+    const float k = KD_W ? __ldg(kw + b * J + j) : w;
+    const float k2 = k * k;
     const float g = tgt[j * (kPix + 1) + px];
     const float t = teacher ? __ldg(teacher + base + i) : 0.f;
     for (int s = 0; s < S; ++s) {
@@ -51,10 +58,14 @@ fpd_loss_kernel(StackPtrs sp, int S, const float* __restrict__ target, const flo
       const float dp = o - g;
       const float dk = o - t;
       pose = fmaf(w2 * dp, dp, pose);
-      if (teacher) kd = fmaf(w2 * dk, dk, kd);
+      if (teacher) kd = fmaf(k2 * dk, dk, kd);
       if (sp.grad[s]) {
-        const float gr = teacher ? ((1.f - alpha) * dp + alpha * dk) : dp;
-        sp.grad[s][base + i] = grad_scale * w2 * gr * inv_norm;
+        if (!KD_W || k == w) {
+          const float gr = teacher ? ((1.f - alpha) * dp + alpha * dk) : dp;
+          sp.grad[s][base + i] = grad_scale * w2 * gr * inv_norm;
+        } else {
+          sp.grad[s][base + i] = grad_scale * ((1.f - alpha) * w2 * dp + alpha * k2 * dk) * inv_norm;
+        }
       }
     }
   }
@@ -132,9 +143,15 @@ size_t fpd_loss_workspace_bytes(int B, int J, int h, int w) {
   return (size_t)nblocks * 2 * sizeof(double);
 }
 
-int fpd_loss_fused(const float* const* outs, int S, const float* target_nchw, const float* teacher_nhwc, const float* tw,
-                   float alpha, float* const* grads, float grad_scale, float* losses, int B, int J, int h, int w,
-                   void* workspace, size_t ws_bytes, fpd_stream_t stream) {
+}  // extern "C"
+
+namespace fpd {
+namespace {
+
+// kw: the kd term's weights, or NULL for tw (the single-weight kernel)
+int loss_mse_launch(const float* const* outs, int S, const float* target_nchw, const float* teacher_nhwc,
+                    const float* tw, const float* kw, float alpha, float* const* grads, float grad_scale, float* losses,
+                    int B, int J, int h, int w, void* workspace, size_t ws_bytes, fpd_stream_t stream) {
   FPD_REQUIRE(outs != nullptr, "fpd_loss_fused: outs_host is NULL");
   const int hw = h * w;
   FPD_REQUIRE(S >= 1 && S <= kMaxStacks, "fpd_loss: S=%d out of range [1,%d]", S, kMaxStacks);
@@ -149,13 +166,32 @@ int fpd_loss_fused(const float* const* outs, int S, const float* target_nchw, co
     sp.grad[s] = grads ? grads[s] : nullptr;
   }
   const double norm = (double)J * (double)B * (double)hw;
-  fpd_loss_kernel<<<nblocks, kThreads, (size_t)J * (kPix + 1) * sizeof(float), stream>>>(
-      sp, S, target_nchw, teacher_nhwc, tw, alpha, (float)(1.0 / norm), grad_scale, B, J, hw, (double*)workspace);
+  const size_t smem = (size_t)J * (kPix + 1) * sizeof(float);
+  if (kw)
+    fpd_loss_kernel<true><<<nblocks, kThreads, smem, stream>>>(sp, S, target_nchw, teacher_nhwc, tw, kw, alpha,
+                                                                (float)(1.0 / norm), grad_scale, B, J, hw,
+                                                                (double*)workspace);
+  else
+    fpd_loss_kernel<false><<<nblocks, kThreads, smem, stream>>>(sp, S, target_nchw, teacher_nhwc, tw, nullptr, alpha,
+                                                                 (float)(1.0 / norm), grad_scale, B, J, hw,
+                                                                 (double*)workspace);
   FPD_LAUNCH_CHECK();
   fpd_loss_final_kernel<<<1, 256, 0, stream>>>((const double*)workspace, nblocks, 0.5 / norm, alpha,
                                                teacher_nhwc != nullptr, losses);
   FPD_LAUNCH_CHECK();
   return FPD_OK;
+}
+
+}  // namespace
+}  // namespace fpd
+
+extern "C" {
+
+int fpd_loss_fused(const float* const* outs, int S, const float* target_nchw, const float* teacher_nhwc, const float* tw,
+                   float alpha, float* const* grads, float grad_scale, float* losses, int B, int J, int h, int w,
+                   void* workspace, size_t ws_bytes, fpd_stream_t stream) {
+  return loss_mse_launch(outs, S, target_nchw, teacher_nhwc, tw, nullptr, alpha, grads, grad_scale, losses, B, J, h, w,
+                         workspace, ws_bytes, stream);
 }
 
 int fpd_joints_mse(const float* out_nchw, const float* target_nchw, const float* tw, float* loss, float* grad_out, int B,
@@ -309,10 +345,11 @@ ohkm_sums_nchw_kernel(const float* __restrict__ out, const float* __restrict__ t
 
 // (2) one block per sample: per-(s, term, j) losses l = 0.5 * w^2 * sum / hw, then one warp per (s, term) selects and
 // writes the sample's share of the term (selected sum / topk, or sum / J for plain MSE) and the gradient
-// coefficients grad_scale * {1-alpha | alpha | 1} * w^2 / (B * {topk | J} * hw) of the selected joints.
+// coefficients grad_scale * {1-alpha | alpha | 1} * w^2 / (B * {topk | J} * hw) of the selected joints. w is tw for the
+// pose term and kw for the kd term.
 __global__ void __launch_bounds__(kThreads)
 ohkm_select_kernel(const double* __restrict__ part, int nch, int S, int J, int hw, int B, const float* __restrict__ tw,
-                   int has_teacher, int pose_topk, int kd_topk, float alpha, float grad_scale,
+                   const float* __restrict__ kw, int has_teacher, int pose_topk, int kd_topk, float alpha, float grad_scale,
                    double* __restrict__ contrib, float* __restrict__ coef) {
   __shared__ double ld[kMaxStacks * 2][kMaxJ];
   __shared__ float lf[kMaxStacks * 2][kMaxJ];
@@ -322,7 +359,8 @@ ohkm_select_kernel(const double* __restrict__ part, int nch, int S, int J, int h
     const int st = q / J, j = q % J;
     double acc = 0.0;
     for (int c = 0; c < nch; ++c) acc += part[((size_t)b * nch + c) * SJ2 + q];
-    const double w = tw ? (double)__ldg(tw + (size_t)b * J + j) : 1.0;
+    const float* wt = (st & 1) ? kw : tw;
+    const double w = wt ? (double)__ldg(wt + (size_t)b * J + j) : 1.0;
     const double l = 0.5 * (w * w) * acc / (double)hw;
     ld[st][j] = l;
     lf[st][j] = (float)l;
@@ -344,8 +382,9 @@ ohkm_select_kernel(const double* __restrict__ part, int nch, int S, int J, int h
     const int cnt = k > 0 ? k : J;
     const double factor = has_teacher ? (term ? (double)alpha : 1.0 - (double)alpha) : 1.0;
     const double scale = (double)grad_scale * factor / ((double)B * (double)cnt * (double)hw);
+    const float* wt = term ? kw : tw;
     for (int j = lane; j < J; j += 32) {
-      const double w = tw ? (double)__ldg(tw + (size_t)b * J + j) : 1.0;
+      const double w = wt ? (double)__ldg(wt + (size_t)b * J + j) : 1.0;
       cf[j] = ((mask >> j) & 1ull) ? (float)(scale * w * w) : 0.f;
     }
     if (lane == 0) {
@@ -460,10 +499,15 @@ size_t fpd_joints_ohkm_workspace_bytes(int B, int J) {
   return ohkm_ws_bytes(B, 1, 1, J);
 }
 
-int fpd_loss_ohkm_fused(const float* const* outs, int S, const float* target_nchw, const float* teacher_nhwc,
-                        const float* tw, float alpha, float* const* grads, float grad_scale, float* losses, int B, int J,
-                        int h, int w, int pose_topk, int kd_topk, void* workspace, size_t ws_bytes,
-                        fpd_stream_t stream) {
+}  // extern "C"
+
+namespace fpd {
+namespace {
+
+int loss_ohkm_launch(const float* const* outs, int S, const float* target_nchw, const float* teacher_nhwc,
+                     const float* tw, const float* kw, float alpha, float* const* grads, float grad_scale,
+                     float* losses, int B, int J, int h, int w, int pose_topk, int kd_topk, void* workspace,
+                     size_t ws_bytes, fpd_stream_t stream) {
   FPD_REQUIRE(outs != nullptr, "fpd_loss_ohkm_fused: outs_host is NULL");
   FPD_REQUIRE(S >= 1 && S <= kMaxStacks, "fpd_loss_ohkm: S=%d out of range [1,%d]", S, kMaxStacks);
   FPD_REQUIRE(B >= 1, "fpd_loss_ohkm: B=%d (an empty batch has no loss)", B);
@@ -494,8 +538,8 @@ int fpd_loss_ohkm_fused(const float* const* outs, int S, const float* target_nch
   ohkm_sums_nhwc_kernel<<<(int)(B * nch), kThreads, smem1, stream>>>(sp, S, target_nchw, teacher_nhwc, J, hw, ws.part);
   FPD_LAUNCH_CHECK();
   const int has_teacher = teacher_nhwc != nullptr;
-  ohkm_select_kernel<<<B, kThreads, 0, stream>>>(ws.part, (int)nch, S, J, hw, B, tw, has_teacher, pose_topk, kd_topk,
-                                                 alpha, grad_scale, ws.contrib, ws.coef);
+  ohkm_select_kernel<<<B, kThreads, 0, stream>>>(ws.part, (int)nch, S, J, hw, B, tw, kw, has_teacher, pose_topk,
+                                                 kd_topk, alpha, grad_scale, ws.contrib, ws.coef);
   FPD_LAUNCH_CHECK();
   ohkm_final_kernel<<<1, 32, 0, stream>>>(ws.contrib, B, S, has_teacher, alpha, losses);
   FPD_LAUNCH_CHECK();
@@ -505,6 +549,19 @@ int fpd_loss_ohkm_fused(const float* const* outs, int S, const float* target_nch
     FPD_LAUNCH_CHECK();
   }
   return FPD_OK;
+}
+
+}  // namespace
+}  // namespace fpd
+
+extern "C" {
+
+int fpd_loss_ohkm_fused(const float* const* outs, int S, const float* target_nchw, const float* teacher_nhwc,
+                        const float* tw, float alpha, float* const* grads, float grad_scale, float* losses, int B, int J,
+                        int h, int w, int pose_topk, int kd_topk, void* workspace, size_t ws_bytes,
+                        fpd_stream_t stream) {
+  return loss_ohkm_launch(outs, S, target_nchw, teacher_nhwc, tw, tw, alpha, grads, grad_scale, losses, B, J, h, w,
+                          pose_topk, kd_topk, workspace, ws_bytes, stream);
 }
 
 int fpd_joints_ohkm(const float* out_nchw, const float* target_nchw, const float* tw, int topk, float* loss3,
@@ -520,7 +577,7 @@ int fpd_joints_ohkm(const float* out_nchw, const float* target_nchw, const float
   const OhkmWs ws = ohkm_ws_split(workspace, B, 1, 1, J);
   ohkm_sums_nchw_kernel<<<B * J, kThreads, 0, stream>>>(out_nchw, target_nchw, J, hw, ws.part);
   FPD_LAUNCH_CHECK();
-  ohkm_select_kernel<<<B, kThreads, 0, stream>>>(ws.part, 1, 1, J, hw, B, tw, 0, topk, 0, 0.f, 1.f, ws.contrib,
+  ohkm_select_kernel<<<B, kThreads, 0, stream>>>(ws.part, 1, 1, J, hw, B, tw, tw, 0, topk, 0, 0.f, 1.f, ws.contrib,
                                                  ws.coef);
   FPD_LAUNCH_CHECK();
   ohkm_final_kernel<<<1, 32, 0, stream>>>(ws.contrib, B, 1, 0, 0.f, loss3);
@@ -699,7 +756,7 @@ kl_stats_kernel(StackPtrs sp, int S, const float* __restrict__ target, const flo
 // ohkm_final_kernel sums them) and the gradient constants. For a KL term l = T^2 w KL and every joint counts (1/J).
 __global__ void __launch_bounds__(kThreads)
 kl_select_kernel(const double* __restrict__ part, int nch, int S, int J, int hw, int B, const float* __restrict__ tw,
-                 int has_teacher, int pose_topk, int kd_topk, KlTerms tm, float alpha, float grad_scale,
+                 const float* __restrict__ kw, int has_teacher, int pose_topk, int kd_topk, KlTerms tm, float alpha, float grad_scale,
                  double* __restrict__ contrib, float4* __restrict__ coef) {
   __shared__ double ld[kMaxStacks * 2][kMaxJ];
   __shared__ float lf[kMaxStacks * 2][kMaxJ];
@@ -725,7 +782,8 @@ kl_select_kernel(const double* __restrict__ part, int nch, int S, int J, int hw,
   __syncthreads();
   for (int q = threadIdx.x; q < S * 2 * J; q += kThreads) {
     const int stt = q / J, j = q % J, term = stt & 1;
-    const double w = tw ? (double)__ldg(tw + (size_t)b * J + j) : 1.0;
+    const float* wt = term ? kw : tw;
+    const double w = wt ? (double)__ldg(wt + (size_t)b * J + j) : 1.0;
     const size_t off = (size_t)q * 3;
     double l = 0.0;
     if (term == 1 && !has_teacher) {
@@ -770,8 +828,9 @@ kl_select_kernel(const double* __restrict__ part, int nch, int S, int J, int hw,
     const double factor = has_teacher ? (term ? (double)alpha : 1.0 - (double)alpha) : 1.0;
     const double scale = kl ? (double)grad_scale * factor * (double)tm.t[term] / ((double)B * (double)J)
                             : (double)grad_scale * factor / ((double)B * (double)cnt * (double)hw);
+    const float* wt = term ? kw : tw;
     for (int j = lane; j < J; j += 32) {
-      const double w = tw ? (double)__ldg(tw + (size_t)b * J + j) : 1.0;
+      const double w = wt ? (double)__ldg(wt + (size_t)b * J + j) : 1.0;
       cf[j].x = ((mask >> j) & 1ull) ? (float)(kl ? scale * w : scale * w * w) : 0.f;
     }
     if (lane == 0) {
@@ -885,10 +944,15 @@ size_t fpd_joints_kld_workspace_bytes(int B, int J, int hw) {
   return kl_ws_bytes(B, ((int64_t)hw + kPix - 1) / kPix, 1, J) + 16;
 }
 
-int fpd_loss_kl_fused(const float* const* outs, int S, const float* target_nchw, const float* teacher_nhwc,
-                      const float* tw, float alpha, float* const* grads, float grad_scale, float* losses, int B, int J,
-                      int h, int w, int pose_topk, int kd_topk, float pose_temperature, float kd_temperature,
-                      void* workspace, size_t ws_bytes, fpd_stream_t stream) {
+}  // extern "C"
+
+namespace fpd {
+namespace {
+
+int loss_kl_launch(const float* const* outs, int S, const float* target_nchw, const float* teacher_nhwc,
+                   const float* tw, const float* kw, float alpha, float* const* grads, float grad_scale, float* losses,
+                   int B, int J, int h, int w, int pose_topk, int kd_topk, float pose_temperature,
+                   float kd_temperature, void* workspace, size_t ws_bytes, fpd_stream_t stream) {
   FPD_REQUIRE(outs != nullptr, "fpd_loss_kl_fused: outs_host is NULL");
   FPD_REQUIRE(S >= 1 && S <= kMaxStacks, "fpd_loss_kl: S=%d out of range [1,%d]", S, kMaxStacks);
   FPD_REQUIRE(B >= 1, "fpd_loss_kl: B=%d (an empty batch has no loss)", B);
@@ -935,8 +999,8 @@ int fpd_loss_kl_fused(const float* const* outs, int S, const float* target_nchw,
                                                                                     J, hw, tm, ws.part);
   FPD_LAUNCH_CHECK();
   const int has_teacher = teacher_nhwc != nullptr;
-  kl_select_kernel<<<B, kThreads, 0, stream>>>(ws.part, (int)nch, S, J, hw, B, tw, has_teacher, pose_topk, kd_topk, tm,
-                                               alpha, grad_scale, ws.contrib, ws.coef);
+  kl_select_kernel<<<B, kThreads, 0, stream>>>(ws.part, (int)nch, S, J, hw, B, tw, kw, has_teacher, pose_topk, kd_topk,
+                                               tm, alpha, grad_scale, ws.contrib, ws.coef);
   FPD_LAUNCH_CHECK();
   ohkm_final_kernel<<<1, 32, 0, stream>>>(ws.contrib, B, S, has_teacher, alpha, losses);
   FPD_LAUNCH_CHECK();
@@ -947,6 +1011,19 @@ int fpd_loss_kl_fused(const float* const* outs, int S, const float* target_nchw,
     FPD_LAUNCH_CHECK();
   }
   return FPD_OK;
+}
+
+}  // namespace
+}  // namespace fpd
+
+extern "C" {
+
+int fpd_loss_kl_fused(const float* const* outs, int S, const float* target_nchw, const float* teacher_nhwc,
+                      const float* tw, float alpha, float* const* grads, float grad_scale, float* losses, int B, int J,
+                      int h, int w, int pose_topk, int kd_topk, float pose_temperature, float kd_temperature,
+                      void* workspace, size_t ws_bytes, fpd_stream_t stream) {
+  return loss_kl_launch(outs, S, target_nchw, teacher_nhwc, tw, tw, alpha, grads, grad_scale, losses, B, J, h, w,
+                        pose_topk, kd_topk, pose_temperature, kd_temperature, workspace, ws_bytes, stream);
 }
 
 int fpd_joints_kld(const float* out_nchw, const float* target_nchw, const float* tw, float temperature, float* loss3,
@@ -975,8 +1052,8 @@ int fpd_joints_kld(const float* out_nchw, const float* target_nchw, const float*
   kl_stats_kernel<true><<<(int)(B * nch), kThreads, kl_stats_smem(1, J), stream>>>(sp, 1, target_nchw, nullptr, J, hw,
                                                                                   tm, ws.part);
   FPD_LAUNCH_CHECK();
-  kl_select_kernel<<<B, kThreads, 0, stream>>>(ws.part, (int)nch, 1, J, hw, B, tw, 0, 0, 0, tm, 0.f, 1.f, ws.contrib,
-                                               ws.coef);
+  kl_select_kernel<<<B, kThreads, 0, stream>>>(ws.part, (int)nch, 1, J, hw, B, tw, tw, 0, 0, 0, tm, 0.f, 1.f,
+                                               ws.contrib, ws.coef);
   FPD_LAUNCH_CHECK();
   ohkm_final_kernel<<<1, 32, 0, stream>>>(ws.contrib, B, 1, 0, 0.f, loss3);
   FPD_LAUNCH_CHECK();
@@ -989,6 +1066,119 @@ int fpd_joints_kld(const float* out_nchw, const float* target_nchw, const float*
     FPD_LAUNCH_CHECK();
   }
   return FPD_OK;
+}
+
+}  // extern "C"
+
+// ---------------------------------------------------------------------------------------------------------------
+// Distillation from unlabeled samples. A sample is unlabeled when all J of its target weights are exactly 0; its kd
+// weight for joint j is 1 when the teacher's map [b, :, :, j] has a maximum strictly above `thre` (a map holding a NaN
+// has a NaN maximum: weight 0), else 0. A labeled sample's kd weights are its target weights.
+//
+// fpd_kd_weights: one cluster of kKdSplit blocks per sample, each block takes the per-joint maxima of 1/kKdSplit of the
+// sample's pixels; block 0 of the cluster reads the others' maxima from their shared memory and writes the weights.
+// Maxima are exact, so the result does not depend on the order; no atomics, graph-capturable.
+//
+// fpd_loss_kdw_fused: the fused loss with the kd term weighted by kd_weight instead of target_weight. It runs the
+// launcher fpd_loss_fused / fpd_loss_ohkm_fused / fpd_loss_kl_fused would run for the same topks and temperatures.
+namespace fpd {
+namespace {
+
+namespace cg = cooperative_groups;
+
+constexpr int kKdSplit = 8;     // blocks per sample: one cluster
+constexpr int kKdUnroll = 8;    // loads in flight per thread
+
+// the larger of a and b; a NaN on either side wins
+__device__ __forceinline__ float max_nan(float a, float b) { return (isnan(a) || a > b) ? a : b; }
+
+__global__ void __cluster_dims__(kKdSplit, 1, 1) __launch_bounds__(kThreads)
+kd_weights_kernel(const float* __restrict__ teacher, const float* __restrict__ tw, float thre, int J, int hw,
+                  float* __restrict__ kdw) {
+  __shared__ float red[kThreads];
+  __shared__ float bmax[kMaxJ];
+  cg::cluster_group cluster = cg::this_cluster();
+  const int rank = (int)cluster.block_rank();
+  const int b = blockIdx.y;
+  const int t = threadIdx.x;
+  const int L = kThreads / J;     // pixel lanes: thread (pl, j) owns joint j, pixels p0 + pl, p0 + pl + L, ...
+  float m = -INFINITY;
+  if (t < L * J) {
+    const int j = t % J, pl = t / J;
+    const int64_t p1 = (int64_t)hw * (rank + 1) / kKdSplit;
+    const float* src = teacher + (int64_t)b * hw * J + j;
+    int64_t px = (int64_t)hw * rank / kKdSplit + pl;
+    for (; px + (kKdUnroll - 1) * L < p1; px += kKdUnroll * L) {
+      float v[kKdUnroll];
+#pragma unroll
+      for (int u = 0; u < kKdUnroll; ++u) v[u] = __ldg(src + (px + u * L) * J);
+#pragma unroll
+      for (int u = 0; u < kKdUnroll; ++u) m = max_nan(m, v[u]);
+    }
+    for (; px < p1; px += L) m = max_nan(m, __ldg(src + px * J));
+  }
+  red[t] = m;
+  __syncthreads();
+  if (t < J) {
+    float r = -INFINITY;
+    for (int l = 0; l < L; ++l) r = max_nan(r, red[l * J + t]);
+    bmax[t] = r;
+  }
+  cluster.sync();
+  if (rank == 0) {
+    const float w = t < J ? __ldg(tw + (size_t)b * J + t) : 0.f;
+    const int labeled = __syncthreads_or(w != 0.f);
+    if (t < J) {
+      float r = -INFINITY;
+      for (int q = 0; q < kKdSplit; ++q) r = max_nan(r, cluster.map_shared_rank(bmax, q)[t]);
+      kdw[(size_t)b * J + t] = labeled ? w : (r > thre ? 1.f : 0.f);
+    }
+  }
+  cluster.sync();   // every block's maxima stay in its shared memory until block 0 has read them
+}
+
+}  // namespace
+}  // namespace fpd
+
+extern "C" {
+
+int fpd_kd_weights(const float* teacher_nhwc, const float* tw, float thre, float* kd_weight, int B, int J, int h, int w,
+                   fpd_stream_t stream) {
+  FPD_REQUIRE(teacher_nhwc != nullptr && tw != nullptr && kd_weight != nullptr,
+              "kd_weights: teacher, target_weight or kd_weight is NULL");
+  FPD_REQUIRE(B >= 1 && B <= 65535, "kd_weights: B=%d out of range [1,65535]", B);
+  FPD_REQUIRE(J >= 1 && J <= kMaxJ, "kd_weights: J=%d out of range [1,%d]", J, kMaxJ);
+  FPD_REQUIRE(h >= 1 && w >= 1 && (int64_t)h * w <= (1 << 30), "kd_weights: heat-map %dx%d out of range", h, w);
+  FPD_REQUIRE(isfinite(thre), "kd_weights: thre=%g must be finite", (double)thre);
+  kd_weights_kernel<<<dim3(kKdSplit, B), kThreads, 0, stream>>>(teacher_nhwc, tw, thre, J, h * w, kd_weight);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int fpd_loss_kdw_fused(const float* const* outs, int S, const float* target_nchw, const float* teacher_nhwc,
+                       const float* tw, const float* kd_weight, float alpha, float* const* grads, float grad_scale,
+                       float* losses, int B, int J, int h, int w, int pose_topk, int kd_topk, float pose_temperature,
+                       float kd_temperature, void* workspace, size_t ws_bytes, fpd_stream_t stream) {
+  FPD_REQUIRE(outs != nullptr, "fpd_loss_kdw: outs_host is NULL");
+  FPD_REQUIRE(S >= 1 && S <= kMaxStacks, "fpd_loss_kdw: S=%d out of range [1,%d]", S, kMaxStacks);
+  FPD_REQUIRE(B >= 1, "fpd_loss_kdw: B=%d (an empty batch has no loss)", B);
+  FPD_REQUIRE(h >= 1 && w >= 1, "fpd_loss_kdw: empty heat-map %dx%d", h, w);
+  FPD_REQUIRE(target_nchw != nullptr && losses != nullptr && tw != nullptr,
+              "fpd_loss_kdw: target, losses or target_weight is NULL");
+  FPD_REQUIRE(teacher_nhwc != nullptr && kd_weight != nullptr, "fpd_loss_kdw: kd_weight and a teacher are required");
+  FPD_REQUIRE(workspace != nullptr, "fpd_loss_kdw: workspace is NULL");
+  for (int s = 0; s < S; ++s) {
+    FPD_REQUIRE(outs[s] != nullptr, "fpd_loss_kdw: outs[%d] is NULL", s);
+    FPD_REQUIRE(grads == nullptr || grads[s] != nullptr, "fpd_loss_kdw: grads[%d] is NULL", s);
+  }
+  if (pose_temperature != 0.f || kd_temperature != 0.f)
+    return loss_kl_launch(outs, S, target_nchw, teacher_nhwc, tw, kd_weight, alpha, grads, grad_scale, losses, B, J, h,
+                          w, pose_topk, kd_topk, pose_temperature, kd_temperature, workspace, ws_bytes, stream);
+  if (pose_topk != 0 || kd_topk != 0)
+    return loss_ohkm_launch(outs, S, target_nchw, teacher_nhwc, tw, kd_weight, alpha, grads, grad_scale, losses, B, J,
+                            h, w, pose_topk, kd_topk, workspace, ws_bytes, stream);
+  return loss_mse_launch(outs, S, target_nchw, teacher_nhwc, tw, kd_weight, alpha, grads, grad_scale, losses, B, J, h, w,
+                         workspace, ws_bytes, stream);
 }
 
 }  // extern "C"

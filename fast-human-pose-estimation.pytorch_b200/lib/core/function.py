@@ -16,6 +16,8 @@ What changes underneath:
     with the weight gradients on their own stream, PCK counts); the caller's optimizer then steps on the gradients. Losses
     and counts go to pinned host buffers asynchronously; the host waits only to log and at the end of the epoch. Other
     batch shapes (the short last batch) and config.DEBUG.DEBUG take the eager fused route, which gives the same bits.
+  * fpd_train with config.KD.UNLABELED: samples whose target weights are all 0 (unlabeled person boxes, augment.
+    add_unlabeled_boxes) are distilled from the teacher's confident joints (_kd_unlabeled_thre), on every route.
   * validate: for the fpd_b200 models with JointsMSELoss, JointsOHKMMSELoss or JointsKLDLoss, each batch is one CUDA graph replay (infer_step.
     FlipTestInference with its decode stage: both forwards, flip merge, loss, keypoints, PCK counts); the results are
     copied to pinned host buffers asynchronously and the host waits only to log and at the end of the epoch.
@@ -92,11 +94,33 @@ def _criterion_term(c, term):
     return {term + "_topk": c.topk if isinstance(c, JointsOHKMMSELoss) else 0}
 
 
-def _fused_step(model, tmodel, input, target, target_weight, alpha, use_tw, graph=None, **terms):
+def _kd_unlabeled_thre(config):
+    """config.KD.UNLABELED / KD.UNLABELED_THRE: None when distillation from unlabeled samples is off (keys absent or
+    UNLABELED false), else the confidence threshold (default 0.2, the reference's TEST.IN_VIS_THRE)."""
+    kd = getattr(config, "KD", None)
+    if kd is None or not bool(getattr(kd, "UNLABELED", False)):
+        return None
+    thre = getattr(kd, "UNLABELED_THRE", 0.2)
+    if isinstance(thre, bool) or not isinstance(thre, (int, float)) or not np.isfinite(thre):
+        raise ValueError("KD.UNLABELED_THRE=%r must be a finite number" % (thre,))
+    return float(thre)
+
+
+def _kd_weights_torch(toutput, target_weight, thre):
+    """ops.kd_weights in torch ops, for the generic route: toutput NCHW [B,J,h,w]; returns target_weight's shape."""
+    B, J = toutput.shape[:2]
+    tw = target_weight.reshape(B, J)
+    unlabeled = (tw == 0).all(dim=1, keepdim=True)
+    confident = (toutput.reshape(B, J, -1).amax(dim=2) > thre).to(tw.dtype)      # amax of a map with a NaN is NaN
+    return torch.where(unlabeled, confident, tw).reshape(target_weight.shape)
+
+
+def _fused_step(model, tmodel, input, target, target_weight, alpha, use_tw, graph=None, kd_unlabeled_thre=None,
+                **terms):
     """student fwd -> teacher fwd -> fused loss+grad -> backward tape; returns (losses[3] dev, last output NHWC).
     terms: the criteria's _criterion_term selectors. graph: a _GraphTraining whose batch shape this batch has -- the
     same step is then one replay of its graph, and the last output is None (the PCK counts come out of the graph
-    instead)."""
+    instead). kd_unlabeled_thre: the kd term is weighted by ops.kd_weights (distillation from unlabeled samples)."""
     if graph is not None:
         return graph.step(input, target, target_weight), None
     from fpd_b200 import ops
@@ -109,8 +133,10 @@ def _fused_step(model, tmodel, input, target, target_weight, alpha, use_tw, grap
     if tmodel is not None:
         t_last = _unwrap(tmodel).forward_nhwc(x, training=False)[-1]
     B, _, _, J = outs[0].shape
-    tw = target_weight.reshape(B, J) if use_tw else torch.ones(B, J, device=x.device)
-    losses, grads = ops.fpd_loss(outs, target.contiguous().float(), t_last, tw.contiguous().float(), alpha, **terms)
+    tw = (target_weight.reshape(B, J) if use_tw else torch.ones(B, J, device=x.device)).contiguous().float()
+    if kd_unlabeled_thre is not None:
+        terms["kd_weight"] = ops.kd_weights(t_last, tw, kd_unlabeled_thre)
+    losses, grads = ops.fpd_loss(outs, target.contiguous().float(), t_last, tw, alpha, **terms)
     pg = eng.backward(ctx, grads)
     params = [p for p in net.parameters() if p.requires_grad]      # frozen parameters keep whatever .grad they had
     glist = []
@@ -148,22 +174,25 @@ def _train_route(config, model, tmodel, criteria, target_shape):
 
 class _GraphTraining:
     """train()/fpd_train()'s per-batch work as replays of one FPDTrainStep(fused_adam=False, accuracy=True), which is
-    cached across calls keyed on the networks, the batch shapes, alpha and the loss terms (topks and temperatures).
+    cached across calls keyed on the networks, the batch shapes, alpha, the loss terms (topks and temperatures) and the
+    threshold of distillation from unlabeled samples (kd_unlabeled_thre, None: off).
     Losses and PCK counts go to pinned host buffers with non-blocking copies; `flush` waits for them and applies the
     meter updates in batch order. terms: the criteria's _criterion_term selectors."""
 
-    def __init__(self, model, tmodel, alpha, use_tw, terms, input, target, target_weight, num_batches):
+    def __init__(self, model, tmodel, alpha, use_tw, terms, input, target, target_weight, num_batches,
+                 kd_unlabeled_thre=None):
         from fpd_b200.train_step import FPDTrainStep
         net = _unwrap(model)
         tnet = _unwrap(tmodel) if tmodel is not None else None
         self.shapes = (tuple(input.shape), tuple(target.shape), tuple(target_weight.shape))
         alpha = float(alpha) if tnet is not None else 0.0
-        key = (id(net), id(tnet), self.shapes, alpha, tuple(sorted(terms.items())))
+        key = (id(net), id(tnet), self.shapes, alpha, tuple(sorted(terms.items())), kd_unlabeled_thre)
         step = _train_step_cache.get(key)
         if step is None:
             _train_step_cache.clear()          # one graph pool at a time
+            extra = {} if kd_unlabeled_thre is None else {"kd_unlabeled_thre": kd_unlabeled_thre}
             step = _train_step_cache[key] = FPDTrainStep(net, tnet, alpha=alpha, fused_adam=False, accuracy=True,
-                                                         **terms)
+                                                         **terms, **extra)
         self.train_step = step
         self.trainable = [(p, g) for p, g in zip(step.params, step.grad_views) if p.requires_grad]
         B, J = target.shape[0], target.shape[1]
@@ -321,7 +350,18 @@ def train(config, train_loader, model, criterion, optimizer, epoch, output_dir, 
 def fpd_train(config, train_loader, model, tmodel, pose_criterion, kd_pose_criterion, optimizer, epoch,
               output_dir, tb_log_dir, writer_dict):
     """Fast-Pose-Distillation epoch (reference function.py:99-187):
-    loss = (1-KD.ALPHA) * sum_s L(out_s, target) + KD.ALPHA * sum_s L(out_s, teacher_last)."""
+    loss = (1-KD.ALPHA) * sum_s L(out_s, target) + KD.ALPHA * sum_s L(out_s, teacher_last).
+    With config.KD.UNLABELED the kd term of a sample whose target weights are all 0 is weighted by the teacher's
+    confident joints (last-stack map maximum > KD.UNLABELED_THRE) instead; both criteria need use_target_weight."""
+    kd_thre = _kd_unlabeled_thre(config)
+    if kd_thre is not None:
+        if tmodel is None:
+            raise ValueError("KD.UNLABELED needs a teacher")
+        if not (getattr(pose_criterion, "use_target_weight", False)
+                and getattr(kd_pose_criterion, "use_target_weight", False)):
+            raise ValueError("KD.UNLABELED needs LOSS.USE_TARGET_WEIGHT: without target weights unlabeled samples cannot "
+                             "be told apart, and the pose term would pull them towards empty heat-maps")
+    unl = {} if kd_thre is None else {"kd_unlabeled_thre": kd_thre}
     batch_time, data_time = AverageMeter(), AverageMeter()
     losses, pose_losses, kd_pose_losses, acc = AverageMeter(), AverageMeter(), AverageMeter(), AverageMeter()
     alpha = config.KD.ALPHA
@@ -352,14 +392,14 @@ def fpd_train(config, train_loader, model, tmodel, pose_criterion, kd_pose_crite
             shape_checked = True
             if route == "graph":
                 graph = _GraphTraining(model, tmodel, alpha, pose_criterion.use_target_weight, terms, input, target,
-                                       target_weight, len(train_loader))
+                                       target_weight, len(train_loader), **unl)
         replay = graph if graph is not None and graph.accepts(input, target, target_weight) else None
         if graph is not None and replay is None:
             graph.flush(apply)          # meter updates stay in batch order
         if fused:
             optimizer.zero_grad()
             l3, out_nhwc = _fused_step(model, tmodel, input, target, target_weight, alpha,
-                                       pose_criterion.use_target_weight, replay, **terms)
+                                       pose_criterion.use_target_weight, replay, **terms, **unl)
             optimizer.step()
             if replay is not None:
                 replay.record(i, l3, input.size(0))
@@ -380,11 +420,12 @@ def fpd_train(config, train_loader, model, tmodel, pose_criterion, kd_pose_crite
             if isinstance(toutput, list):
                 toutput = toutput[-1]
             outs = outputs if isinstance(outputs, list) else [outputs]
+            kd_weight = target_weight if kd_thre is None else _kd_weights_torch(toutput, target_weight, kd_thre)
             pose_loss = pose_criterion(outs[0], target, target_weight)
-            kd_pose_loss = kd_pose_criterion(outs[0], toutput, target_weight)
+            kd_pose_loss = kd_pose_criterion(outs[0], toutput, kd_weight)
             for output in outs[1:]:
                 pose_loss += pose_criterion(output, target, target_weight)
-                kd_pose_loss += kd_pose_criterion(output, toutput, target_weight)
+                kd_pose_loss += kd_pose_criterion(output, toutput, kd_weight)
             loss = (1 - alpha) * pose_loss + alpha * kd_pose_loss
             optimizer.zero_grad()
             loss.backward()

@@ -32,18 +32,29 @@ def _chk(t, name):
 class Workspace:
     """Grow-only scratch buffers handed to the kernels that need one (no allocation at call time once warm).
     One buffer per CUDA stream: kernels enqueued on different streams (teacher / weight-gradient side streams) may run
-    concurrently and must not share reduction scratch."""
+    concurrently and must not share reduction scratch.
+    A buffer that was handed to a CUDA graph capture is kept when a larger request outgrows it: the graph holds its
+    address. Streams come from torch's pool of 32, so two captured steps in one process (e.g. two FPDTrainSteps) can share
+    a stream handle, and the second one's larger request must not free memory the first one's graph still writes. Other
+    outgrown buffers are freed."""
 
     def __init__(self):
         self.bufs = {}
+        self.in_graph = set()      # keys whose current buffer a capture has taken
+        self.outgrown = []         # outgrown buffers that captured graphs may still use
 
     def get(self, nbytes, device):
         nbytes = int(nbytes)
         key = (device, torch.cuda.current_stream(device).cuda_stream)
         buf = self.bufs.get(key)
         if buf is None or buf.numel() < nbytes:
+            if key in self.in_graph:
+                self.outgrown.append(buf)
+                self.in_graph.discard(key)
             buf = torch.empty(max(nbytes, 1 << 20), dtype=torch.uint8, device=device)
             self.bufs[key] = buf
+        if torch.cuda.is_current_stream_capturing():
+            self.in_graph.add(key)
         return buf
 
 
@@ -777,12 +788,38 @@ def _check_temperature(t, name, allow_zero):
     return float(t)
 
 
+def check_kd_unlabeled_thre(thre):
+    """The confidence threshold of distillation from unlabeled samples: a finite number."""
+    if isinstance(thre, bool) or not isinstance(thre, numbers.Real) or not math.isfinite(thre):
+        raise ValueError("kd_unlabeled_thre=%r must be a finite number" % (thre,))
+    return float(thre)
+
+
+def kd_weights(teacher_nhwc, target_weight, thre, out=None):
+    """The kd term's weights [B,J] (device) for distillation from unlabeled samples: a sample whose target weights are
+    all exactly 0 gets 1.0 for joint j when the teacher's map teacher_nhwc[b, :, :, j] has a maximum > thre (0.0
+    otherwise, and for a map holding a NaN); every other sample keeps its target weights."""
+    thre = check_kd_unlabeled_thre(thre)
+    if teacher_nhwc is None:
+        raise ValueError("kd_weights: the teacher's heat-maps are required")
+    _chk(teacher_nhwc, "teacher")
+    B, h, w, J = teacher_nhwc.shape
+    tw = target_weight.reshape(B, J).contiguous()
+    _chk(tw, "target_weight")
+    kdw = out if out is not None else torch.empty(B, J, dtype=torch.float32, device=teacher_nhwc.device)
+    N.check(N.lib().fpd_kd_weights(_p(teacher_nhwc), _p(tw), thre, _p(kdw), B, J, h, w, _stream()), "kd_weights")
+    return kdw
+
+
 def fpd_loss(outs_nhwc, target_nchw, teacher_nhwc, target_weight, alpha, want_grads=True, grad_scale=1.0,
-             grads_out=None, losses_out=None, pose_topk=0, kd_topk=0, pose_temperature=0, kd_temperature=0):
+             grads_out=None, losses_out=None, pose_topk=0, kd_topk=0, pose_temperature=0, kd_temperature=0,
+             kd_weight=None):
     """Fused FPD loss. outs_nhwc: list of [B,h,w,J]; returns (losses[3] device tensor, grads list or None).
     pose_topk / kd_topk > 0 make that term JointsOHKMMSELoss(topk) instead of JointsMSELoss (fpd_loss_ohkm_fused);
     pose_temperature / kd_temperature > 0 make it JointsKLDLoss(temperature) (fpd_loss_kl_fused, which takes any mix
-    of the three kinds). A term cannot have both a topk and a temperature."""
+    of the three kinds). A term cannot have both a topk and a temperature.
+    kd_weight [B,J] (e.g. kd_weights(...)) weights the kd term in place of target_weight (fpd_loss_kdw_fused, which
+    runs the same kernels); None is target_weight."""
     pose_temperature = _check_temperature(pose_temperature, "pose_temperature", True)
     kd_temperature = _check_temperature(kd_temperature, "kd_temperature", True)
     if (pose_topk and pose_temperature) or (kd_topk and kd_temperature):
@@ -797,6 +834,26 @@ def fpd_loss(outs_nhwc, target_nchw, teacher_nhwc, target_weight, alpha, want_gr
         grads = grads_out if grads_out is not None else [torch.empty_like(o) for o in outs_nhwc]
     outs_arr = (ctypes.c_void_p * S)(*[o.data_ptr() for o in outs_nhwc])
     grads_arr = (ctypes.c_void_p * S)(*[g.data_ptr() for g in grads]) if grads is not None else None
+    if kd_weight is not None:
+        if teacher_nhwc is None:
+            raise ValueError("fpd_loss: kd_weight without a teacher")
+        pose_topk = _check_topk(pose_topk, J, 0, "pose_topk")
+        kd_topk = _check_topk(kd_topk, J, 0, "kd_topk")
+        kdw = kd_weight.reshape(B, J).contiguous()
+        for t in list(outs_nhwc) + [target_nchw, teacher_nhwc, tw, kdw]:
+            _chk(t, "fpd_loss argument")
+        if pose_temperature or kd_temperature:
+            nbytes = N.lib().fpd_loss_kl_workspace_bytes(S, B, J, h, w)
+        elif pose_topk or kd_topk:
+            nbytes = N.lib().fpd_loss_ohkm_workspace_bytes(S, B, J, h, w)
+        else:
+            nbytes = N.lib().fpd_loss_workspace_bytes(B, J, h, w)
+        ws = _ws.get(nbytes, dev)
+        N.check(N.lib().fpd_loss_kdw_fused(outs_arr, S, _p(target_nchw), _p(teacher_nhwc), _p(tw), _p(kdw),
+                                           float(alpha), grads_arr, float(grad_scale), _p(losses), B, J, h, w,
+                                           pose_topk, kd_topk, pose_temperature, kd_temperature, _p(ws), ws.numel(),
+                                           _stream()), "loss_kdw_fused")
+        return losses, grads
     if pose_temperature or kd_temperature:
         pose_topk = _check_topk(pose_topk, J, 0, "pose_topk")
         kd_topk = _check_topk(kd_topk, J, 0, "kd_topk")

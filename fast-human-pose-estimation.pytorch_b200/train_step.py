@@ -12,7 +12,8 @@ eager ATen launches plus a DataParallel replicate/scatter/gather. Here the same 
 With fused_adam=False the step stops after the all-reduce: the parameters keep their own storage and the caller's
 optimizer (any torch.optim optimizer, its state dict, LR schedules) steps on the per-parameter views of the flat gradient
 buffer -- lib/core/function.py's train / fpd_train run this way. pose_topk / kd_topk select JointsOHKMMSELoss for a term,
-pose_temperature / kd_temperature JointsKLDLoss; accuracy=True adds accuracy()'s PCK counts of the last stack to the graph.
+pose_temperature / kd_temperature JointsKLDLoss; accuracy=True adds accuracy()'s PCK counts of the last stack to the graph;
+kd_unlabeled_thre distils from unlabeled samples (ops.kd_weights weights the kd term, inside the graph).
 
 The teacher is forward-only (its gradients never influence the student update; the reference's teacher
 backward is wasted work). `plain=True` drops the teacher (function.train semantics,
@@ -73,14 +74,17 @@ def _check_topk(value, name):
 class FPDTrainStep:
     def __init__(self, student, teacher=None, alpha=0.5, lr=2.5e-4, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0,
                  process_group=None, use_graph=True, pose_topk=0, kd_topk=0, fused_adam=True, accuracy=False,
-                 pose_temperature=0.0, kd_temperature=0.0):
+                 pose_temperature=0.0, kd_temperature=0.0, kd_unlabeled_thre=None):
         """pose_topk / kd_topk: > 0 makes that loss term JointsOHKMMSELoss(topk) instead of JointsMSELoss.
         pose_temperature / kd_temperature: > 0 makes that term JointsKLDLoss(temperature) (not together with a topk).
         fused_adam=False (external-optimizer mode): step() stops once the gradients are in the flat gradient buffer
         (all-reduced, mean over ranks); the parameters keep their own storage and the caller's optimizer steps on
         `grad_views`. lr / betas / eps / weight_decay are then unused.
         accuracy=True: the step also computes accuracy()'s per-joint PCK counts of the last stack (`counts`, int32 [J,2],
-        lib.core.evaluate.pck_from_counts)."""
+        lib.core.evaluate.pck_from_counts).
+        kd_unlabeled_thre: None (off), or distil from unlabeled samples, those whose target weights are all exactly 0:
+        their kd term is weighted by the teacher's confident joints (last-stack map maximum > kd_unlabeled_thre,
+        ops.kd_weights), while labeled samples keep their target weights. Needs a teacher and real target weights."""
         pose_topk, kd_topk = _check_topk(pose_topk, "pose_topk"), _check_topk(kd_topk, "kd_topk")
         if kd_topk and teacher is None:
             raise ValueError("kd_topk=%d needs a teacher" % kd_topk)
@@ -90,6 +94,11 @@ class FPDTrainStep:
             raise ValueError("kd_temperature=%r needs a teacher" % kd_temperature)
         if (pose_topk and pose_temperature) or (kd_topk and kd_temperature):
             raise ValueError("a loss term is JointsOHKMMSELoss (topk) or JointsKLDLoss (temperature), not both")
+        if kd_unlabeled_thre is not None:
+            kd_unlabeled_thre = ops.check_kd_unlabeled_thre(kd_unlabeled_thre)
+            if teacher is None:
+                raise ValueError("kd_unlabeled_thre=%r needs a teacher" % kd_unlabeled_thre)
+        self.kd_unlabeled_thre = kd_unlabeled_thre
         self.student, self.teacher = student, teacher
         self.alpha = float(alpha) if teacher is not None else 0.0
         self.lr, self.betas, self.eps, self.wd = lr, betas, eps, weight_decay
@@ -201,7 +210,14 @@ class FPDTrainStep:
 
     def _loss(self, outs, target, t_last, tw):
         """The fused FPD loss and its gradients (+ the PCK counts of the last stack when accuracy=True)."""
-        if self.pose_temperature or self.kd_temperature:
+        if self.kd_unlabeled_thre is not None:
+            # the teacher's stream has joined by now: t_last is complete
+            kdw = ops.kd_weights(t_last, tw, self.kd_unlabeled_thre)
+            losses, grads = ops.fpd_loss(outs, target, t_last, tw, self.alpha, losses_out=self.losses,
+                                         pose_topk=self.pose_topk, kd_topk=self.kd_topk,
+                                         pose_temperature=self.pose_temperature, kd_temperature=self.kd_temperature,
+                                         kd_weight=kdw)
+        elif self.pose_temperature or self.kd_temperature:
             losses, grads = ops.fpd_loss(outs, target, t_last, tw, self.alpha, losses_out=self.losses,
                                          pose_topk=self.pose_topk, kd_topk=self.kd_topk,
                                          pose_temperature=self.pose_temperature, kd_temperature=self.kd_temperature)

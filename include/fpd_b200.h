@@ -367,6 +367,21 @@ size_t fpd_joints_kld_workspace_bytes(int B, int J, int hw);
 int fpd_joints_kld(const float* out_nchw, const float* target_nchw, const float* target_weight, float temperature,
                    float* loss3, float* grad, int B, int J, int hw, void* workspace, size_t workspace_bytes,
                    fpd_stream_t stream);
+/* Distillation from unlabeled samples. teacher_nhwc [B,h,w,J] (the teacher's last stack), target_weight [B,J];
+ * writes kd_weight [B,J] (device): a sample whose J target weights are all exactly 0 (unlabeled) gets 1 for joint j
+ * when the maximum of teacher[b,:,:,j] is > thre (a map holding a NaN gets 0) and 0 otherwise; any other sample gets
+ * its target weights. thre finite, J <= 64. No atomics, graph-capturable. */
+int fpd_kd_weights(const float* teacher_nhwc, const float* target_weight, float thre, float* kd_weight, int B, int J,
+                   int h, int w, fpd_stream_t stream);
+/* The fused FPD loss with the kd term weighted by kd_weight [B,J] (where it enters exactly as target_weight does)
+ * and the pose term by target_weight. Arguments as fpd_loss_kl_fused, plus kd_weight; a teacher is required. Runs
+ * what fpd_loss_fused (no topk, no temperature), fpd_loss_ohkm_fused (a topk) or fpd_loss_kl_fused (a temperature)
+ * runs, with that entry point's workspace; kd_weight == target_weight gives that entry point's bits. */
+int fpd_loss_kdw_fused(const float* const* outs_host, int S, const float* target_nchw, const float* teacher_nhwc,
+                       const float* target_weight, const float* kd_weight, float alpha, float* const* grads_host,
+                       float grad_scale, float* losses, int B, int J, int h, int w, int pose_topk, int kd_topk,
+                       float pose_temperature, float kd_temperature, void* workspace, size_t workspace_bytes,
+                       fpd_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------
  * Decode. Replaces the numpy round-trips of lib/core/function.py:218-240 (flip test),
