@@ -113,6 +113,8 @@ _SIGNATURES = {
     "fpd_kd_weights": (c_int, [P, P, c_float, P, c_int, c_int, c_int, c_int, P]),
     "fpd_loss_kdw_fused": (c_int, [POINTER(c_void_p), c_int, P, P, P, P, c_float, POINTER(c_void_p), c_float, P, c_int,
                                    c_int, c_int, c_int, c_int, c_int, c_float, c_float, P, c_size_t, P]),
+    "fpd_feature_mse_workspace_bytes": (c_size_t, [c_int64]),
+    "fpd_feature_mse": (c_int, [P, P, c_int, c_float, P, P, P, c_int64, P, c_size_t, P]),
     "fpd_flip_merge_argmax": (c_int, [P, P, P, c_int, P, P, P, c_int, c_int, c_int, c_int, P]),
     "fpd_argmax_nchw": (c_int, [P, P, P, c_int, c_int, P]),
     "fpd_final_preds": (c_int, [P, P, P, P, c_int, P, c_int, c_int, c_int, c_int, P]),

@@ -1182,3 +1182,153 @@ int fpd_loss_kdw_fused(const float* const* outs, int S, const float* target_nchw
 }
 
 }  // extern "C"
+
+// ---------------------------------------------------------------------------------------------------------------
+// Feature distillation, a hint term in the FitNets sense (Romero et al., ICLR 2015). With a = A(s) the student's head
+// feature through the 1x1 adapter and t the teacher's head feature, both NHWC with n elements,
+//   L_feat = (1/n) * sum (a - t)^2,   grad = (2 * weight / n) * (a - t),   losses[2] += weight * L_feat.
+// One pass: each thread reads 4 consecutive elements of a and of t per step (t in fp32, or in fp16 widened on load),
+// writes the gradient and adds (a - t)^2 in fp64; each block writes one fp64 partial, and a one-block kernel adds the
+// partials in index order. No atomics and a grid that depends on n alone: runs and graph replays are bit-identical, and
+// an fp16 teacher gives the bits of the same teacher widened to fp32 (widening is exact). A NaN anywhere in a or t makes
+// L_feat NaN.
+namespace fpd {
+namespace {
+
+constexpr int kFeatBlocks = kNumSMs * 4;   // grid cap
+constexpr int kFeatUnroll = 4;             // 4-element steps in flight per thread
+
+__device__ __forceinline__ float4 feat_load4(const float* t, int64_t g) {
+  return __ldg(reinterpret_cast<const float4*>(t) + g);
+}
+__device__ __forceinline__ float4 feat_load4(const __half* t, int64_t g) {
+  const uint2 r = __ldg(reinterpret_cast<const uint2*>(t) + g);
+  const float2 lo = __half22float2(*reinterpret_cast<const __half2*>(&r.x));
+  const float2 hi = __half22float2(*reinterpret_cast<const __half2*>(&r.y));
+  return make_float4(lo.x, lo.y, hi.x, hi.y);
+}
+__device__ __forceinline__ float feat_load1(const float* t, int64_t i) { return __ldg(t + i); }
+__device__ __forceinline__ float feat_load1(const __half* t, int64_t i) { return __half2float(t[i]); }
+
+// VEC: n % 4 == 0 and every pointer aligned to its 4-element access (the host checks)
+template <typename T, bool VEC>
+__global__ void __launch_bounds__(kThreads)
+feature_mse_kernel(const float* __restrict__ a, const T* __restrict__ t, float coef, int64_t n,
+                   float* __restrict__ grad, double* __restrict__ part) {
+  double acc = 0.0;
+  const int64_t stride = (int64_t)gridDim.x * kThreads;
+  const int64_t first = (int64_t)blockIdx.x * kThreads + threadIdx.x;
+  if (VEC) {
+    const int64_t ng = n / 4;
+    for (int64_t g0 = first; g0 < ng; g0 += stride * kFeatUnroll) {
+      float4 av[kFeatUnroll], tv[kFeatUnroll];
+#pragma unroll
+      for (int u = 0; u < kFeatUnroll; ++u) {
+        const int64_t g = g0 + u * stride;
+        if (g < ng) {
+          av[u] = __ldg(reinterpret_cast<const float4*>(a) + g);
+          tv[u] = feat_load4(t, g);
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < kFeatUnroll; ++u) {
+        const int64_t g = g0 + u * stride;
+        if (g < ng) {
+          const float d0 = av[u].x - tv[u].x, d1 = av[u].y - tv[u].y, d2 = av[u].z - tv[u].z, d3 = av[u].w - tv[u].w;
+          acc = fma((double)d0, (double)d0, acc);
+          acc = fma((double)d1, (double)d1, acc);
+          acc = fma((double)d2, (double)d2, acc);
+          acc = fma((double)d3, (double)d3, acc);
+          reinterpret_cast<float4*>(grad)[g] = make_float4(coef * d0, coef * d1, coef * d2, coef * d3);
+        }
+      }
+    }
+  } else {
+    for (int64_t i = first; i < n; i += stride) {
+      const float d = __ldg(a + i) - feat_load1(t, i);
+      acc = fma((double)d, (double)d, acc);
+      grad[i] = coef * d;
+    }
+  }
+  __shared__ double red[kThreads / 32];
+  acc = warp_sum(acc);
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  if (lane == 0) red[wid] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+    for (int i = 0; i < kThreads / 32; ++i) s += red[i];
+    part[blockIdx.x] = s;
+  }
+}
+
+__global__ void __launch_bounds__(kThreads)
+feature_mse_final_kernel(const double* __restrict__ part, int nblocks, double inv_n, float weight,
+                         float* __restrict__ feat_loss, float* __restrict__ losses) {
+  __shared__ double red[kThreads / 32];
+  double s = 0.0;
+  for (int i = threadIdx.x; i < nblocks; i += kThreads) s += part[i];
+  s = warp_sum(s);
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  if (lane == 0) red[wid] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double tot = 0.0;
+    for (int i = 0; i < kThreads / 32; ++i) tot += red[i];
+    const double L = tot * inv_n;
+    feat_loss[0] = (float)L;
+    if (losses) losses[2] = (float)((double)losses[2] + (double)weight * L);
+  }
+}
+
+bool feature_vec_ok(const void* p, int64_t n, int align) {
+  return n % 4 == 0 && (reinterpret_cast<uintptr_t>(p) % align) == 0;
+}
+
+int feature_blocks(int64_t n, bool vec) {
+  const int64_t units = vec ? n / 4 : n;
+  int64_t nb = (units + (int64_t)kThreads * kFeatUnroll - 1) / ((int64_t)kThreads * kFeatUnroll);
+  if (nb > kFeatBlocks) nb = kFeatBlocks;
+  return nb < 1 ? 1 : (int)nb;
+}
+
+}  // namespace
+}  // namespace fpd
+
+extern "C" {
+
+size_t fpd_feature_mse_workspace_bytes(int64_t n) {
+  return (size_t)feature_blocks(n, false) * sizeof(double);
+}
+
+int fpd_feature_mse(const float* student, const void* teacher, int teacher_f16, float weight, float* grad,
+                    float* feat_loss, float* losses, int64_t n, void* workspace, size_t workspace_bytes,
+                    fpd_stream_t stream) {
+  FPD_REQUIRE(student != nullptr && teacher != nullptr && grad != nullptr && feat_loss != nullptr,
+              "fpd_feature_mse: student, teacher, grad or feat_loss is NULL");
+  FPD_REQUIRE(workspace != nullptr, "fpd_feature_mse: workspace is NULL");
+  FPD_REQUIRE(n >= 1, "fpd_feature_mse: n=%lld (an empty feature has no loss)", (long long)n);
+  FPD_REQUIRE(teacher_f16 == 0 || teacher_f16 == 1, "fpd_feature_mse: teacher_f16=%d must be 0 or 1", teacher_f16);
+  FPD_REQUIRE(isfinite(weight) && weight >= 0.f, "fpd_feature_mse: weight=%g must be finite and >= 0", (double)weight);
+  const bool vec = feature_vec_ok(student, n, 16) && feature_vec_ok(grad, n, 16) &&
+                   feature_vec_ok(teacher, n, teacher_f16 ? 8 : 16);
+  const int nblocks = feature_blocks(n, vec);
+  FPD_REQUIRE(workspace_bytes >= (size_t)nblocks * sizeof(double), "fpd_feature_mse: workspace too small");
+  const float coef = (float)(2.0 * (double)weight / (double)n);
+  double* part = (double*)workspace;
+  if (teacher_f16) {
+    const __half* t = (const __half*)teacher;
+    if (vec) feature_mse_kernel<__half, true><<<nblocks, kThreads, 0, stream>>>(student, t, coef, n, grad, part);
+    else feature_mse_kernel<__half, false><<<nblocks, kThreads, 0, stream>>>(student, t, coef, n, grad, part);
+  } else {
+    const float* t = (const float*)teacher;
+    if (vec) feature_mse_kernel<float, true><<<nblocks, kThreads, 0, stream>>>(student, t, coef, n, grad, part);
+    else feature_mse_kernel<float, false><<<nblocks, kThreads, 0, stream>>>(student, t, coef, n, grad, part);
+  }
+  FPD_LAUNCH_CHECK();
+  feature_mse_final_kernel<<<1, kThreads, 0, stream>>>(part, nblocks, 1.0 / (double)n, weight, feat_loss, losses);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+}  // extern "C"

@@ -127,6 +127,11 @@ class Var:
 STRIDE2_TC = os.environ.get("FPD_STRIDE2_TC", "1") != "0"
 
 
+# the ConvRef name of the feature distillation adapter: module names never contain "<", so it cannot collide with a
+# network's convolutions in PreparedWeights
+ADAPTER_CONV = "<feature_adapter>"
+
+
 class ConvRef:
     __slots__ = ("name", "weight", "bias", "k", "stride", "pad", "cin", "cout", "as_s1", "pick_first")
 
@@ -810,6 +815,7 @@ class Engine:
             y = self.residual_seq(ctx, y, "res.%d" % i, nb)
             y = self.conv(ctx, y, "fc.%d.0" % i, out_bn="fc.%d.1" % i)
             y = self.bn_act(ctx, y, "fc.%d.1" % i, relu=True)
+            ctx.head_feature = y        # the last stack's is what the heat-map head reads (feature distillation)
             score = self.conv(ctx, y, "score.%d" % i, head=True)
             outs.append(score)
             if i < net.num_stacks - 1:
@@ -832,8 +838,15 @@ class Engine:
             shared_stem["cols"] = ops.im2col(x, c.k, c.stride, c.pad, kpad)
 
     def run_network(self, ctx, img_nchw):
-        """Topology hook: subclasses (engine_hrnet.HRNetEngine) override this."""
+        """Topology hook: subclasses (engine_hrnet.HRNetEngine) override this. Sets ctx.head_feature to the Var the last
+        heat-map head reads, where the network materialises it."""
         return self.hourglass_net(ctx, img_nchw)
+
+    def feature_adapter(self, ctx, head_feature, conv):
+        """A(s): the feature distillation adapter `conv` (a 1x1 nn.Conv2d outside the network) applied to the head
+        feature Var, recorded on ctx's tape like the network's own convolutions, so that its backward accumulates into
+        head_feature.grad next to the head's and its parameter gradients land in ctx.pgrads."""
+        return self.conv(ctx, head_feature, ConvRef(ADAPTER_CONV, conv))
 
     # ------------------------------------------------------------------ entry points
     def forward(self, img_nchw, training, record_tape, shared_stem=None):
@@ -914,3 +927,4 @@ class _Ctx:
         self.wgrad_stream = None
         self.keepalive = []
         self.shared_stem = None
+        self.head_feature = None   # Var the last heat-map head reads (hourglass, HRNet; None for PoseResNet)

@@ -155,4 +155,5 @@ class HRNetEngine(Engine):
         for s, sc in zip((2, 3, 4), net.stage_cfgs):
             xs = self.transition(ctx, ys, "transition%d" % (s - 1), sc["num_branches"])
             ys = self.stage(ctx, xs, "stage%d" % s, sc["num_modules"])
+        ctx.head_feature = ys[0]        # the stage-4 high-resolution output final_layer reads (feature distillation)
         return [self.conv(ctx, ys[0], "final_layer", head=True)]

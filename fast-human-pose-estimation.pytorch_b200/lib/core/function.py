@@ -18,6 +18,8 @@ What changes underneath:
     batch shapes (the short last batch) and config.DEBUG.DEBUG take the eager fused route, which gives the same bits.
   * fpd_train with config.KD.UNLABELED: samples whose target weights are all 0 (unlabeled person boxes, augment.
     add_unlabeled_boxes) are distilled from the teacher's confident joints (_kd_unlabeled_thre), on every route.
+  * fpd_train with config.KD.FEATURE_WEIGHT > 0 and feature_adapter=: feature distillation from the teacher's head
+    feature (train_step.FeatureAdapter, ops.feature_mse) on the graph and the eager fused route; logged as FEAT_Loss.
   * validate: for the fpd_b200 models with JointsMSELoss, JointsOHKMMSELoss or JointsKLDLoss, each batch is one CUDA graph replay (infer_step.
     FlipTestInference with its decode stage: both forwards, flip merge, loss, keypoints, PCK counts); the results are
     copied to pinned host buffers asynchronously and the host waits only to log and at the end of the epoch.
@@ -116,11 +118,13 @@ def _kd_weights_torch(toutput, target_weight, thre):
 
 
 def _fused_step(model, tmodel, input, target, target_weight, alpha, use_tw, graph=None, kd_unlabeled_thre=None,
-                **terms):
+                feature_weight=0.0, feature_adapter=None, **terms):
     """student fwd -> teacher fwd -> fused loss+grad -> backward tape; returns (losses[3] dev, last output NHWC).
     terms: the criteria's _criterion_term selectors. graph: a _GraphTraining whose batch shape this batch has -- the
     same step is then one replay of its graph, and the last output is None (the PCK counts come out of the graph
-    instead). kd_unlabeled_thre: the kd term is weighted by ops.kd_weights (distillation from unlabeled samples)."""
+    instead). kd_unlabeled_thre: the kd term is weighted by ops.kd_weights (distillation from unlabeled samples).
+    feature_weight > 0: feature distillation through feature_adapter; the losses are then [4] (pose, kd, total,
+    feature) and the adapter's parameters get their .grad too."""
     if graph is not None:
         return graph.step(input, target, target_weight), None
     from fpd_b200 import ops
@@ -129,16 +133,28 @@ def _fused_step(model, tmodel, input, target, target_weight, alpha, use_tw, grap
     eng = net.engine()
     ctx = eng.forward(x, True, record_tape=True)
     outs = [v.data for v in ctx.outs]
-    t_last = None
+    t_last = t_ctx = None
     if tmodel is not None:
-        t_last = _unwrap(tmodel).forward_nhwc(x, training=False)[-1]
+        t_ctx = _unwrap(tmodel).engine().forward(x, False, record_tape=False)
+        t_last = t_ctx.outs[-1].data
     B, _, _, J = outs[0].shape
     tw = (target_weight.reshape(B, J) if use_tw else torch.ones(B, J, device=x.device)).contiguous().float()
     if kd_unlabeled_thre is not None:
         terms["kd_weight"] = ops.kd_weights(t_last, tw, kd_unlabeled_thre)
+    losses4 = None
+    if feature_weight:
+        losses4 = torch.zeros(4, dtype=torch.float32, device=x.device)
+        terms["losses_out"] = losses4[:3]
     losses, grads = ops.fpd_loss(outs, target.contiguous().float(), t_last, tw, alpha, **terms)
+    if feature_weight:
+        a = eng.feature_adapter(ctx, ctx.head_feature, feature_adapter.conv)
+        _, g = ops.feature_mse(a.data, t_ctx.head_feature.data, feature_weight, loss_out=losses4[3:], losses=losses)
+        a.add_grad(g, owned=False)
+        losses = losses4
     pg = eng.backward(ctx, grads)
     params = [p for p in net.parameters() if p.requires_grad]      # frozen parameters keep whatever .grad they had
+    if feature_weight:
+        params += [p for p in feature_adapter.parameters() if p.requires_grad]
     glist = []
     for p in params:
         g = pg.get(p)
@@ -159,6 +175,22 @@ _TRAIN_GRAPH = True
 _train_step_cache = {}      # key -> FPDTrainStep: one captured step, reused across epochs (it keeps the networks alive)
 
 
+def _feature_weight(config):
+    """config.KD.FEATURE_WEIGHT: the weight of feature distillation (0.0, off, when the key is absent)."""
+    from fpd_b200 import ops
+    kd = getattr(config, "KD", None)
+    return ops.check_feature_weight(getattr(kd, "FEATURE_WEIGHT", 0.0) if kd is not None else 0.0)
+
+
+def _check_feature_adapter_trains(adapter, optimizer):
+    """The adapter's parameters must be in the optimizer's param_groups, or they would never train."""
+    held = {id(p) for g in optimizer.param_groups for p in g["params"]}
+    if not all(id(p) in held for p in adapter.parameters()):
+        raise ValueError("KD.FEATURE_WEIGHT: the feature adapter's parameters are in none of the optimizer's "
+                         "param_groups (optimizer.add_param_group({'params': adapter.parameters()})): they would never "
+                         "train")
+
+
 def _train_route(config, model, tmodel, criteria, target_shape):
     """'graph', 'fused' or 'generic' for a train (tmodel None, one criterion) / fpd_train epoch whose first batch has
     targets of `target_shape`. The graph route replays exactly the eager fused route's kernels; debug images need the
@@ -174,30 +206,36 @@ def _train_route(config, model, tmodel, criteria, target_shape):
 
 class _GraphTraining:
     """train()/fpd_train()'s per-batch work as replays of one FPDTrainStep(fused_adam=False, accuracy=True), which is
-    cached across calls keyed on the networks, the batch shapes, alpha, the loss terms (topks and temperatures) and the
-    threshold of distillation from unlabeled samples (kd_unlabeled_thre, None: off).
+    cached across calls keyed on the networks, the batch shapes, alpha, the loss terms (topks and temperatures), the
+    threshold of distillation from unlabeled samples (kd_unlabeled_thre, None: off) and the feature distillation weight
+    and adapter.
     Losses and PCK counts go to pinned host buffers with non-blocking copies; `flush` waits for them and applies the
     meter updates in batch order. terms: the criteria's _criterion_term selectors."""
 
     def __init__(self, model, tmodel, alpha, use_tw, terms, input, target, target_weight, num_batches,
-                 kd_unlabeled_thre=None):
+                 kd_unlabeled_thre=None, feature_weight=0.0, feature_adapter=None):
         from fpd_b200.train_step import FPDTrainStep
         net = _unwrap(model)
         tnet = _unwrap(tmodel) if tmodel is not None else None
         self.shapes = (tuple(input.shape), tuple(target.shape), tuple(target_weight.shape))
         alpha = float(alpha) if tnet is not None else 0.0
         key = (id(net), id(tnet), self.shapes, alpha, tuple(sorted(terms.items())), kd_unlabeled_thre)
+        if feature_weight:
+            key += (feature_weight, id(feature_adapter))
         step = _train_step_cache.get(key)
         if step is None:
             _train_step_cache.clear()          # one graph pool at a time
             extra = {} if kd_unlabeled_thre is None else {"kd_unlabeled_thre": kd_unlabeled_thre}
+            if feature_weight:
+                extra.update(feature_weight=feature_weight, feature_adapter=feature_adapter)
             step = _train_step_cache[key] = FPDTrainStep(net, tnet, alpha=alpha, fused_adam=False, accuracy=True,
                                                          **terms, **extra)
         self.train_step = step
         self.trainable = [(p, g) for p, g in zip(step.params, step.grad_views) if p.requires_grad]
         B, J = target.shape[0], target.shape[1]
         self.ones = None if use_tw else torch.ones(B, J, device=target.device)
-        self.loss = torch.empty((num_batches, 3), dtype=torch.float32, pin_memory=True)
+        self.feature = bool(feature_weight)    # losses [4]: pose, kd, total, feature
+        self.loss = torch.empty((num_batches, 4 if self.feature else 3), dtype=torch.float32, pin_memory=True)
         self.counts = torch.empty((num_batches, J, 2), dtype=torch.int32, pin_memory=True)
         self.done = torch.cuda.Event()
         self.pending = []          # (batch, num_images) not yet applied to the meters
@@ -207,11 +245,11 @@ class _GraphTraining:
 
     def step(self, input, target, target_weight):
         """Replay (gradients all-reduced when there are several ranks) and hand the gradients to the parameters'
-        .grad, as _fused_step does; returns the device losses[3]."""
+        .grad, as _fused_step does; returns the device losses[3] (with feature distillation losses[4])."""
         l3 = self.train_step.step(input, target, target_weight if self.ones is None else self.ones)
         for p, g in self.trainable:     # frozen parameters keep whatever .grad they had
             p.grad = g
-        return l3
+        return self.train_step.losses_feature if self.feature else l3
 
     def record(self, i, l3, num_images):
         """Queue batch i's losses and PCK counts for the host (call after the optimizer step)."""
@@ -272,7 +310,7 @@ def _log_train(config, writer_dict, epoch, i, n_batches, batch_time, data_time, 
         step = writer_dict['train_global_steps']
         for label, m, _ in meters:
             tag = {'Loss': 'train_loss', 'POSE_Loss': 'train_pose_loss', 'KD_POSE_Loss': 'train_kd_pose_loss',
-                   'Accuracy': 'train_acc'}[label]
+                   'FEAT_Loss': 'train_feat_loss', 'Accuracy': 'train_acc'}[label]
             writer.add_scalar(tag, m.val, step)
         writer_dict['train_global_steps'] = step + 1
 
@@ -348,11 +386,14 @@ def train(config, train_loader, model, criterion, optimizer, epoch, output_dir, 
 
 
 def fpd_train(config, train_loader, model, tmodel, pose_criterion, kd_pose_criterion, optimizer, epoch,
-              output_dir, tb_log_dir, writer_dict):
+              output_dir, tb_log_dir, writer_dict, feature_adapter=None):
     """Fast-Pose-Distillation epoch (reference function.py:99-187):
     loss = (1-KD.ALPHA) * sum_s L(out_s, target) + KD.ALPHA * sum_s L(out_s, teacher_last).
     With config.KD.UNLABELED the kd term of a sample whose target weights are all 0 is weighted by the teacher's
-    confident joints (last-stack map maximum > KD.UNLABELED_THRE) instead; both criteria need use_target_weight."""
+    confident joints (last-stack map maximum > KD.UNLABELED_THRE) instead; both criteria need use_target_weight.
+    With config.KD.FEATURE_WEIGHT = w > 0, loss += w * mean((A(s) - t)^2), s and t the student's and the teacher's head
+    features and A feature_adapter (train_step.FeatureAdapter, whose parameters the optimizer must hold); fused routes
+    only."""
     kd_thre = _kd_unlabeled_thre(config)
     if kd_thre is not None:
         if tmodel is None:
@@ -362,25 +403,44 @@ def fpd_train(config, train_loader, model, tmodel, pose_criterion, kd_pose_crite
             raise ValueError("KD.UNLABELED needs LOSS.USE_TARGET_WEIGHT: without target weights unlabeled samples cannot "
                              "be told apart, and the pose term would pull them towards empty heat-maps")
     unl = {} if kd_thre is None else {"kd_unlabeled_thre": kd_thre}
+    feat_w = _feature_weight(config)
+    feat = {}
+    if feat_w:
+        if feature_adapter is None:
+            raise ValueError("KD.FEATURE_WEIGHT=%r needs fpd_train(..., feature_adapter=FeatureAdapter(student, teacher))"
+                             % feat_w)
+        from fpd_b200.train_step import check_feature_kd
+        check_feature_kd(_unwrap(model), _unwrap(tmodel) if tmodel is not None else None, feat_w, feature_adapter)
+        _check_feature_adapter_trains(feature_adapter, optimizer)
+        feat = {"feature_weight": feat_w, "feature_adapter": feature_adapter}
     batch_time, data_time = AverageMeter(), AverageMeter()
     losses, pose_losses, kd_pose_losses, acc = AverageMeter(), AverageMeter(), AverageMeter(), AverageMeter()
+    feat_losses = AverageMeter()
     alpha = config.KD.ALPHA
     model.train()
     tmodel.eval()
     fused = (_is_fpd_net(model) and _is_fpd_net(tmodel) and _is_fpd_criterion(pose_criterion)
              and _is_fpd_criterion(kd_pose_criterion)
              and pose_criterion.use_target_weight == kd_pose_criterion.use_target_weight)
+    if feat_w and not fused:
+        raise ValueError("KD.FEATURE_WEIGHT runs on the fused routes only (fpd_b200 hourglass / HRNet networks, "
+                         "JointsMSELoss / JointsOHKMMSELoss / JointsKLDLoss criteria with one use_target_weight); these "
+                         "arguments would take the generic autograd route")
     terms = {**_criterion_term(pose_criterion, "pose"), **_criterion_term(kd_pose_criterion, "kd")} if fused else None
     end = time.time()
     shape_checked = False
     graph = None
     meters = [('POSE_Loss', pose_losses, '%.5f'), ('KD_POSE_Loss', kd_pose_losses, '%.5f'), ('Loss', losses, '%.5f'),
               ('Accuracy', acc, '%.3f')]
+    if feat_w:
+        meters.insert(2, ('FEAT_Loss', feat_losses, '%.5f'))
 
     def apply(l3, avg_acc, cnt, n):
         pose_losses.update(l3[0], n)
         kd_pose_losses.update(l3[1], n)
         losses.update(l3[2], n)
+        if feat_w:
+            feat_losses.update(l3[3], n)
         acc.update(avg_acc, cnt)
     for i, (input, target, target_weight, meta) in enumerate(train_loader):
         data_time.update(time.time() - end)
@@ -390,16 +450,20 @@ def fpd_train(config, train_loader, model, tmodel, pose_criterion, kd_pose_crite
             route = _train_route(config, model, tmodel, [pose_criterion, kd_pose_criterion], target.shape)
             fused = route != "generic"
             shape_checked = True
+            if feat_w and not fused:
+                raise ValueError("KD.FEATURE_WEIGHT runs on the fused routes only: heat-maps of %dx%d with %d joints "
+                                 "would take the generic autograd route" % (target.shape[2], target.shape[3],
+                                                                            target.shape[1]))
             if route == "graph":
                 graph = _GraphTraining(model, tmodel, alpha, pose_criterion.use_target_weight, terms, input, target,
-                                       target_weight, len(train_loader), **unl)
+                                       target_weight, len(train_loader), **unl, **feat)
         replay = graph if graph is not None and graph.accepts(input, target, target_weight) else None
         if graph is not None and replay is None:
             graph.flush(apply)          # meter updates stay in batch order
         if fused:
             optimizer.zero_grad()
             l3, out_nhwc = _fused_step(model, tmodel, input, target, target_weight, alpha,
-                                       pose_criterion.use_target_weight, replay, **terms, **unl)
+                                       pose_criterion.use_target_weight, replay, **terms, **unl, **feat)
             optimizer.step()
             if replay is not None:
                 replay.record(i, l3, input.size(0))
@@ -410,7 +474,10 @@ def fpd_train(config, train_loader, model, tmodel, pose_criterion, kd_pose_crite
                     _log_train(config, writer_dict, epoch, i, len(train_loader), batch_time, data_time, meters,
                                input.size(0))
                 continue
-            pose_v, kd_v, loss_v = [float(v) for v in l3.cpu()]
+            lv = [float(v) for v in l3.cpu()]
+            pose_v, kd_v, loss_v = lv[:3]
+            if feat_w:
+                feat_losses.update(lv[3], input.size(0))
             avg_acc, cnt, pred = _device_accuracy(out_nhwc, target)
             last_out = out_nhwc
         else:

@@ -882,6 +882,40 @@ def fpd_loss(outs_nhwc, target_nchw, teacher_nhwc, target_weight, alpha, want_gr
     return losses, grads
 
 
+def check_feature_weight(weight):
+    """The feature distillation weight: a finite number >= 0 (0: off)."""
+    if isinstance(weight, bool) or not isinstance(weight, numbers.Real) or not (math.isfinite(weight) and weight >= 0):
+        raise ValueError("feature_weight=%r must be a finite number >= 0 (0: off)" % (weight,))
+    return float(weight)
+
+
+def feature_mse(student_nhwc, teacher_nhwc, weight, grad_out=None, loss_out=None, losses=None):
+    """Feature distillation loss (a FitNets hint) and its gradient: L_feat = mean((student - teacher)^2) over all
+    elements, grad = (2 * weight / n) * (student - teacher). student_nhwc: the adapted student head feature (fp32);
+    teacher_nhwc: the teacher's head feature of the same shape, fp32 or fp16 (read as stored, no conversion launch).
+    losses: an FPD losses[3] buffer, whose total losses[2] gains weight * L_feat. Returns (L_feat [1] device, grad)."""
+    weight = check_feature_weight(weight)
+    _chk(student_nhwc, "student feature")
+    if not (teacher_nhwc.is_cuda and teacher_nhwc.dtype in (torch.float32, torch.float16) and teacher_nhwc.is_contiguous()):
+        raise ValueError("teacher feature must be a contiguous fp32 or fp16 CUDA tensor (got %s %s %s)" % (
+            teacher_nhwc.device, teacher_nhwc.dtype, teacher_nhwc.is_contiguous()))
+    if tuple(student_nhwc.shape) != tuple(teacher_nhwc.shape):
+        raise ValueError("feature_mse: student feature %s and teacher feature %s differ in shape" % (
+            tuple(student_nhwc.shape), tuple(teacher_nhwc.shape)))
+    n = student_nhwc.numel()
+    if n == 0:
+        raise ValueError("feature_mse: empty feature")
+    dev = student_nhwc.device
+    grad = grad_out if grad_out is not None else torch.empty_like(student_nhwc)
+    loss = loss_out if loss_out is not None else torch.empty(1, dtype=torch.float32, device=dev)
+    for t, name in ((grad, "grad_out"), (loss, "loss_out"), (losses, "losses")):
+        _chk(t, name)
+    ws = _ws.get(N.lib().fpd_feature_mse_workspace_bytes(n), dev)
+    N.check(N.lib().fpd_feature_mse(_p(student_nhwc), _p(teacher_nhwc), int(teacher_nhwc.dtype == torch.float16), weight,
+                                    _p(grad), _p(loss), _p(losses), n, _p(ws), ws.numel(), _stream()), "feature_mse")
+    return loss, grad
+
+
 def joints_mse(out_nchw, target_nchw, target_weight=None, want_grad=True):
     B, J = out_nchw.shape[:2]
     hw = out_nchw.numel() // (B * J)

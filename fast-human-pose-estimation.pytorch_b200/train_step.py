@@ -13,7 +13,8 @@ With fused_adam=False the step stops after the all-reduce: the parameters keep t
 optimizer (any torch.optim optimizer, its state dict, LR schedules) steps on the per-parameter views of the flat gradient
 buffer -- lib/core/function.py's train / fpd_train run this way. pose_topk / kd_topk select JointsOHKMMSELoss for a term,
 pose_temperature / kd_temperature JointsKLDLoss; accuracy=True adds accuracy()'s PCK counts of the last stack to the graph;
-kd_unlabeled_thre distils from unlabeled samples (ops.kd_weights weights the kd term, inside the graph).
+kd_unlabeled_thre distils from unlabeled samples (ops.kd_weights weights the kd term, inside the graph); feature_weight with
+a FeatureAdapter adds feature distillation, a hint from the teacher's head feature (ops.feature_mse).
 
 The teacher is forward-only (its gradients never influence the student update; the reference's teacher
 backward is wasted work). `plain=True` drops the teacher (function.train semantics,
@@ -33,10 +34,12 @@ class FlatParams:
     """Re-homes a module's parameters as views into one flat fp32 buffer (needed for the single all-reduce and the
     single Adam launch). Parameter objects are preserved (only .data changes), so optimizers / state_dict keep
     working. rehome=False keeps the parameters' own storage and builds only the flat gradient buffer (`flat` is then
-    None)."""
+    None). extra: a second module whose parameters follow the first one's (the feature distillation adapter)."""
 
-    def __init__(self, net, rehome=True):
+    def __init__(self, net, rehome=True, extra=None):
         self.params = [p for p in net.parameters()]
+        if extra is not None:
+            self.params += [p for p in extra.parameters()]
         dev = self.params[0].device
         sizes = [p.numel() for p in self.params]
         # pad every tensor to a multiple of 4 floats so float4 kernels can run over the flat buffer
@@ -71,10 +74,67 @@ def _check_topk(value, name):
     return int(value)
 
 
+def head_feature_channels(net):
+    """Channels of the feature the network's last heat-map head reads: NUM_FEATURES for the hourglass (the last stack's
+    relu(bn(fc)), NUM_CHANNELS[0] for HRNet (the stage-4 branch-0 output). PoseResNet fuses its last BatchNorm + ReLU
+    into final_layer's operand pass and has no materialised head feature: ValueError."""
+    from .lib.models.hourglass import HourglassNet
+    from .lib.models.pose_hrnet import PoseHighResolutionNet
+    net = net.module if isinstance(net, torch.nn.DataParallel) else net
+    if isinstance(net, HourglassNet):
+        return net.fc[-1][0].out_channels
+    if isinstance(net, PoseHighResolutionNet):
+        return net.final_layer.in_channels
+    raise ValueError("feature distillation needs an hourglass (HourglassNet) or HRNet (PoseHighResolutionNet) network, "
+                     "got %s: PoseResNet has no materialised head feature" % type(net).__name__)
+
+
+class FeatureAdapter(torch.nn.Module):
+    """The 1x1 convolution (with bias) from the student's head-feature width to the teacher's that feature distillation
+    trains with the student: conv(s) is matched to the teacher's head feature. Initialised like the reference's HRNet /
+    pose_resnet convolutions (normal, std 0.001; zero bias). It is not a submodule of the student, so the student's
+    state_dict keeps the reference's keys: train and checkpoint it next to the student."""
+
+    def __init__(self, student, teacher):
+        super().__init__()
+        self.conv = torch.nn.Conv2d(head_feature_channels(student), head_feature_channels(teacher), 1, bias=True)
+        torch.nn.init.normal_(self.conv.weight, std=0.001)
+        torch.nn.init.constant_(self.conv.bias, 0)
+
+    def forward(self, x):
+        return self.conv(x)
+
+
+def check_feature_kd(student, teacher, weight, adapter):
+    """The arguments of feature distillation: -> the weight as a float (0.0: off). A weight > 0 needs a teacher and a
+    FeatureAdapter whose widths match the two networks' head features, on the student's device."""
+    from . import ops
+    weight = ops.check_feature_weight(weight)
+    if not weight:
+        return 0.0
+    if teacher is None:
+        raise ValueError("feature_weight=%r needs a teacher" % weight)
+    if adapter is None:
+        raise ValueError("feature_weight=%r needs a feature_adapter (FeatureAdapter(student, teacher))" % weight)
+    cs, ct = head_feature_channels(student), head_feature_channels(teacher)
+    conv = getattr(adapter, "conv", None)
+    if (not isinstance(conv, torch.nn.Conv2d) or conv.kernel_size != (1, 1) or conv.stride != (1, 1)
+            or conv.padding != (0, 0) or conv.groups != 1 or conv.bias is None):
+        raise ValueError("feature_adapter must be a FeatureAdapter: a module whose .conv is a 1x1 nn.Conv2d with a bias")
+    if (conv.in_channels, conv.out_channels) != (cs, ct):
+        raise ValueError("feature_adapter maps %d -> %d channels, the student's head feature has %d and the teacher's %d"
+                         % (conv.in_channels, conv.out_channels, cs, ct))
+    dev = next(student.parameters()).device
+    if any(p.device != dev for p in adapter.parameters()):
+        raise ValueError("feature_adapter must be on the student's device (%s)" % dev)
+    return weight
+
+
 class FPDTrainStep:
     def __init__(self, student, teacher=None, alpha=0.5, lr=2.5e-4, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0,
                  process_group=None, use_graph=True, pose_topk=0, kd_topk=0, fused_adam=True, accuracy=False,
-                 pose_temperature=0.0, kd_temperature=0.0, kd_unlabeled_thre=None):
+                 pose_temperature=0.0, kd_temperature=0.0, kd_unlabeled_thre=None, feature_weight=0.0,
+                 feature_adapter=None):
         """pose_topk / kd_topk: > 0 makes that loss term JointsOHKMMSELoss(topk) instead of JointsMSELoss.
         pose_temperature / kd_temperature: > 0 makes that term JointsKLDLoss(temperature) (not together with a topk).
         fused_adam=False (external-optimizer mode): step() stops once the gradients are in the flat gradient buffer
@@ -84,7 +144,12 @@ class FPDTrainStep:
         lib.core.evaluate.pck_from_counts).
         kd_unlabeled_thre: None (off), or distil from unlabeled samples, those whose target weights are all exactly 0:
         their kd term is weighted by the teacher's confident joints (last-stack map maximum > kd_unlabeled_thre,
-        ops.kd_weights), while labeled samples keep their target weights. Needs a teacher and real target weights."""
+        ops.kd_weights), while labeled samples keep their target weights. Needs a teacher and real target weights.
+        feature_weight > 0: feature distillation. feature_adapter (a FeatureAdapter(student, teacher)) maps the student's
+        head feature s to the teacher's width, and total += feature_weight * mean((A(s) - t)^2) over every element of
+        every sample, labeled or not (ops.feature_mse; not scaled by alpha). The adapter's parameters follow the
+        student's in the flat buffers (params, grad_views, fused Adam, state_dict); `feature_loss` is the device scalar
+        mean((A(s) - t)^2) of the latest step. Hourglass and HRNet networks only; not with FPD_PIPELINE_TEACHER."""
         pose_topk, kd_topk = _check_topk(pose_topk, "pose_topk"), _check_topk(kd_topk, "kd_topk")
         if kd_topk and teacher is None:
             raise ValueError("kd_topk=%d needs a teacher" % kd_topk)
@@ -99,6 +164,9 @@ class FPDTrainStep:
             if teacher is None:
                 raise ValueError("kd_unlabeled_thre=%r needs a teacher" % kd_unlabeled_thre)
         self.kd_unlabeled_thre = kd_unlabeled_thre
+        self.feature_weight = check_feature_kd(student, teacher, feature_weight, feature_adapter)
+        self.adapter = feature_adapter if self.feature_weight else None
+        self.feature_loss = None
         self.student, self.teacher = student, teacher
         self.alpha = float(alpha) if teacher is not None else 0.0
         self.lr, self.betas, self.eps, self.wd = lr, betas, eps, weight_decay
@@ -111,7 +179,7 @@ class FPDTrainStep:
         self.world = 1
         if process_group is not None or (torch.distributed.is_available() and torch.distributed.is_initialized()):
             self.world = torch.distributed.get_world_size(process_group)
-        self.flat = FlatParams(student, rehome=self.fused_adam)
+        self.flat = FlatParams(student, rehome=self.fused_adam, extra=self.adapter)
         self.exp_avg = torch.zeros_like(self.flat.flat) if self.fused_adam else None
         self.exp_avg_sq = torch.zeros_like(self.flat.flat) if self.fused_adam else None
         self.step_count = 0
@@ -124,6 +192,9 @@ class FPDTrainStep:
         self.overlap_teacher = os.environ.get("FPD_OVERLAP_TEACHER", "1") != "0"
         self.pipeline = (teacher is not None and use_graph and self.overlap_teacher
                          and os.environ.get("FPD_PIPELINE_TEACHER", "0") != "0")   # measured: no gain over the plain 2nd stream
+        if self.pipeline and self.feature_weight:
+            raise ValueError("feature distillation needs the teacher's head feature of the same batch: it does not run "
+                             "with the teacher pipelined (FPD_PIPELINE_TEACHER)")
         self.x_next = self.t_cur = self.t_next = None
         self._have_next = False
         self._static_shapes = None
@@ -204,9 +275,19 @@ class FPDTrainStep:
         outs = [v.data for v in ctx.outs]
         self.last_outs, self.last_teacher = outs, t_last
         losses, grads = self._loss(outs, target, t_last, tw)
+        if self.feature_weight:
+            self._feature_term(s_eng, ctx, t_ctx, losses)
         pg = s_eng.backward(ctx, grads, wgrad_stream=self._wstream)
         self._gather_grads(pg)
         return losses
+
+    def _feature_term(self, s_eng, ctx, t_ctx, losses):
+        """Feature distillation: A(s) on the student's tape, the hint loss added to losses[2], and its gradient seeded at
+        A(s) for the backward (the teacher's stream has joined: its head feature is complete)."""
+        a = s_eng.feature_adapter(ctx, ctx.head_feature, self.adapter.conv)
+        _, g = ops.feature_mse(a.data, t_ctx.head_feature.data, self.feature_weight, loss_out=self.feature_loss,
+                               losses=losses)
+        a.add_grad(g, owned=False)
 
     def _loss(self, outs, target, t_last, tw):
         """The fused FPD loss and its gradients (+ the PCK counts of the last stack when accuracy=True)."""
@@ -233,7 +314,12 @@ class FPDTrainStep:
 
     def _outputs(self, target):
         """The step's device outputs: losses[3] and, with accuracy=True, the PCK counts [J,2]."""
-        self.losses = torch.zeros(3, dtype=torch.float32, device=target.device)
+        if self.feature_weight:
+            # one buffer: losses[3] and the feature loss next to it (fpd_train copies all four with one copy)
+            self.losses_feature = torch.zeros(4, dtype=torch.float32, device=target.device)
+            self.losses, self.feature_loss = self.losses_feature[:3], self.losses_feature[3:]
+        else:
+            self.losses = torch.zeros(3, dtype=torch.float32, device=target.device)
         if self.want_accuracy:
             self.counts = torch.zeros((target.shape[1], 2), dtype=torch.int32, device=target.device)
 
@@ -357,7 +443,7 @@ class FPDTrainStep:
 
     @property
     def params(self):
-        """The student's parameters, in the order of `grad_views`."""
+        """The student's parameters (then the feature adapter's), in the order of `grad_views`."""
         return self.flat.params
 
     @property

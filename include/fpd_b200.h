@@ -382,6 +382,15 @@ int fpd_loss_kdw_fused(const float* const* outs_host, int S, const float* target
                        float grad_scale, float* losses, int B, int J, int h, int w, int pose_topk, int kd_topk,
                        float pose_temperature, float kd_temperature, void* workspace, size_t workspace_bytes,
                        fpd_stream_t stream);
+/* Feature distillation (a FitNets hint). student: the adapted student head feature A(s), fp32, n elements (NHWC);
+ * teacher: the teacher's head feature, same shape, fp32 (teacher_f16 = 0) or __half (teacher_f16 = 1, widened on load).
+ * Writes grad = (2 * weight / n) * (A(s) - t) (fp32, n elements), feat_loss[0] = (1/n) * sum (A(s) - t)^2 and, when
+ * losses is not NULL, adds weight * feat_loss to losses[2]. weight finite and >= 0. Fixed-order fp64 sums, no atomics,
+ * graph-capturable; an fp16 teacher gives the bits of the same teacher widened to fp32. */
+size_t fpd_feature_mse_workspace_bytes(int64_t n);
+int fpd_feature_mse(const float* student, const void* teacher, int teacher_f16, float weight, float* grad,
+                    float* feat_loss, float* losses, int64_t n, void* workspace, size_t workspace_bytes,
+                    fpd_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------
  * Decode. Replaces the numpy round-trips of lib/core/function.py:218-240 (flip test),
