@@ -120,6 +120,7 @@ _SIGNATURES = {
     "fpd_final_preds": (c_int, [P, P, P, P, c_int, P, c_int, c_int, c_int, c_int, P]),
     "fpd_final_preds_dark": (c_int, [P, P, P, P, c_int, P, c_int, c_int, c_int, c_int, P]),
     "fpd_pck_counts": (c_int, [P, P, P, P, P, c_int, c_int, c_int, c_int, P]),
+    "fpd_heatmap_resample": (c_int, [P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, P]),
     "fpd_nms_workspace_bytes": (c_size_t, [c_int]),
     "fpd_nms_device": (c_int, [P, c_int, c_int, c_float, P, P, P, c_size_t, P]),
     "fpd_nms_host": (c_int, [P, P, P, c_int, c_int, c_float, c_int]),

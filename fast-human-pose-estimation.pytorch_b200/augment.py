@@ -136,13 +136,27 @@ class RawJointsDataset(torch.utils.data.Dataset):
 
     udp=True crops with udp_crop_matrix instead of the reference's matrix, for UDP training and validation; pair it with
     DeviceCropLoader(..., udp=True) and, for validation, TEST.UDP.
+    teacher_image_size=(w, h): a teacher distilled at its own input size. The item also holds teacher_inv, the inverse of
+    the same crop (same centre, scale, rotation, flip and half-body draw) at that size, and the region covers what both
+    crops read; DeviceCropLoader then crops the teacher's input too. The size must have the student's aspect ratio: the
+    crop matrix scales both axes by the box width, so another aspect would crop another part of the box.
     """
 
-    def __init__(self, base, udp=False):
+    def __init__(self, base, udp=False, teacher_image_size=None):
         self.base = base
         self.udp = bool(udp)
         self.mean, self.std = _normalize_of(base.transform)
         self.image_size = (int(base.image_size[0]), int(base.image_size[1]))
+        self.teacher_image_size = None
+        if teacher_image_size is not None:
+            tw, th = (int(v) for v in teacher_image_size)
+            sw, sh = self.image_size
+            if tw < 1 or th < 1:
+                raise ValueError("RawJointsDataset: teacher_image_size=%r must be positive" % (teacher_image_size,))
+            if tw * sh != sw * th:
+                raise ValueError("RawJointsDataset: teacher_image_size %dx%d has another aspect ratio than the student's "
+                                 "%dx%d: the crop would cover another part of the box" % (tw, th, sw, sh))
+            self.teacher_image_size = (tw, th)
 
     def __len__(self):
         return len(self.base)
@@ -181,10 +195,15 @@ class RawJointsDataset(torch.utils.data.Dataset):
                 flipped = True
                 joints, joints_vis = _flip_joints(joints, joints_vis, img.shape[1], b.flip_pairs)
                 c[0] = img.shape[1] - c[0] - 1
-        trans = (udp_crop_matrix if self.udp else crop_matrix)(c, s, r, b.image_size)
+        matrix = udp_crop_matrix if self.udp else crop_matrix
+        trans = matrix(c, s, r, b.image_size)
         inv = invert_affine(trans)
         img_h, img_w = img.shape[:2]
         x0, y0, x1, y1 = source_window(inv, self.image_size, img_w, img_h)
+        teacher_inv = None
+        if self.teacher_image_size is not None:
+            teacher_inv = invert_affine(matrix(c, s, r, self.teacher_image_size))
+            x0, y0, x1, y1 = _union(source_window(teacher_inv, self.teacher_image_size, img_w, img_h), (x0, y0, x1, y1))
         # one copy: rows, the columns of the mirrored image (reversed when flipped), channels reversed for RGB
         cols = slice(img_w - 1 - x0, img_w - 1 - x1 if x1 < img_w else None, -1) if flipped else slice(x0, x1)
         chans = slice(None, None, -1) if b.color_rgb else slice(None)
@@ -197,8 +216,23 @@ class RawJointsDataset(torch.utils.data.Dataset):
                 'joints': joints, 'joints_vis': joints_vis, 'center': c, 'scale': s, 'rotation': r,
                 'score': rec.get('score', 1)}
         desc = np.array([0, x0, y0, region.shape[1], region.shape[0], img_w, img_h], np.int64)
-        return {'region': region, 'desc': desc, 'inv': inv, 'joints': joints, 'joints_vis': joints_vis,
+        item = {'region': region, 'desc': desc, 'inv': inv, 'joints': joints, 'joints_vis': joints_vis,
                 'out_size': self.image_size, 'mean': self.mean, 'std': self.std, 'meta': meta}
+        if teacher_inv is not None:
+            item.update(teacher_inv=teacher_inv, teacher_out_size=self.teacher_image_size, teacher_udp=self.udp)
+        return item
+
+
+def _union(a, b):
+    """The smallest window (x0, y0, x1, y1) holding windows a and b; an empty window adds nothing. The crop kernel reads
+    each tap relative to the region, so a region grown beyond a crop's own window leaves that crop's pixels unchanged."""
+    def empty(w):
+        return w[2] <= w[0] or w[3] <= w[1]
+    if empty(a):
+        return b
+    if empty(b):
+        return a
+    return min(a[0], b[0]), min(a[1], b[1]), max(a[2], b[2]), max(a[3], b[3])
 
 
 def add_unlabeled_boxes(dataset, bbox_file, image_path=None, score_thre=0.0):
@@ -232,18 +266,23 @@ def raw_collate(items):
     """Batch of RawJointsDataset items -> dict of CPU tensors (pinned by the DataLoader's pin_memory):
     pixels uint8 [total bytes] (the regions back to back), desc int64 [N,7] (column 0 = byte offset), inv float64 [N,6],
     joints / joints_vis float32 [N,J,3], out_size int64 [2] = (w, h), norm float32 [6] = mean, std, and meta collated
-    as default_collate does."""
+    as default_collate does. Items with a teacher crop add teacher_inv float64 [N,6], teacher_out_size int64 [2] and
+    teacher_udp (bool)."""
     from torch.utils.data import default_collate
     first = items[0]
+    teacher = 'teacher_inv' in first
     for it in items[1:]:
         if it['out_size'] != first['out_size'] or not (np.array_equal(it['mean'], first['mean'])
                                                         and np.array_equal(it['std'], first['std'])):
             raise ValueError("raw_collate: samples of one batch need the same output size and normalisation")
+        if ('teacher_inv' in it) != teacher or (teacher and (it['teacher_out_size'] != first['teacher_out_size']
+                                                             or it['teacher_udp'] != first['teacher_udp'])):
+            raise ValueError("raw_collate: samples of one batch need the same teacher crop size and convention")
     sizes = [it['region'].size for it in items]
     desc = np.stack([it['desc'] for it in items])
     desc[:, 0] = np.cumsum([0] + sizes[:-1])
     pixels = np.concatenate([it['region'].reshape(-1) for it in items]) if sum(sizes) else np.zeros(0, np.uint8)
-    return {
+    batch = {
         'pixels': torch.from_numpy(pixels),
         'desc': torch.from_numpy(desc),
         'inv': torch.from_numpy(np.stack([it['inv'].reshape(6) for it in items])),
@@ -253,6 +292,11 @@ def raw_collate(items):
         'norm': torch.from_numpy(np.concatenate([first['mean'], first['std']]).astype(np.float32)),
         'meta': default_collate([it['meta'] for it in items]),
     }
+    if teacher:
+        batch.update(teacher_inv=torch.from_numpy(np.stack([it['teacher_inv'].reshape(6) for it in items])),
+                     teacher_out_size=torch.tensor(first['teacher_out_size'], dtype=torch.int64),
+                     teacher_udp=bool(first['teacher_udp']))
+    return batch
 
 
 class DeviceCropLoader:
@@ -261,7 +305,9 @@ class DeviceCropLoader:
     Per batch: the H2D copies, one crop launch and one TargetGenerator call. heatmap_size = (w, h) and sigma as
     cfg.MODEL.HEATMAP_SIZE / SIGMA; joints_weight as the dataset's when LOSS.USE_DIFFERENT_JOINTS_WEIGHT; unbiased=True
     builds DARK's unbiased targets, udp=True UDP's targets for a RawJointsDataset(udp=True) loader (TargetGenerator;
-    not both)."""
+    not both). A batch of a RawJointsDataset(teacher_image_size=...) gets a second crop launch over the same pixels at
+    the teacher's size and normalisation: meta['teacher_input'] (device [N,3,Ht,Wt]) and meta['teacher_udp'] (the
+    dataset's udp), which fpd_train hands to the teacher."""
 
     def __init__(self, loader, heatmap_size, sigma, joints_weight=None, device=None, unbiased=False, udp=False):
         if unbiased and udp:
@@ -284,8 +330,8 @@ class DeviceCropLoader:
 
     def to_device(self, batch):
         """The batch's tensors (not meta) copied to the device, asynchronously from pinned memory."""
-        return {k: batch[k].to(self.device, non_blocking=True)
-                for k in ('pixels', 'desc', 'inv', 'joints', 'joints_vis')}
+        keys = ('pixels', 'desc', 'inv', 'joints', 'joints_vis') + (('teacher_inv',) if 'teacher_inv' in batch else ())
+        return {k: batch[k].to(self.device, non_blocking=True) for k in keys}
 
     def device_step(self, dev, batch):
         """(input, target, target_weight) from the device tensors of to_device(batch); enqueues only device work (it can
@@ -301,6 +347,19 @@ class DeviceCropLoader:
         target, target_weight = gen(dev['joints'], dev['joints_vis'])
         return inp, target, target_weight
 
+    def teacher_crop(self, dev, batch):
+        """The teacher's input [N,3,Ht,Wt] from the device tensors of to_device(batch): the student's region and
+        normalisation through the teacher's inverse matrices."""
+        norm = batch['norm'].numpy()
+        return ops.crop_affine_normalize(dev['pixels'], dev['desc'], dev['teacher_inv'],
+                                         tuple(int(v) for v in batch['teacher_out_size']), norm[:3], norm[3:],
+                                         desc_host=batch['desc'], inv_host=batch['teacher_inv'])
+
     def process(self, batch):
-        inp, target, target_weight = self.device_step(self.to_device(batch), batch)
-        return inp, target, target_weight, batch['meta']
+        dev = self.to_device(batch)
+        inp, target, target_weight = self.device_step(dev, batch)
+        meta = batch['meta']
+        if 'teacher_inv' in batch:
+            meta['teacher_input'] = self.teacher_crop(dev, batch)
+            meta['teacher_udp'] = batch['teacher_udp']
+        return inp, target, target_weight, meta

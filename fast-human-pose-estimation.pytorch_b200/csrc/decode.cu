@@ -14,6 +14,7 @@
 // the results are bit-identical to lib/core/inference.py::get_final_preds and lib/core/evaluate.py::accuracy.
 // final_preds_dark is the opt-in alternative to the quarter-pixel nudge: DARK's Taylor step on the log of the blurred
 // map (Zhang et al., "Distribution-Aware Coordinate Representation for Human Pose Estimation", CVPR 2020).
+// heatmap_resample carries a teacher's heat-maps from its own crop size onto the student's heat-map grid.
 #include "common.cuh"
 
 namespace fpd {
@@ -317,6 +318,35 @@ __global__ void pck_counts_kernel(const int* __restrict__ idx, const float* __re
   if (d < 0.5) atomicAdd(counts + j * 2 + 1, 1);
 }
 
+// (1 - f) a + f b with explicit roundings; f == 0 returns a itself (an equal-size resample is an exact copy even next to
+// an infinite or NaN neighbour)
+__device__ __forceinline__ float lerp_rn(float a, float b, float f) {
+  return f == 0.f ? a : __fadd_rn(__fmul_rn(__fsub_rn(1.f, f), a), __fmul_rn(f, b));
+}
+
+// heatmap_resample: one thread per output element of an NHWC map; the source position is one fp32 multiply of the
+// output pixel index by the host's ratio, clamped to the input (replicate edge), then bilinear
+__global__ void heatmap_resample_kernel(const float* __restrict__ in, float* __restrict__ out, int Hi, int Wi, int Ho,
+                                        int Wo, int C, float ry, float rx, int64_t total) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= total) return;
+  const int c = (int)(t % C);
+  const int64_t p = t / C;
+  const int u = (int)(p % Wo);
+  const int64_t q = p / Wo;
+  const int v = (int)(q % Ho);
+  const int64_t b = q / Ho;
+  const float x = fminf(fmaxf(__fmul_rn((float)u, rx), 0.f), (float)(Wi - 1));
+  const float y = fminf(fmaxf(__fmul_rn((float)v, ry), 0.f), (float)(Hi - 1));
+  const int x0 = (int)x, y0 = (int)y;
+  const int x1 = min(x0 + 1, Wi - 1), y1 = min(y0 + 1, Hi - 1);
+  const float fx = __fsub_rn(x, (float)x0), fy = __fsub_rn(y, (float)y0);
+  const float* m = in + b * Hi * Wi * C + c;
+  const float top = lerp_rn(__ldg(m + ((int64_t)y0 * Wi + x0) * C), __ldg(m + ((int64_t)y0 * Wi + x1) * C), fx);
+  const float bot = lerp_rn(__ldg(m + ((int64_t)y1 * Wi + x0) * C), __ldg(m + ((int64_t)y1 * Wi + x1) * C), fx);
+  out[t] = lerp_rn(top, bot, fy);
+}
+
 }  // namespace
 }  // namespace fpd
 
@@ -386,6 +416,24 @@ int fpd_pck_counts(const int* idx, const float* maxval, const float* target_nchw
   const int BJ = B * J, threads = 256;
   pck_counts_kernel<<<(BJ * 32 + threads - 1) / threads, threads, 0, stream>>>(idx, maxval, target_nchw, counts, pred_hm,
                                                                               BJ, J, h, w);
+  FPD_LAUNCH_CHECK();
+  return FPD_OK;
+}
+
+int fpd_heatmap_resample(const float* in, float* out, int B, int Hi, int Wi, int Ho, int Wo, int C, int udp,
+                         fpd_stream_t stream) {
+  FPD_REQUIRE(B >= 0 && C >= 1 && C <= 64, "heatmap_resample: B=%d C=%d out of range", B, C);
+  FPD_REQUIRE(Hi >= 1 && Wi >= 1 && Ho >= 1 && Wo >= 1, "heatmap_resample: empty map %dx%d -> %dx%d", Hi, Wi, Ho, Wo);
+  FPD_REQUIRE(in && out, "heatmap_resample: null pointer");
+  if (B == 0) return FPD_OK;
+  // reference crops: output pixel u is the box fraction u / Wo, so u_in = u * Wi / Wo; UDP crops measure sizes in pixel
+  // spacings, so u_in = u * (Wi - 1) / (Wo - 1). The ratio is rounded to fp32 once, here.
+  const float rx = udp ? (Wo > 1 ? (float)((double)(Wi - 1) / (Wo - 1)) : 0.f) : (float)((double)Wi / Wo);
+  const float ry = udp ? (Ho > 1 ? (float)((double)(Hi - 1) / (Ho - 1)) : 0.f) : (float)((double)Hi / Ho);
+  const int64_t total = (int64_t)B * Ho * Wo * C;
+  const int threads = 256;
+  heatmap_resample_kernel<<<(unsigned)((total + threads - 1) / threads), threads, 0, stream>>>(in, out, Hi, Wi, Ho, Wo, C,
+                                                                                              ry, rx, total);
   FPD_LAUNCH_CHECK();
   return FPD_OK;
 }

@@ -20,6 +20,9 @@ What changes underneath:
     add_unlabeled_boxes) are distilled from the teacher's confident joints (_kd_unlabeled_thre), on every route.
   * fpd_train with config.KD.FEATURE_WEIGHT > 0 and feature_adapter=: feature distillation from the teacher's head
     feature (train_step.FeatureAdapter, ops.feature_mse) on the graph and the eager fused route; logged as FEAT_Loss.
+  * fpd_train with a teacher input of its own size (meta['teacher_input'] from augment.DeviceCropLoader over a
+    RawJointsDataset(teacher_image_size=...)): the teacher reads its own crop and its last heat-map is resampled onto the
+    student's grid (ops.resample_heatmaps) before the loss, on every route. train and validate ignore it.
   * validate: for the fpd_b200 models with JointsMSELoss, JointsOHKMMSELoss or JointsKLDLoss, each batch is one CUDA graph replay (infer_step.
     FlipTestInference with its decode stage: both forwards, flip merge, loss, keypoints, PCK counts); the results are
     copied to pinned host buffers asynchronously and the host waits only to log and at the end of the epoch.
@@ -117,30 +120,42 @@ def _kd_weights_torch(toutput, target_weight, thre):
     return torch.where(unlabeled, confident, tw).reshape(target_weight.shape)
 
 
+def _teacher_input(meta):
+    """(teacher input or None, its crop convention udp) from a batch's meta: DeviceCropLoader's meta['teacher_input'] and
+    meta['teacher_udp'] when the dataset crops a teacher input of its own size."""
+    if isinstance(meta, dict) and meta.get('teacher_input') is not None:
+        return meta['teacher_input'], bool(meta.get('teacher_udp', False))
+    return None, False
+
+
 def _fused_step(model, tmodel, input, target, target_weight, alpha, use_tw, graph=None, kd_unlabeled_thre=None,
-                feature_weight=0.0, feature_adapter=None, **terms):
+                feature_weight=0.0, feature_adapter=None, teacher_input=None, teacher_udp=False, **terms):
     """student fwd -> teacher fwd -> fused loss+grad -> backward tape; returns (losses[3] dev, last output NHWC).
     terms: the criteria's _criterion_term selectors. graph: a _GraphTraining whose batch shape this batch has -- the
     same step is then one replay of its graph, and the last output is None (the PCK counts come out of the graph
     instead). kd_unlabeled_thre: the kd term is weighted by ops.kd_weights (distillation from unlabeled samples).
     feature_weight > 0: feature distillation through feature_adapter; the losses are then [4] (pose, kd, total,
-    feature) and the adapter's parameters get their .grad too."""
+    feature) and the adapter's parameters get their .grad too. teacher_input: the teacher's own crop of the batch; its
+    last map is resampled onto the target's grid (teacher_udp: the crops' convention), kd_weights reads its own map."""
     if graph is not None:
-        return graph.step(input, target, target_weight), None
+        return graph.step(input, target, target_weight, teacher_input), None
     from fpd_b200 import ops
     net = _unwrap(model)
     x = input.cuda(non_blocking=True).float().contiguous()
     eng = net.engine()
     ctx = eng.forward(x, True, record_tape=True)
     outs = [v.data for v in ctx.outs]
-    t_last = t_ctx = None
+    t_last = t_native = t_ctx = None
     if tmodel is not None:
-        t_ctx = _unwrap(tmodel).engine().forward(x, False, record_tape=False)
-        t_last = t_ctx.outs[-1].data
+        tx = x if teacher_input is None else teacher_input.cuda(non_blocking=True).float().contiguous()
+        t_ctx = _unwrap(tmodel).engine().forward(tx, False, record_tape=False)
+        t_last = t_native = t_ctx.outs[-1].data
+        if teacher_input is not None:
+            t_last = ops.resample_heatmaps(t_native, target.shape[2:], udp=teacher_udp)
     B, _, _, J = outs[0].shape
     tw = (target_weight.reshape(B, J) if use_tw else torch.ones(B, J, device=x.device)).contiguous().float()
     if kd_unlabeled_thre is not None:
-        terms["kd_weight"] = ops.kd_weights(t_last, tw, kd_unlabeled_thre)
+        terms["kd_weight"] = ops.kd_weights(t_native, tw, kd_unlabeled_thre)
     losses4 = None
     if feature_weight:
         losses4 = torch.zeros(4, dtype=torch.float32, device=x.device)
@@ -213,19 +228,24 @@ class _GraphTraining:
     meter updates in batch order. terms: the criteria's _criterion_term selectors."""
 
     def __init__(self, model, tmodel, alpha, use_tw, terms, input, target, target_weight, num_batches,
-                 kd_unlabeled_thre=None, feature_weight=0.0, feature_adapter=None):
+                 kd_unlabeled_thre=None, feature_weight=0.0, feature_adapter=None, teacher_input=None, teacher_udp=False):
         from fpd_b200.train_step import FPDTrainStep
         net = _unwrap(model)
         tnet = _unwrap(tmodel) if tmodel is not None else None
-        self.shapes = (tuple(input.shape), tuple(target.shape), tuple(target_weight.shape))
+        self.shapes = (tuple(input.shape), tuple(target.shape), tuple(target_weight.shape),
+                       None if teacher_input is None else tuple(teacher_input.shape))
         alpha = float(alpha) if tnet is not None else 0.0
         key = (id(net), id(tnet), self.shapes, alpha, tuple(sorted(terms.items())), kd_unlabeled_thre)
+        if teacher_input is not None:
+            key += (bool(teacher_udp),)
         if feature_weight:
             key += (feature_weight, id(feature_adapter))
         step = _train_step_cache.get(key)
         if step is None:
             _train_step_cache.clear()          # one graph pool at a time
             extra = {} if kd_unlabeled_thre is None else {"kd_unlabeled_thre": kd_unlabeled_thre}
+            if teacher_input is not None:
+                extra["teacher_input_udp"] = bool(teacher_udp)
             if feature_weight:
                 extra.update(feature_weight=feature_weight, feature_adapter=feature_adapter)
             step = _train_step_cache[key] = FPDTrainStep(net, tnet, alpha=alpha, fused_adam=False, accuracy=True,
@@ -240,13 +260,16 @@ class _GraphTraining:
         self.done = torch.cuda.Event()
         self.pending = []          # (batch, num_images) not yet applied to the meters
 
-    def accepts(self, input, target, target_weight):
-        return (tuple(input.shape), tuple(target.shape), tuple(target_weight.shape)) == self.shapes
+    def accepts(self, input, target, target_weight, teacher_input=None, teacher_udp=False):
+        return ((tuple(input.shape), tuple(target.shape), tuple(target_weight.shape),
+                 None if teacher_input is None else tuple(teacher_input.shape)) == self.shapes
+                and (teacher_input is None or bool(teacher_udp) == self.train_step.teacher_input_udp))
 
-    def step(self, input, target, target_weight):
+    def step(self, input, target, target_weight, teacher_input=None):
         """Replay (gradients all-reduced when there are several ranks) and hand the gradients to the parameters'
         .grad, as _fused_step does; returns the device losses[3] (with feature distillation losses[4])."""
-        l3 = self.train_step.step(input, target, target_weight if self.ones is None else self.ones)
+        l3 = self.train_step.step(input, target, target_weight if self.ones is None else self.ones,
+                                  teacher_x=teacher_input)
         for p, g in self.trainable:     # frozen parameters keep whatever .grad they had
             p.grad = g
         return self.train_step.losses_feature if self.feature else l3
@@ -393,7 +416,11 @@ def fpd_train(config, train_loader, model, tmodel, pose_criterion, kd_pose_crite
     confident joints (last-stack map maximum > KD.UNLABELED_THRE) instead; both criteria need use_target_weight.
     With config.KD.FEATURE_WEIGHT = w > 0, loss += w * mean((A(s) - t)^2), s and t the student's and the teacher's head
     features and A feature_adapter (train_step.FeatureAdapter, whose parameters the optimizer must hold); fused routes
-    only."""
+    only.
+    A batch whose meta holds 'teacher_input' (DeviceCropLoader over RawJointsDataset(teacher_image_size=...)) runs the
+    teacher on that input, at the teacher's own size, and resamples its last heat-map onto the target's grid
+    (ops.resample_heatmaps; meta['teacher_udp'] gives the crops' convention) before the kd term. KD.UNLABELED then reads
+    the teacher's own map. Not together with KD.FEATURE_WEIGHT."""
     kd_thre = _kd_unlabeled_thre(config)
     if kd_thre is not None:
         if tmodel is None:
@@ -446,6 +473,11 @@ def fpd_train(config, train_loader, model, tmodel, pose_criterion, kd_pose_crite
         data_time.update(time.time() - end)
         target = target.cuda(non_blocking=True)
         target_weight = target_weight.cuda(non_blocking=True)
+        t_input, t_udp = _teacher_input(meta)
+        tin = {} if t_input is None else {"teacher_input": t_input, "teacher_udp": t_udp}
+        if feat_w and t_input is not None:
+            raise ValueError("KD.FEATURE_WEIGHT does not run with a teacher input of its own size (meta['teacher_input']): "
+                             "the teacher's head feature would have other spatial sizes than the student's")
         if fused and not shape_checked:
             route = _train_route(config, model, tmodel, [pose_criterion, kd_pose_criterion], target.shape)
             fused = route != "generic"
@@ -456,14 +488,14 @@ def fpd_train(config, train_loader, model, tmodel, pose_criterion, kd_pose_crite
                                                                             target.shape[1]))
             if route == "graph":
                 graph = _GraphTraining(model, tmodel, alpha, pose_criterion.use_target_weight, terms, input, target,
-                                       target_weight, len(train_loader), **unl, **feat)
-        replay = graph if graph is not None and graph.accepts(input, target, target_weight) else None
+                                       target_weight, len(train_loader), **unl, **feat, **tin)
+        replay = graph if graph is not None and graph.accepts(input, target, target_weight, **tin) else None
         if graph is not None and replay is None:
             graph.flush(apply)          # meter updates stay in batch order
         if fused:
             optimizer.zero_grad()
             l3, out_nhwc = _fused_step(model, tmodel, input, target, target_weight, alpha,
-                                       pose_criterion.use_target_weight, replay, **terms, **unl, **feat)
+                                       pose_criterion.use_target_weight, replay, **terms, **unl, **feat, **tin)
             optimizer.step()
             if replay is not None:
                 replay.record(i, l3, input.size(0))
@@ -483,11 +515,15 @@ def fpd_train(config, train_loader, model, tmodel, pose_criterion, kd_pose_crite
         else:
             outputs = model(input)
             with torch.no_grad():  # the teacher's gradients never reach the student update
-                toutput = tmodel(input)
+                toutput = tmodel(input if t_input is None else t_input)
             if isinstance(toutput, list):
                 toutput = toutput[-1]
             outs = outputs if isinstance(outputs, list) else [outputs]
             kd_weight = target_weight if kd_thre is None else _kd_weights_torch(toutput, target_weight, kd_thre)
+            if t_input is not None:
+                from fpd_b200 import ops
+                t_nhwc = toutput.detach().float().permute(0, 2, 3, 1).contiguous()
+                toutput = ops.resample_heatmaps(t_nhwc, target.shape[2:], udp=t_udp).permute(0, 3, 1, 2).contiguous()
             pose_loss = pose_criterion(outs[0], target, target_weight)
             kd_pose_loss = kd_pose_criterion(outs[0], toutput, kd_weight)
             for output in outs[1:]:

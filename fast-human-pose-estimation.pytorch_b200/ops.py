@@ -985,6 +985,29 @@ def flip_merge_argmax(hm_nhwc, hm_flip_nhwc=None, flip_perm=None, shift=False, w
     return avg, idx, maxval
 
 
+def resample_heatmaps(hm_nhwc, out_hw, udp=False, out=None):
+    """A teacher's heat-maps [B,Hi,Wi,C] (fp32 NHWC, C <= 64) on the heat-map grid out_hw = (h, w) of another crop of the
+    same box (fpd_heatmap_resample): bilinear at (u * Wi / Wo, v * Hi / Ho) for the reference's crops, at
+    (u * (Wi-1) / (Wo-1), v * (Hi-1) / (Ho-1)) for UDP crops (udp=True), clamped to the map. Returns [B,h,w,C]."""
+    _chk(hm_nhwc, "hm_nhwc")
+    if hm_nhwc.dim() != 4:
+        raise ValueError("resample_heatmaps: hm_nhwc must be [B, H, W, C], got %s" % (tuple(hm_nhwc.shape),))
+    B, Hi, Wi, C = hm_nhwc.shape
+    Ho, Wo = int(out_hw[0]), int(out_hw[1])
+    if min(Hi, Wi, Ho, Wo) < 1 or not 1 <= C <= 64:
+        raise ValueError("resample_heatmaps: sizes must be positive and C <= 64 (got [%d,%d,%d,%d] -> %dx%d)"
+                         % (B, Hi, Wi, C, Ho, Wo))
+    if out is None:
+        out = torch.empty((B, Ho, Wo, C), dtype=torch.float32, device=hm_nhwc.device)
+    else:
+        _chk(out, "out")
+        if tuple(out.shape) != (B, Ho, Wo, C):
+            raise ValueError("resample_heatmaps: out must be %s" % ((B, Ho, Wo, C),))
+    N.check(N.lib().fpd_heatmap_resample(_p(hm_nhwc), _p(out), B, Hi, Wi, Ho, Wo, C, int(bool(udp)), _stream()),
+            "heatmap_resample")
+    return out
+
+
 def argmax_nchw(hm):
     B, J = hm.shape[:2]
     hw = hm.numel() // (B * J)

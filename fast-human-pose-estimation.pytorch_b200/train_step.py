@@ -14,7 +14,9 @@ optimizer (any torch.optim optimizer, its state dict, LR schedules) steps on the
 buffer -- lib/core/function.py's train / fpd_train run this way. pose_topk / kd_topk select JointsOHKMMSELoss for a term,
 pose_temperature / kd_temperature JointsKLDLoss; accuracy=True adds accuracy()'s PCK counts of the last stack to the graph;
 kd_unlabeled_thre distils from unlabeled samples (ops.kd_weights weights the kd term, inside the graph); feature_weight with
-a FeatureAdapter adds feature distillation, a hint from the teacher's head feature (ops.feature_mse).
+a FeatureAdapter adds feature distillation, a hint from the teacher's head feature (ops.feature_mse). step(..., teacher_x=)
+distils from a teacher at its own input size: the teacher reads its own crop of the batch and its heat-maps are resampled
+onto the student's heat-map grid (ops.resample_heatmaps).
 
 The teacher is forward-only (its gradients never influence the student update; the reference's teacher
 backward is wasted work). `plain=True` drops the teacher (function.train semantics,
@@ -134,7 +136,7 @@ class FPDTrainStep:
     def __init__(self, student, teacher=None, alpha=0.5, lr=2.5e-4, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0,
                  process_group=None, use_graph=True, pose_topk=0, kd_topk=0, fused_adam=True, accuracy=False,
                  pose_temperature=0.0, kd_temperature=0.0, kd_unlabeled_thre=None, feature_weight=0.0,
-                 feature_adapter=None):
+                 feature_adapter=None, teacher_input_udp=False):
         """pose_topk / kd_topk: > 0 makes that loss term JointsOHKMMSELoss(topk) instead of JointsMSELoss.
         pose_temperature / kd_temperature: > 0 makes that term JointsKLDLoss(temperature) (not together with a topk).
         fused_adam=False (external-optimizer mode): step() stops once the gradients are in the flat gradient buffer
@@ -149,7 +151,9 @@ class FPDTrainStep:
         head feature s to the teacher's width, and total += feature_weight * mean((A(s) - t)^2) over every element of
         every sample, labeled or not (ops.feature_mse; not scaled by alpha). The adapter's parameters follow the
         student's in the flat buffers (params, grad_views, fused Adam, state_dict); `feature_loss` is the device scalar
-        mean((A(s) - t)^2) of the latest step. Hourglass and HRNet networks only; not with FPD_PIPELINE_TEACHER."""
+        mean((A(s) - t)^2) of the latest step. Hourglass and HRNet networks only; not with FPD_PIPELINE_TEACHER.
+        teacher_input_udp: the crop convention of the teacher inputs step(..., teacher_x=) is given (False: the reference's
+        crop_matrix, True: udp_crop_matrix); it picks how teacher heat-map pixels map onto the student's."""
         pose_topk, kd_topk = _check_topk(pose_topk, "pose_topk"), _check_topk(kd_topk, "kd_topk")
         if kd_topk and teacher is None:
             raise ValueError("kd_topk=%d needs a teacher" % kd_topk)
@@ -164,6 +168,7 @@ class FPDTrainStep:
             if teacher is None:
                 raise ValueError("kd_unlabeled_thre=%r needs a teacher" % kd_unlabeled_thre)
         self.kd_unlabeled_thre = kd_unlabeled_thre
+        self.teacher_input_udp = bool(teacher_input_udp)
         self.feature_weight = check_feature_kd(student, teacher, feature_weight, feature_adapter)
         self.adapter = feature_adapter if self.feature_weight else None
         self.feature_loss = None
@@ -196,6 +201,7 @@ class FPDTrainStep:
             raise ValueError("feature distillation needs the teacher's head feature of the same batch: it does not run "
                              "with the teacher pipelined (FPD_PIPELINE_TEACHER)")
         self.x_next = self.t_cur = self.t_next = None
+        self.static_tx = None       # the graph's teacher input, when the teacher reads its own crop
         self._have_next = False
         self._static_shapes = None
         self._static_ptrs = None
@@ -247,34 +253,45 @@ class FPDTrainStep:
                 dsts.append(gv)
         torch._foreach_copy_(dsts, srcs)
 
-    def _body(self, x, target, tw):
+    def _teacher_last(self, t_ctx, tx, target):
+        """(the map the loss distils from, the teacher's own last-stack map). With a teacher input of its own size (tx) the
+        former is the latter resampled onto the target's heat-map grid."""
+        t_native = t_ctx.outs[-1].data
+        if tx is None:
+            return t_native, t_native
+        return ops.resample_heatmaps(t_native, target.shape[2:], udp=self.teacher_input_udp), t_native
+
+    def _body(self, x, target, tw, tx=None):
+        """tx: the teacher's own input (its crop of the batch at its input size), or None: the teacher reads x."""
         s_eng = self.student.engine()
-        t_last = None
+        t_last = t_native = None
+        t_in = x if tx is None else tx
         if self.teacher is not None and self.overlap_teacher:
             # the frozen teacher's forward is independent of the student's: run it on a second stream so its many
             # small-grid kernels (low-resolution hourglass levels) fill SMs the student leaves idle. It uses no shared
             # workspace (eval-mode BN: no statistics passes), so the two streams touch disjoint memory.
             # Both networks start from the same image: the NHWC conversion and the 7x7-stem im2col columns (335 MB at
             # B=32) are built once, on the main stream, before the fork.
+            # (a teacher input of its own size shares nothing with the student's)
             main = torch.cuda.current_stream()
-            stem = {} if SHARE_STEM else None
+            stem = {} if SHARE_STEM and tx is None else None
             if stem is not None:
                 s_eng.prepare_stem(x, stem)
             self._side.wait_stream(main)
             with torch.cuda.stream(self._side):
-                t_ctx = self.teacher.engine().forward(x, False, record_tape=False, shared_stem=stem)
+                t_ctx = self.teacher.engine().forward(t_in, False, record_tape=False, shared_stem=stem)
                 self._t_keep = t_ctx            # keep every teacher tensor alive until the streams have joined
-                t_last = t_ctx.outs[-1].data
+                t_last, t_native = self._teacher_last(t_ctx, tx, target)
             ctx = s_eng.forward(x, True, record_tape=True, shared_stem=stem)
             main.wait_stream(self._side)
         else:
             ctx = s_eng.forward(x, True, record_tape=True)
             if self.teacher is not None:
-                t_ctx = self.teacher.engine().forward(x, False, record_tape=False)
-                t_last = t_ctx.outs[-1].data
+                t_ctx = self.teacher.engine().forward(t_in, False, record_tape=False)
+                t_last, t_native = self._teacher_last(t_ctx, tx, target)
         outs = [v.data for v in ctx.outs]
         self.last_outs, self.last_teacher = outs, t_last
-        losses, grads = self._loss(outs, target, t_last, tw)
+        losses, grads = self._loss(outs, target, t_last, tw, t_native)
         if self.feature_weight:
             self._feature_term(s_eng, ctx, t_ctx, losses)
         pg = s_eng.backward(ctx, grads, wgrad_stream=self._wstream)
@@ -289,11 +306,13 @@ class FPDTrainStep:
                                losses=losses)
         a.add_grad(g, owned=False)
 
-    def _loss(self, outs, target, t_last, tw):
-        """The fused FPD loss and its gradients (+ the PCK counts of the last stack when accuracy=True)."""
+    def _loss(self, outs, target, t_last, tw, t_native=None):
+        """The fused FPD loss and its gradients (+ the PCK counts of the last stack when accuracy=True). t_native: the
+        teacher's map at its own size, when t_last was resampled from it."""
         if self.kd_unlabeled_thre is not None:
-            # the teacher's stream has joined by now: t_last is complete
-            kdw = ops.kd_weights(t_last, tw, self.kd_unlabeled_thre)
+            # the teacher's stream has joined by now: t_last is complete. A joint's confidence is the maximum of the
+            # teacher's own map, as in the reference's rule: bilinear resampling would lower it.
+            kdw = ops.kd_weights(t_last if t_native is None else t_native, tw, self.kd_unlabeled_thre)
             losses, grads = ops.fpd_loss(outs, target, t_last, tw, self.alpha, losses_out=self.losses,
                                          pose_topk=self.pose_topk, kd_topk=self.kd_topk,
                                          pose_temperature=self.pose_temperature, kd_temperature=self.kd_temperature,
@@ -326,12 +345,13 @@ class FPDTrainStep:
     def _run_body(self):
         if self.pipeline:
             return self._body_pipelined(self.static[0], self.static[1], self.static[2], self.x_next)
-        return self._body(*self.static)
+        return self._body(*self.static, tx=self.static_tx)
 
-    def _capture(self, x, target, tw):
+    def _capture(self, x, target, tw, tx=None):
         self.static = (torch.empty_like(x), torch.empty_like(target), torch.empty_like(tw))
         for s, v in zip(self.static, (x, target, tw)):
             s.copy_(v)
+        self.static_tx = None if tx is None else tx.clone()
         self._outputs(target)
         if self.pipeline:
             self.x_next = x.clone()
@@ -363,7 +383,7 @@ class FPDTrainStep:
             b.copy_(s)
 
     # ------------------------------------------------------------------ public
-    def step(self, x, target, target_weight, next_x=None):
+    def step(self, x, target, target_weight, next_x=None, teacher_x=None):
         """x [B,3,H,W], target [B,J,h,w], target_weight [B,J,1] -- CUDA or pinned-host tensors.
         Returns the device tensor losses[3] = (pose, kd, total); no host synchronisation.
         `next_x` (optional): the NEXT step's images as a pinned host tensor -- their H2D copy then runs on a copy stream
@@ -372,10 +392,17 @@ class FPDTrainStep:
         hand anyway): the teacher runs on them while the student trains on `x`, and the following call must pass that
         same batch as `x`. Without `next_x` the teacher for the following step is run up front (no overlap).
         With fused_adam=False the step ends with the gradients in `grad_views` (mean over ranks); the caller's optimizer
-        does the update."""
+        does the update.
+        `teacher_x` (optional): the teacher's own input [B,3,Ht,Wt], the same boxes cropped at the teacher's input size
+        (DeviceCropLoader's meta['teacher_input']). The teacher reads it instead of `x`, and its last-stack map is resampled
+        onto the target's grid (ops.resample_heatmaps, in the constructor's teacher_input_udp convention) before every loss
+        term; kd_unlabeled_thre still reads the teacher's own map. Not with feature distillation or teacher pipelining."""
         tw = target_weight.reshape(target_weight.shape[0], -1)
+        if teacher_x is not None:
+            self._check_teacher_x(x, teacher_x)
         if self.use_graph:
-            shapes = (tuple(x.shape), tuple(target.shape), tuple(tw.shape))
+            shapes = (tuple(x.shape), tuple(target.shape), tuple(tw.shape),
+                      None if teacher_x is None else (tuple(teacher_x.shape), self.teacher_input_udp))
             t_gen = self.teacher.engine().generation if self.teacher is not None else 0
             s_prec = self.student.engine().training_precision
             # fused-Adam mode owns the parameters' storage (FlatParams); otherwise the caller may give them new storage
@@ -389,7 +416,8 @@ class FPDTrainStep:
                 self.graph = None
             if self.graph is None:
                 xd, td, wd = (t.cuda(non_blocking=True).float().contiguous() for t in (x, target, tw))
-                self._capture(xd, td, wd)
+                txd = None if teacher_x is None else teacher_x.cuda(non_blocking=True).float().contiguous()
+                self._capture(xd, td, wd, txd)
                 self._static_shapes = shapes
                 self._static_ptrs = ptrs
                 self._student_prec = s_prec
@@ -412,6 +440,8 @@ class FPDTrainStep:
                 self._have_next = next_x is not None
             else:
                 self._stage_inputs(x, target, tw)
+                if teacher_x is not None:
+                    self.static_tx.copy_(teacher_x, non_blocking=True)
             self.graph.replay()
             if not self.pipeline:
                 self._prefetch(next_x)
@@ -420,8 +450,9 @@ class FPDTrainStep:
             xd, td, wd = (t.cuda(non_blocking=True).float().contiguous() for t in (x, target, tw))
             if self.losses is None or (self.want_accuracy and self.counts.shape[0] != td.shape[1]):
                 self._outputs(td)
+            txd = None if teacher_x is None else teacher_x.cuda(non_blocking=True).float().contiguous()
             n0 = N.lib().fpd_launch_count()
-            losses = self._body(xd, td, wd)
+            losses = self._body(xd, td, wd, txd)
             self.launches_per_step = int(N.lib().fpd_launch_count() - n0) + int(self.fused_adam)
         if self.fused_adam:
             gscale = 1.0
@@ -440,6 +471,19 @@ class FPDTrainStep:
         # Python): drop the student's cached eval-mode operands so a following validation sees the new values
         self.student.engine().invalidate_eval_cache()
         return losses
+
+    def _check_teacher_x(self, x, teacher_x):
+        if self.teacher is None:
+            raise ValueError("teacher_x needs a teacher")
+        if self.feature_weight:
+            raise ValueError("feature distillation does not run with a teacher input of its own size: the teacher's head "
+                             "feature would have other spatial sizes than the student's")
+        if self.pipeline:
+            raise ValueError("teacher_x does not run with the teacher pipelined (FPD_PIPELINE_TEACHER), which runs the "
+                             "teacher on next_x")
+        if teacher_x.dim() != 4 or teacher_x.shape[0] != x.shape[0] or teacher_x.shape[1] != x.shape[1]:
+            raise ValueError("teacher_x %s must be [B, %d, Ht, Wt] with x's batch B = %d" % (
+                tuple(teacher_x.shape), x.shape[1], x.shape[0]))
 
     @property
     def params(self):

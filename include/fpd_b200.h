@@ -417,6 +417,13 @@ int fpd_final_preds(const float* avg_nhwc, const int* idx, const float* maxval, 
  * preds[..., 2] = maxval. Deterministic: no atomics. */
 int fpd_final_preds_dark(const float* avg_nhwc, const int* idx, const float* maxval, const double* inv, int blur_kernel,
                          float* preds, int B, int J, int h, int w, fpd_stream_t stream);
+/* Heat-maps of one crop size onto the heat-map grid of another crop of the same box (a teacher distilled at its own
+ * input size): in NHWC [B,Hi,Wi,C] -> out NHWC [B,Ho,Wo,C], fp32, C <= 64. Output pixel (u, v) samples the input
+ * bilinearly at (u * rx, v * ry), clamped to [0, Wi-1] x [0, Hi-1] (replicate edge); the ratios are rounded to fp32 once
+ * on the host and the position is one fp32 multiply: rx = Wi / Wo for the reference's crops (udp = 0), rx = (Wi - 1) /
+ * (Wo - 1) for UDP crops (udp = 1), the same for y. Equal sizes copy exactly. No allocation, no synchronisation. */
+int fpd_heatmap_resample(const float* in, float* out, int B, int Hi, int Wi, int Ho, int Wo, int C, int udp,
+                         fpd_stream_t stream);
 /* accuracy(), lib/core/evaluate.py:16-71, as per-joint counts: the arg-max of each target map target_nchw [B,J,h,w]
  * against the prediction's idx / maxval [B,J]. counts: device int32[J,2] = {joints whose target lies at x > 1 and
  * y > 1, those of them within 0.5 of the target after normalising x by h/10 and y by w/10}; zeroed by the call.
